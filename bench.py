@@ -4,6 +4,7 @@ MinkUNet34C forward+backward(+SGD) over synthetic 100k-voxel clouds, batch 8 per
 reporting active-voxels/s.  Contract: see the one JSON line printed by rank 0.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config cfgN]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 
 --config selects the BASELINE.json configuration the line is measured on:
@@ -20,6 +21,9 @@ starts from host buffers and rebuilds every map.
   value : inputs already resident in HBM when the timed region starts
   e2e   : the same step driven through the public API from PINNED HOST buffers — H2D copy of
           coordinates/features/labels and a D2H read of the loss inside the timed region
+--dump-outputs DIR writes what the last timed step computed (rank 0) as DIR/<name>.npy, float32 or
+float64, at most 64 MB in all (seeded row / element samples of the large arrays).  The inputs and
+the seeded weights depend only on the arguments, so two builds can be compared output for output.
 --impl reference times the reference's own CPU implementation (oracle/_ref, compiled from
 the reference sources by oracle/build_ref.py) on the host cores, on a bounded sample.
 """
@@ -41,18 +45,18 @@ FLOP_PER_VOXEL_FWD_BWD = 601.6e9 / 100_000
 
 CONFIGS = {
     "cfg3": dict(kind="net", model="MinkUNet34C", clouds=8, voxels=100_000,
-                 metric="active-voxels/sec MinkUNet34C fwd+bwd @100k pts, 1/2/4/8 B200 vs CPU ref",
+                 metric="active-voxels/sec MinkUNet34C fwd+bwd @100k pts, 1/2/4/8 H100 vs CPU ref",
                  what="BASELINE configs[3]"),
     "cfg2": dict(kind="net", model="MinkUNet14", clouds=1, voxels=50_000,
-                 metric="active-voxels/sec MinkUNet14 fwd+bwd @50k pts, 1xB200 vs CPU ref",
+                 metric="active-voxels/sec MinkUNet14 fwd+bwd @50k pts, 1xH100 vs CPU ref",
                  what="BASELINE configs[2]"),
     "cfg1": dict(kind="conv", D=3, voxels=100_000, c_in=64, c_out=128, ks=3, stride=2,
                  metric="active-voxels/sec single MinkowskiConvolution k3 s2 64->128 bf16 "
-                        "fwd+bwd @100k coords, 1xB200 vs CPU ref",
+                        "fwd+bwd @100k coords, 1xH100 vs CPU ref",
                  what="BASELINE configs[1]"),
     "cfg4": dict(kind="conv", D=4, voxels=200_000, c_in=32, c_out=32, ks=3, stride=1,
                  metric="active-voxels/sec 4-D (D=4) MinkowskiConvolution k3 C=32: hashing + "
-                        "kernel map (K=81) + fwd+bwd @200k coordinate draws, 1xB200 vs CPU ref",
+                        "kernel map (K=81) + fwd+bwd @200k coordinate draws, 1xH100 vs CPU ref",
                  what="BASELINE configs[4]"),
 }
 # bf16 network on bf16-rounded inputs vs the reference's fp32 loss (tests/golden/bench_step0_loss.json):
@@ -74,6 +78,7 @@ def parse_args():
     ap.add_argument("--voxels", type=int, default=None)
     ap.add_argument("--model", default=None)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     a = ap.parse_args()
     cfg = dict(CONFIGS[a.config])
     if cfg["kind"] == "net":
@@ -128,22 +133,32 @@ def load_peaks():
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0,
-            "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0,
+            "source": "fallback (H100 SXM data sheet)"}
 
 
-def load_traffic(kernel):
-    """DRAM bytes of one `ncu --set full` capture of `kernel` (committed under profiles/)."""
-    for name in ("r2_ncu_traffic.json", "r1_ncu_traffic.json"):
-        try:
-            cap = json.load(open(os.path.join(ROOT, "profiles", name)))[kernel]
-            return {"traffic": cap["dram_bytes_read"] + cap["dram_bytes_write"],
-                    "traffic_launch": cap["launch"],
-                    "traffic_algorithmic_bytes": cap["algorithmic_bytes"],
-                    "traffic_source": cap["capture"]}
-        except (OSError, KeyError, ValueError):
-            continue
-    return {"traffic": None}
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays, seed=0):
+    """Writes {name: tensor} as out_dir/<name>.npy (float64 stays float64, everything else
+    float32).  Arrays whose rows do not fit the remaining share of DUMP_LIMIT_BYTES are replaced
+    by a fixed, seeded sample of rows (2-D) or elements (1-D), saved with the indices taken."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_LIMIT_BYTES // max(1, len(arrays))
+    for name, t in sorted(arrays.items()):
+        a = t.detach().cpu()
+        a = np.atleast_1d(a.double().numpy() if a.dtype == torch.float64 else a.float().numpy())
+        row_bytes = a.itemsize * (a.size // max(1, a.shape[0]))
+        keep = max(1, share // (row_bytes + 8))          # + 8: the float64 index of a kept row
+        if a.nbytes > share and keep < a.shape[0]:
+            idx = np.sort(np.random.default_rng(seed).choice(a.shape[0], keep, replace=False))
+            np.save(os.path.join(out_dir, f"{name}.sample_index.npy"), idx.astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 class NvmlClockSampler:
@@ -425,6 +440,7 @@ def run_ours(args):
     loss_check = None
     flush_l2 = False
     ablate = []
+    last = {}          # --dump-outputs: the arrays the last step computed
 
     torch.manual_seed(0)
     if is_net:
@@ -433,7 +449,7 @@ def run_ours(args):
         net = net.to(dev)
         raw_net = net
         # MEB200_BENCH_ABLATE=nosyncbn,noddp,samedata: DIAGNOSIS ONLY (which part of the N>1 step
-        # costs what, profiles/r2_notes.md §6); recorded in config.ablate, never a bench value.
+        # costs what); recorded in config.ablate, never a bench value.
         ablate = sorted(x for x in os.environ.get("MEB200_BENCH_ABLATE", "").split(",") if x)
         if world > 1 and "nosyncbn" not in ablate:
             net = ME.MinkowskiSyncBatchNorm.convert_sync_batchnorm(net)
@@ -462,6 +478,9 @@ def run_ours(args):
             out = net(ME.SparseTensor(f, c))
             loss = crit(out.F.float(), l)
             loss.backward()
+            if args.dump_outputs:
+                last.update(logits=out.F, loss=loss, **{
+                    "grad." + n: p.grad for n, p in raw_net.named_parameters() if p.grad is not None})
             opt.step()
             return loss
 
@@ -504,11 +523,13 @@ def run_ours(args):
             y = conv(x)
             loss = y.F.float().square().mean()
             loss.backward()
+            if args.dump_outputs:
+                last.update(out=y.F, loss=loss, grad_kernel=conv.kernel.grad, grad_in=x.F.grad)
             return loss
 
         if D == 3:
             # cfg1: maps built once; the step is the layer's forward + backward alone, with an
-            # L2 flush between iterations (inputs + outputs + table = 26 MB < 126 MB L2)
+            # L2 flush between iterations (inputs + outputs + table = 26 MB < 50 MB L2)
             x_fixed = ME.SparseTensor(feats_d, coords_d)
             y0 = conv(x_fixed)
             gout = torch.rand(y0.F.shape, device=dev).to(dtype)
@@ -520,6 +541,8 @@ def run_ours(args):
                 y = conv(ME.SparseTensor(f, coordinate_map_key=x_fixed.coordinate_map_key,
                                          coordinate_manager=x_fixed.coordinate_manager))
                 y.F.backward(gout)
+                if args.dump_outputs:
+                    last.update(out=y.F, grad_kernel=conv.kernel.grad, grad_in=f.grad)
                 return y.F
         else:
             def step_resident():
@@ -571,7 +594,9 @@ def run_ours(args):
         if not sampler.start():
             sampler = ClockSampler(local_rank)
             sampler.start()
+    last.clear()
     ms, launches = timed(step_resident, args.steps, flush=flush_l2)
+    dumped = {k: v.detach().clone() for k, v in last.items() if v is not None}
     clocks = None
     if rank == 0:
         try:
@@ -620,8 +645,8 @@ def run_ours(args):
                     "hbm": {"achieved_gbs": gb(d), "peak_gbs": peaks["hbm_gbs"],
                             "frac": gb(d) / peaks["hbm_gbs"],
                             "note": "compulsory bytes (SURVEY.md 8d) / same durations"}}
-        fam = {"conv_fwd_dgrad": "k_conv_ts (tcgen05 sparse-conv forward/dgrad, operand A in tensor memory)",
-               "conv_wgrad": "k_wgrad_pairs (tcgen05 wgrad over compacted pair lists; its time "
+        fam = {"conv_fwd_dgrad": "k_conv_wg (wgmma sparse-conv forward/dgrad)",
+               "conv_wgrad": "k_wgrad_wg (wgmma wgrad over compacted pair lists; its time "
                              "includes building the lists when the map is new)"}
         km = prof["kernel_map"]
         km_entry = {"kernel": "k_kernel_map (hash probes -> neighbour tables)", "bound": "hbm",
@@ -636,7 +661,6 @@ def run_ours(args):
         if not is_net and cfg["D"] == 4:
             # cfg4: the hashing stress — the kernel-map probe kernel is the dominant launch
             roof = dict(km_entry)
-            roof.update(load_traffic("k_kernel_map"))
             roof["peak_source"] = f"{peaks['source']} (MEASURED_PEAKS.json hbm_gbs)"
             roof["conv"] = [entry(k, v) for k, v in fam.items() if prof[k]["launches"]]
         else:
@@ -648,7 +672,6 @@ def run_ours(args):
                 roof = {"bound": "tensor", "achieved": e["achieved"], "peak": peak,
                         "unit": "TFLOP/s", "frac": e["frac"],
                         "peak_source": f"{peaks['source']} (MEASURED_PEAKS.json bf16_tflops_sustained)"}
-                roof.update(load_traffic("k_wgrad_pairs" if top == "conv_wgrad" else "k_conv_ts"))
                 roof.update({k: v for k, v in e.items() if k not in ("achieved", "frac")})
                 roof["other"] = [entry(k, fam[k]) for k in live[1:]]
                 if km["launches"]:
@@ -661,7 +684,7 @@ def run_ours(args):
                         f"{args.voxels} voxels per rank ({cfg['what']}), coordinate/kernel maps "
                         "rebuilt every step")
             l2 = ("per-step working set (activations + neighbour tables, several hundred MB or "
-                  "more) exceeds the 126 MB L2; no explicit flush")
+                  "more) exceeds the 50 MB L2; no explicit flush")
         elif cfg["D"] == 3:
             workload = (f"MinkowskiConvolution {cfg['c_in']}->{cfg['c_out']} k{cfg['ks']} "
                         f"s{cfg['stride']} on surface({args.voxels}) ({cfg['what']}): forward + "
@@ -694,6 +717,8 @@ def run_ours(args):
             line["loss_check"] = loss_check
         if cpu is not None:
             line["cpu_baseline"] = cpu
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dumped)
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()

@@ -1,5 +1,5 @@
 /*
- * meb200.h — C ABI of the B200-native sparse-convolution hot path.
+ * meb200.h — C ABI of the H100-native (sm_90a) sparse-convolution hot path.
  *
  * Every entry point is `extern "C"`, takes plain device pointers + sizes + the CUDA
  * stream to launch on (as `void*`, i.e. a cudaStream_t), allocates nothing the caller
@@ -49,12 +49,12 @@ extern "C" {
 
 /* ---- library ---------------------------------------------------------------------- */
 const char *meb200_last_error(void);
-/* Compile-time facts: "sm_100a", CUDA runtime version the library was built with.     */
+/* Compile-time facts: "sm_90a", CUDA runtime version the library was built with.      */
 const char *meb200_build_arch(void);
 int meb200_cudart_version(void); /* reference: cudart_version(), pybind/extern.hpp:808-838 */
 /* Number of kernels this library has launched since load (bench.py's gpu_launches).   */
 uint64_t meb200_launch_count(void);
-/* ... of which launches of the tcgen05 (tensor-core) convolution kernels. */
+/* ... of which launches of the wgmma (tensor-core) convolution kernels. */
 uint64_t meb200_tc_launch_count(void);
 
 /* ---- coordinate hashing (reference a1/a2: src/coordinate.hpp:223-349,
@@ -180,10 +180,9 @@ int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32
  * fp32 master weight [K, Cin, Cout] -> `dtype` (BF16/F16) operand copies
  *   w_cast [K, Cin, Cout]                 w_t  [K, Cout, Cin]
  *   w_cp   [K, Cin, perm(Cout)]           w_tp [K, Cout, perm(Cin)]
- * where perm reorders the reduction axis inside every block of 32 channels to the order in
- * which the A-in-tensor-memory kernel lays gathered rows out (position 16h+4j+2e+b holds
- * channel 8j+4h+2e+b).  w_cp / w_tp may be NULL and are skipped when Cout / Cin is not a
- * multiple of 32.  The reference keeps weights in the feature dtype and needs no such step
+ * where perm reorders the reduction axis inside every block of 32 channels (position
+ * 16h+4j+2e+b holds channel 8j+4h+2e+b).  The convolution kernels read w_cast / w_t; w_cp /
+ * w_tp may be NULL and are skipped when NULL or when Cout / Cin is not a multiple of 32.  The reference keeps weights in the feature dtype and needs no such step
  * (MinkowskiConvolution.py:264-279); this is the bf16/fp16 operand cache of this backend. */
 int meb200_conv_pack_weights(const float *weight, uint32_t K, uint32_t c_in, uint32_t c_out,
                              int dtype, void *w_cast, void *w_t, void *w_cp, void *w_tp,
@@ -208,11 +207,13 @@ int meb200_conv_pack_weights_batched(const meb200_pack_job *jobs_dev, uint32_t n
  * the 64-byte-block gather of the general kernels, so the layer is run as a K = 1 convolution over
  * VIRTUAL channels v = 4 k + c (offset k < 16 ceil(K / 16), channel c < 4):
  *   in4            [n_in, 4]   the features zero-padded to 4 channels
- *   weight_v       [c_out, V]  V = meb200_conv_stem_virtual_channels(K); the `w_tp` output of
+ *   weight_v       [c_out, V]  V = meb200_conv_stem_virtual_channels(K); the `w_t` output of
  *                              meb200_conv_pack_weights(Wv, K=1, c_in=V, c_out) where
  *                              Wv[4 k + c][n] = W[k][c][n] (zero for padded k, c)
- *   grad_weight_v  [V, c_out]  fp32, same indexing (zero-filled by the call)
- * bf16 / fp16 only; c_out a multiple of 16, <= 256; K <= 128. */
+ *   grad_weight_v  [V, c_out]  fp32, same indexing (fully written by the call)
+ *   workspace      meb200_conv_wgrad_workspace_bytes(V, c_out, 1, n_out) bytes, 16-byte aligned,
+ *                  for the row-split partial sums (less, NULL or unaligned is legal: fewer splits)
+ * bf16 / fp16 only; c_out a multiple of 16, <= 256. */
 uint32_t meb200_conv_stem_virtual_channels(uint32_t K);
 int meb200_conv_stem_supported(int dtype, uint32_t K, uint32_t c_out);
 int meb200_conv_stem_forward(const void *in4, int dtype, uint32_t K, const void *weight_v,
@@ -220,33 +221,41 @@ int meb200_conv_stem_forward(const void *in4, int dtype, uint32_t K, const void 
                              int out_dtype, void *stream);
 int meb200_conv_stem_wgrad(const void *in4, const void *grad_out, int dtype, uint32_t K,
                            uint32_t c_out, const int32_t *out_nbr, uint32_t n_out,
-                           float *grad_weight_v, void *stream);
+                           float *grad_weight_v, void *workspace, uint64_t workspace_bytes,
+                           void *stream);
 
 /* meb200_conv_forward with the weight already packed (tensor-core path only: returns
  * MEB200_ERR_UNSUPPORTED for shapes/dtypes outside it, the caller then uses
  * meb200_conv_forward).  Same result, no per-call cast/transpose, no workspace.
- * weight_tp (may be NULL) selects the A-in-tensor-memory kernel when Cin % 32 == 0. */
+ * weight_tp (may be NULL) is accepted for compatibility and not read. */
 int meb200_conv_forward_packed(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
                                const void *weight_t, const void *weight_tp, uint32_t K,
                                uint32_t c_out, const int32_t *out_nbr, uint32_t n_out, void *out,
                                int out_dtype, void *stream);
 
-/* meb200_conv_backward on packed weights (w_cast, and w_cp or NULL), tensor-core path only;
+/* meb200_conv_backward on packed weights (w_cast; w_cp is accepted and not read), tensor-core
+ * path only;
  * grad_in / grad_weight may be NULL to skip dgrad / wgrad.  pairs_in / pairs_out / seg_start
  * (all three or NULL) + n_chunks: the compacted pair lists of out_nbr from
  * meb200_kernel_map_pairs with stage = 64 and their chunk count; with them wgrad reduces over
- * valid pairs only instead of the dense table. */
+ * valid pairs only instead of the dense table.  workspace: as for meb200_conv_stem_wgrad, sized
+ * by meb200_conv_wgrad_workspace_bytes(c_in, c_out, K, n_out). */
 int meb200_conv_backward_packed(const void *in, const void *grad_out, int dtype, uint32_t n_in,
                                 uint32_t c_in, const void *w_cast, const void *w_cp, uint32_t K,
                                 uint32_t c_out, const int32_t *out_nbr, const int32_t *in_nbr,
                                 uint32_t n_out, void *grad_in, int grad_in_dtype,
                                 float *grad_weight, const int32_t *pairs_in,
                                 const int32_t *pairs_out, const int32_t *seg_start,
-                                uint32_t n_chunks, void *stream);
+                                uint32_t n_chunks, void *workspace, uint64_t workspace_bytes,
+                                void *stream);
 
 /* Workspace the two calls above may use (0 is legal: slower fallbacks are chosen). */
 uint64_t meb200_conv_workspace_bytes(uint32_t n_in, uint32_t n_out, uint32_t c_in,
                                      uint32_t c_out, uint32_t K, int dtype);
+/* Workspace for the row-split partial sums of a wgrad over n_out rows (0: none needed).  Row
+ * splits add their sums in a fixed order, so wgrad is deterministic for a given workspace size. */
+uint64_t meb200_conv_wgrad_workspace_bytes(uint32_t c_in, uint32_t c_out, uint32_t K,
+                                           uint32_t n_out);
 
 /* ---- local pooling (reference a11: src/pooling_avg_kernel.hpp:40-150,
  *      src/pooling_max_kernel.hpp:35-115, src/local_pooling_cpu.cpp:43-185) ---------- */

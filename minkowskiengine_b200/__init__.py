@@ -1,4 +1,4 @@
-"""minkowskiengine_b200 — a Blackwell-native (sm_100a) backend for the sparse-convolution
+"""minkowskiengine_b200 — an H100-native (sm_90a) backend for the sparse-convolution
 hot path of NVIDIA/MinkowskiEngine, behind the reference's own Python API.
 
     import minkowskiengine_b200 as ME

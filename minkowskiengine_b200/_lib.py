@@ -8,7 +8,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# MEB200_LIB=libmeb200_g4.so picks an A/B build of the same sources (csrc/build.py)
+# MEB200_LIB=libmeb200_x.so picks an A/B build of the same sources (csrc/build.py)
 LIB_PATH = os.path.join(_HERE, "csrc", os.environ.get("MEB200_LIB", "libmeb200.so"))
 
 OK = 0
@@ -46,16 +46,18 @@ PROTOTYPES = {
     "meb200_conv_stem_virtual_channels": (_u32, [_u32]),
     "meb200_conv_stem_supported": (_i32, [_i32, _u32, _u32]),
     "meb200_conv_stem_forward": (_i32, [_vp, _i32, _u32, _vp, _u32, _vp, _u32, _vp, _i32, _vp]),
-    "meb200_conv_stem_wgrad": (_i32, [_vp, _vp, _i32, _u32, _u32, _vp, _u32, _vp, _vp]),
+    "meb200_conv_stem_wgrad": (_i32, [_vp, _vp, _i32, _u32, _u32, _vp, _u32, _vp, _vp, _u64, _vp]),
     "meb200_conv_forward_packed": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _u32,
                                           _vp, _i32, _vp]),
     "meb200_conv_backward_packed": (_i32, [_vp, _vp, _i32, _u32, _u32, _vp, _vp, _u32, _u32, _vp,
-                                           _vp, _u32, _vp, _i32, _vp, _vp, _vp, _vp, _u32, _vp]),
+                                           _vp, _u32, _vp, _i32, _vp, _vp, _vp, _vp, _u32, _vp, _u64,
+                                           _vp]),
     "meb200_pair_list_chunks": (_u32, [_u32, _u32]),
     "meb200_pair_list_scratch_bytes": (_u64, [_u32, _u32, _u32]),
     "meb200_pair_list_capacity": (_u64, [_u32, _u32, _u32, _u32]),
     "meb200_kernel_map_pairs": (_i32, [_vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "meb200_conv_workspace_bytes": (_u64, [_u32, _u32, _u32, _u32, _u32, _i32]),
+    "meb200_conv_wgrad_workspace_bytes": (_u64, [_u32, _u32, _u32, _u32]),
     "meb200_pool_forward": (_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _u32, _i32, _vp, _vp, _vp]),
     "meb200_pool_backward": (_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _u32, _i32, _vp, _vp,
                                     _vp]),

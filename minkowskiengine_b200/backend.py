@@ -183,10 +183,9 @@ class _KernelMap:
 
     __slots__ = ("out_nbr", "_in_nbr", "_in_thunk", "_n_in", "stride_pairs", "_n_pairs", "_pairs",
                  "_pair_src", "_hint_key")
-    PAIR_STAGE = 64   # pairs per pipeline stage of the wgrad kernel (k_wgrad_pairs)
-    # table rows per chunk of the pair lists (multiple of 2048)
-    # (measured on block8 96->96 wgrad, 800k rows: 16384 rows 0.64 ms, 65536 0.49, 131072 0.45,
-    #  262144 0.44, one chunk 0.46 — profiles/r2_notes.md §7)
+    PAIR_STAGE = 64   # pairs per pipeline stage of the wgrad kernel (k_wgrad_wg)
+    # table rows per chunk of the pair lists (multiple of 2048): one chunk's rows of both feature
+    # matrices stay L2-resident while the wgrad walks its K offsets
     PAIR_CHUNK_ROWS = int(os.environ.get("MEB200_PAIR_CHUNK_ROWS", "262144"))
 
     def __init__(self, out_nbr, in_nbr, stride_pairs=None, n_in=None, in_thunk=None):
@@ -705,13 +704,21 @@ def _workspace(n_in, n_out, c_in, c_out, K, code, device):
     return torch.empty(nbytes, dtype=torch.uint8, device=device), nbytes
 
 
+def _wgrad_workspace(c_in, c_out, K, n_out, device):
+    """Room for the row-split partial sums of a wgrad (added in a fixed order: deterministic)."""
+    nbytes = int(_lib.load().meb200_conv_wgrad_workspace_bytes(c_in, c_out, K, n_out))
+    if nbytes == 0:
+        return None, 0
+    return torch.empty(nbytes, dtype=torch.uint8, device=device), nbytes
+
+
 # ---- live per-kernel timing for bench.py's roofline (CUDA events on the launch stream) ------
 _PROFILE = None   # None, or {"conv_fwd_dgrad": [...], "conv_wgrad": [...], "kernel_map": [...]}
 
 
 def _record(kind, fn, flops, nbytes, always=False):
     """Run fn() between two CUDA events on the current stream; keep the record if it launched
-    a tcgen05 kernel (the family the roofline is reported for) or `always`."""
+    a tensor-core kernel (the family the roofline is reported for) or `always`."""
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     tc0 = _lib.tc_launch_count()
     e0.record()
@@ -778,7 +785,7 @@ class _PackTable:
 
     def __init__(self, device, dtype):
         self.device, self.dtype = device, dtype
-        self.entries = {}        # id(kernel) -> [weakref, data_ptr, packed 4-tuple]
+        self.entries = {}        # id(kernel) -> [weakref, data_ptr, (w_cast, w_t)]
         self.jobs_dev = None
         self.n_jobs = self.total_tiles = 0
         self.order = []          # ids in job order
@@ -795,9 +802,9 @@ class _PackTable:
                 del self.entries[key]
                 continue
             K, c_in, c_out = k.shape
-            w_cast, w_t, w_cp, w_tp = packed
-            jobs.append(_PackJob(ptr, _lib.ptr(w_cast), _lib.ptr(w_t), _lib.ptr(w_cp),
-                                 _lib.ptr(w_tp), K, c_in, c_out, tile))
+            w_cast, w_t = packed
+            jobs.append(_PackJob(ptr, _lib.ptr(w_cast), _lib.ptr(w_t), None, None, K, c_in, c_out,
+                                 tile))
             tile += K * ((c_in + 31) // 32) * ((c_out + 31) // 32)
             self.order.append(key)
         self.n_jobs, self.total_tiles = len(jobs), tile
@@ -833,9 +840,9 @@ _PACK_TABLES = {}      # (device index, dtype) -> _PackTable
 
 
 def _packed_weights(kernel, dtype):
-    """(w_cast [K,Cin,Cout], w_t [K,Cout,Cin], w_cp, w_tp) of an fp32 master weight in `dtype`
-    (w_cp / w_tp: the k_conv_ta layouts, None when the reduction width is not a multiple of 32),
-    rebuilt only when the tensor was modified in place (its autograd version counter moved) or
+    """(w_cast [K,Cin,Cout], w_t [K,Cout,Cin]) of an fp32 master weight in `dtype` (the operand-B
+    layouts of dgrad and forward; the permuted copies the packing ABI can also emit are not read
+    by any kernel and are not built), rebuilt only when the tensor was modified in place (its autograd version counter moved) or
     replaced."""
     key = id(kernel)
     ent = _PACKED.get(key)
@@ -855,17 +862,15 @@ def _packed_weights(kernel, dtype):
     lib = _lib.load()
     K, c_in, c_out = kernel.shape
     src = kernel.detach()
-    buf = torch.empty((4, K * c_in * c_out), dtype=dtype, device=kernel.device)
+    buf = torch.empty((2, K * c_in * c_out), dtype=dtype, device=kernel.device)
     w_cast, w_t = buf[0].view(K, c_in, c_out), buf[1].view(K, c_out, c_in)
-    w_cp = buf[2].view(K, c_in, c_out) if c_out % 32 == 0 else None
-    w_tp = buf[3].view(K, c_out, c_in) if c_in % 32 == 0 else None
     _lib.check(lib.meb200_conv_pack_weights(
         _lib.ptr(src), K, c_in, c_out, _lib.dtype_code(dtype), _lib.ptr(w_cast), _lib.ptr(w_t),
-        _lib.ptr(w_cp), _lib.ptr(w_tp), _lib.current_stream()))
+        None, None, _lib.current_stream()))
     if len(_PACKED) > 4096:      # dead entries of discarded networks
         for k in [k for k, e in _PACKED.items() if e[0]() is None]:
             del _PACKED[k]
-    packed = (w_cast, w_t, w_cp, w_tp)
+    packed = (w_cast, w_t)
     _PACKED[key] = (weakref.ref(kernel), kernel._version, kernel.data_ptr(), dtype, packed)
     if tbl is not None:
         tbl.add(kernel, packed)            # first sight of this kernel: packed alone, batched next time
@@ -896,11 +901,11 @@ def _stem_weights(kernel, dtype):
     V = int(lib.meb200_conv_stem_virtual_channels(K))
     wv = torch.zeros((V // 4, 4, c_out), dtype=torch.float32, device=kernel.device)
     wv[:K, :c_in] = kernel.detach()
-    buf = torch.empty((4, V * c_out), dtype=dtype, device=kernel.device)
+    buf = torch.empty((2, V * c_out), dtype=dtype, device=kernel.device)
     _lib.check(lib.meb200_conv_pack_weights(
         _lib.ptr(wv), 1, V, c_out, _lib.dtype_code(dtype), _lib.ptr(buf[0]), _lib.ptr(buf[1]),
-        _lib.ptr(buf[2]) if c_out % 32 == 0 else None, _lib.ptr(buf[3]), _lib.current_stream()))
-    w_v = buf[3].view(c_out, V)
+        None, None, _lib.current_stream()))
+    w_v = buf[1].view(c_out, V)
     _PACKED[key] = (weakref.ref(kernel), kernel._version, kernel.data_ptr(), dtype, w_v)
     return w_v
 
@@ -935,11 +940,11 @@ def _conv_forward_impl(in_feat, kernel, km, out_dtype=None):
     if _can_pack(kernel, in_feat.dtype):
         K, c_in, c_out = kernel.shape
         _assert(K == km.K, "kernel volume", K, "does not match the kernel map", km.K)
-        _, w_t, _, w_tp = _packed_weights(kernel, in_feat.dtype)
+        _, w_t = _packed_weights(kernel, in_feat.dtype)
         out = torch.empty((km.n_out, c_out), dtype=out_dtype or in_feat.dtype,
                           device=in_feat.device)
         rc = lib.meb200_conv_forward_packed(
-            _lib.ptr(in_feat), code, km.n_in, c_in, _lib.ptr(w_t), _lib.ptr(w_tp), K, c_out,
+            _lib.ptr(in_feat), code, km.n_in, c_in, _lib.ptr(w_t), None, K, c_out,
             _lib.ptr(km.out_nbr), km.n_out, _lib.ptr(out), _lib.dtype_code(out.dtype),
             _lib.current_stream())
         if rc != _ERR_UNSUPPORTED:
@@ -996,23 +1001,26 @@ def _conv_backward_impl(in_feat, grad_out, kernel, km, need_in=True, need_w=True
         V = int(lib.meb200_conv_stem_virtual_channels(K))
         gwv = torch.empty((V // 4, 4, c_out), dtype=torch.float32, device=in_feat.device)
         in4 = _pad4(in_feat)
+        ws, ws_bytes = _wgrad_workspace(V, c_out, 1, n_out, in_feat.device)
         rc = lib.meb200_conv_stem_wgrad(
             _lib.ptr(in4), _lib.ptr(grad_out), code, K, c_out, _lib.ptr(km.out_nbr),
-            n_out, _lib.ptr(gwv), _lib.current_stream())
+            n_out, _lib.ptr(gwv), _lib.ptr(ws), ws_bytes, _lib.current_stream())
         if rc != _ERR_UNSUPPORTED:
             _lib.check(rc)
             return None, gwv[:K, :c_in].contiguous()
     if _can_pack(kernel, in_feat.dtype):
-        w, _, w_cp, _ = _packed_weights(kernel, in_feat.dtype)
+        w, _ = _packed_weights(kernel, in_feat.dtype)
         pin = pout = seg = None
         nch = 0
         if need_w and c_in % 8 == 0 and c_in >= 16 and K <= 1023:
             pin, pout, seg, nch = km.pair_lists()
+        ws, ws_bytes = _wgrad_workspace(c_in, c_out, K, n_out, in_feat.device) if need_w \
+            else (None, 0)
         rc = lib.meb200_conv_backward_packed(
-            _lib.ptr(in_feat), _lib.ptr(grad_out), code, n_in, c_in, _lib.ptr(w), _lib.ptr(w_cp),
+            _lib.ptr(in_feat), _lib.ptr(grad_out), code, n_in, c_in, _lib.ptr(w), None,
             K, c_out, _lib.ptr(km.out_nbr), _lib.ptr(km.in_nbr) if need_in else None, n_out,
             _lib.ptr(grad_in), code, _lib.ptr(grad_w), _lib.ptr(pin), _lib.ptr(pout), _lib.ptr(seg), nch,
-            _lib.current_stream())
+            _lib.ptr(ws), ws_bytes, _lib.current_stream())
         if rc != _ERR_UNSUPPORTED:
             _lib.check(rc)
             return grad_in, grad_w

@@ -3,7 +3,9 @@
 // (MinkowskiNormalization.py:51-99); torch's channels-last kernels run ~8x off the HBM
 // roofline on [800k, 96] bf16 and cost 18 % of a MinkUNet34C step, so the four passes are
 // provided here as streaming kernels: 16-byte row-segment loads, per-thread fp32 partials over
-// a strided set of rows, shared-memory combine, one fp64 atomic per channel per CTA.
+// a strided set of rows, combined in a fixed order: per CTA in shared memory, then the CTAs' fp64
+// partials by the last CTA in block order (no floating-point atomics: results do not depend on
+// the order in which threads or CTAs finish).
 //
 //   stats      : S1[c] = sum_r x[r,c],  S2[c] = sum_r x[r,c]^2                 (fp64 [2C])
 //   finalize   : mean, invstd (biased var, eps) + running-stat update (unbiased var)
@@ -94,8 +96,8 @@ __device__ __forceinline__ BnGeom bn_geom(uint32_t C) {
 }
 
 // What the LAST CTA of a reduction does with the totals (ticket != NULL): the work of the
-// separate finalize launch / gradient conversion, and it leaves `sums` and the ticket zero again,
-// so one workspace serves every layer of a stream without a memset per use (a MinkUNet34C step
+// separate finalize launch / gradient conversion, and it leaves the CTA slots of `sums` and the
+// ticket zero again, so one workspace serves every layer of a stream without a memset per use (a MinkUNet34C step
 // spent ~250 of its ~1030 launches on 2 KB memsets and 1-CTA finalize kernels).
 struct BnTail {
   uint32_t *ticket;
@@ -116,7 +118,16 @@ struct BnTail {
   long long *num_batches_tracked;                       // MODE 0: incremented once (may be NULL)
 };
 constexpr uint32_t kBnMaxC = 2048;
-constexpr size_t kBnWorkspaceBytes = 2 * kBnMaxC * sizeof(double) + 64;   // sums, then the ticket
+constexpr uint32_t kBnMaxCtas = 512;     // reduction CTAs: each owns a [2C] fp64 slot
+constexpr size_t kBnPartialBytes = (size_t)kBnMaxCtas * 2 * kBnMaxC * sizeof(double);
+constexpr size_t kBnWorkspaceBytes = kBnPartialBytes + 64;   // CTA partials, then the ticket
+// dynamic shared memory of k_bn_reduce: per-thread partials [rows_per_pass][2C] fp32, later the
+// totals [2C] fp64 + a [256] fp64 combine scratch
+inline size_t bn_reduce_smem(uint32_t C) {
+  const size_t rpp = kBnThreads / (C / 8);
+  const size_t a = rpp * 2 * C * sizeof(float), b = (2 * (size_t)C + kBnThreads) * sizeof(double);
+  return a > b ? a : b;
+}
 
 // TWO per-channel sums: MODE 0: (x, x^2); MODE 1: (dy, dy * xhat)
 template <typename T, int MODE>
@@ -124,9 +135,10 @@ __global__ void __launch_bounds__(kBnThreads)
 k_bn_reduce(const T *__restrict__ a, const T *__restrict__ x, const T *__restrict__ ymask,
             const float *__restrict__ mean, const float *__restrict__ invstd, uint32_t n,
             uint32_t C, uint32_t rows_per_cta, double *sums, const BnTail tail) {
-  extern __shared__ float s_acc[];   // [2C]
-  for (uint32_t i = threadIdx.x; i < 2 * C; i += kBnThreads) s_acc[i] = 0.f;
-  __syncthreads();
+  // sums: [gridDim.x][2C] fp64, this CTA's slot written once
+  extern __shared__ double s_dyn[];
+  float *s_part = reinterpret_cast<float *>(s_dyn);        // [rows_per_pass][2C]
+  const uint32_t C2 = 2 * C;
   const BnGeom g = bn_geom(C);
   if (threadIdx.x < g.active) {
     const uint32_t cg = threadIdx.x % g.G, r0 = threadIdx.x / g.G;
@@ -178,13 +190,16 @@ k_bn_reduce(const T *__restrict__ a, const T *__restrict__ x, const T *__restric
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      atomicAdd(&s_acc[cg * 8 + i], s1[i]);
-      atomicAdd(&s_acc[C + cg * 8 + i], s2[i]);
+      s_part[r0 * C2 + cg * 8 + i] = s1[i];
+      s_part[r0 * C2 + C + cg * 8 + i] = s2[i];
     }
   }
   __syncthreads();
-  for (uint32_t i = threadIdx.x; i < 2 * C; i += kBnThreads) atomicAdd(&sums[i], (double)s_acc[i]);
-  if (tail.ticket == nullptr) return;
+  for (uint32_t i = threadIdx.x; i < C2; i += kBnThreads) {
+    double v = 0.0;
+    for (uint32_t r = 0; r < g.rows_per_pass; ++r) v += (double)s_part[r * C2 + i];
+    sums[(size_t)blockIdx.x * C2 + i] = v;
+  }
   __shared__ bool s_last;
   __threadfence();
   __syncthreads();
@@ -192,14 +207,38 @@ k_bn_reduce(const T *__restrict__ a, const T *__restrict__ x, const T *__restric
   __syncthreads();
   if (!s_last) return;
   __threadfence();
+  // totals over the CTAs in block order; J threads per value when 2C < 256, combined in j order.
+  // Each slot is read by one thread and cleared as it is read (the workspace is left zero).
+  auto take = [](double *p) { const double v = __ldcg(p); *p = 0.0; return v; };
+  double *s_tot = s_dyn, *s_scr = s_dyn + C2;
+  const uint32_t J = C2 >= kBnThreads ? 1u : kBnThreads / C2;
+  if (J == 1) {
+    for (uint32_t i = threadIdx.x; i < C2; i += kBnThreads) {
+      double v = 0.0;
+      for (uint32_t b = 0; b < gridDim.x; ++b) v += take(sums + (size_t)b * C2 + i);
+      s_tot[i] = v;
+    }
+  } else {
+    if (threadIdx.x < J * C2) {
+      const uint32_t i = threadIdx.x % C2, j = threadIdx.x / C2;
+      double v = 0.0;
+      for (uint32_t b = j; b < gridDim.x; b += J) v += take(sums + (size_t)b * C2 + i);
+      s_scr[j * C2 + i] = v;
+    }
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < C2; i += kBnThreads) {
+      double v = 0.0;
+      for (uint32_t j = 0; j < J; ++j) v += s_scr[j * C2 + i];
+      s_tot[i] = v;
+    }
+  }
+  __syncthreads();
   double count = tail.count;
   const bool synced = tail.peer_bases != nullptr;
   if (synced) {
     double *slot = reinterpret_cast<double *>(tail.peer_bases[tail.peer_rank] + tail.peer_slot_offset);
     for (uint32_t c = threadIdx.x; c < C; c += kBnThreads) {
-      const double t1 = __ldcg(sums + c), t2 = __ldcg(sums + C + c);
-      sums[c] = 0.0;
-      sums[C + c] = 0.0;
+      const double t1 = s_tot[c], t2 = s_tot[C + c];
       slot[c] = t1;
       slot[C + c] = t2;
       if (MODE == 1) {
@@ -232,10 +271,8 @@ k_bn_reduce(const T *__restrict__ a, const T *__restrict__ x, const T *__restric
         t2 += ld_relaxed_sys_f64(ps + C + c);
       }
     } else {
-      t1 = __ldcg(sums + c);
-      t2 = __ldcg(sums + C + c);
-      sums[c] = 0.0;
-      sums[C + c] = 0.0;
+      t1 = s_tot[c];
+      t2 = s_tot[C + c];
     }
     if (tail.totals_out != nullptr) { tail.totals_out[c] = t1; tail.totals_out[C + c] = t2; }
     if (MODE == 0) {
@@ -414,8 +451,13 @@ static int bn_launch_reduce(int mode, const void *a, const void *x, const void *
                             double *sums, const BnTail &tail, cudaStream_t s) {
   unsigned grid;
   uint32_t rows = bn_rows_per_cta(n, C, &grid);
+  if (grid > kBnMaxCtas) {          // one workspace slot per CTA
+    const uint32_t rpp = kBnThreads / (C / 8);
+    rows = cdiv(cdiv(n, kBnMaxCtas), rpp) * rpp;
+    grid = cdiv(n, rows);
+  }
   if (grid == 0) grid = 1;          // an empty rank still takes part in the exchange
-  size_t smem = 2 * (size_t)C * sizeof(float);
+  const size_t smem = bn_reduce_smem(C);
 #define MEB_BN_RED(TT)                                                                            \
   do {                                                                                            \
     if (mode == 0)                                                                                \
@@ -440,7 +482,7 @@ static int bn_launch_reduce(int mode, const void *a, const void *x, const void *
 uint64_t meb200_bn_workspace_bytes(void) { return kBnWorkspaceBytes; }
 
 static inline uint32_t *bn_ticket(void *workspace) {
-  return reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(workspace) + 2 * kBnMaxC * sizeof(double));
+  return reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(workspace) + kBnPartialBytes);
 }
 
 int meb200_bn_forward_train(const void *x, int dtype, uint32_t n, uint32_t C, const float *weight,

@@ -1,4 +1,4 @@
-"""Builds libmeb200.so (the C-ABI library) in-tree with nvcc for sm_100a.
+"""Builds libmeb200.so (the C-ABI library) in-tree with nvcc for sm_90a (H100).
 
     python minkowskiengine_b200/csrc/build.py [--force] [--verbose]
 
@@ -13,14 +13,14 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-# A/B builds for kernel experiments: MEB200_BUILD_SUFFIX=_g4 MEB200_BUILD_DEFINES=-DMEB_TS_GROUPS=4
-# writes libmeb200_g4.so next to the default library (selected at run time with MEB200_LIB).
+# A/B builds for kernel experiments: MEB200_BUILD_SUFFIX=_x MEB200_BUILD_DEFINES=-DNAME=VALUE
+# writes libmeb200_x.so next to the default library (selected at run time with MEB200_LIB).
 SUFFIX = os.environ.get("MEB200_BUILD_SUFFIX", "")
 DEFINES = os.environ.get("MEB200_BUILD_DEFINES", "").split()
 SO = os.path.join(HERE, f"libmeb200{SUFFIX}.so")
 OBJ = os.path.join(HERE, f"build{SUFFIX}")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-lineinfo", "-std=c++17", "-ccbin", "/usr/bin/g++", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr"]
 

@@ -39,7 +39,7 @@ int num_sms() {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
       cached = n;
     else
-      cached = 148;
+      cached = 132;   // H100 SXM
   }
   return cached;
 }
@@ -50,7 +50,7 @@ extern "C" {
 
 const char *meb200_last_error(void) { return meb200::g_err; }
 
-const char *meb200_build_arch(void) { return "sm_100a"; }
+const char *meb200_build_arch(void) { return "sm_90a"; }
 
 int meb200_cudart_version(void) { return CUDART_VERSION; }
 

@@ -1,4 +1,4 @@
-// Shared host/device helpers for the meb200 kernels (sm_100a only).
+// Shared host/device helpers for the meb200 kernels (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

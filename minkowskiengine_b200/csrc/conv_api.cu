@@ -1,4 +1,4 @@
-// C-ABI entry points of the sparse convolution; picks the tcgen05 path when the shape
+// C-ABI entry points of the sparse convolution; picks the tensor-core path when the shape
 // qualifies (conv_tc.cuh) and the SIMT path otherwise.
 #include <stdlib.h>
 
@@ -21,10 +21,18 @@ extern "C" {
 
 uint64_t meb200_conv_workspace_bytes(uint32_t n_in, uint32_t n_out, uint32_t c_in,
                                      uint32_t c_out, uint32_t K, int dtype) {
-  (void)n_in; (void)n_out;
+  (void)n_in;
   if (dtype == MEB200_F32) return 0;
-  // bf16/fp16 weights re-laid out for the tensor-core kernels: W^T per offset
-  return (uint64_t)K * c_in * c_out * 2 + 256;
+  // bf16/fp16 weights re-laid out for the tensor-core kernels (W^T per offset), or the row-split
+  // partial sums of wgrad (the two are never needed by the same call)
+  const uint64_t wt = (uint64_t)K * c_in * c_out * 2 + 256;
+  const uint64_t wg = conv_wgrad_workspace_bytes(c_in, c_out, K, n_out);
+  return wt > wg ? wt : wg;
+}
+
+uint64_t meb200_conv_wgrad_workspace_bytes(uint32_t c_in, uint32_t c_out, uint32_t K,
+                                           uint32_t n_out) {
+  return conv_wgrad_workspace_bytes(c_in, c_out, K, n_out);
 }
 
 int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
@@ -96,14 +104,15 @@ int meb200_conv_stem_forward(const void *in4, int dtype, uint32_t K, const void 
 
 int meb200_conv_stem_wgrad(const void *in4, const void *grad_out, int dtype, uint32_t K,
                            uint32_t c_out, const int32_t *out_nbr, uint32_t n_out,
-                           float *grad_weight_v, void *stream_) {
+                           float *grad_weight_v, void *workspace, uint64_t workspace_bytes,
+                           void *stream_) {
   MEB_CHECK_ARG(grad_weight_v && (n_out == 0 || (in4 && grad_out && out_nbr)), "null buffer");
   if (tc_disabled() || !conv_stem_wgrad_tc_supported(dtype, K, c_out)) {
     set_error("stem wgrad: shape/dtype outside the tensor-core path (K=%u c_out=%u)", K, c_out);
     return MEB200_ERR_UNSUPPORTED;
   }
   return conv_stem_wgrad_tc(in4, grad_out, dtype, K, c_out, out_nbr, n_out, grad_weight_v,
-                            (cudaStream_t)stream_);
+                            workspace, workspace_bytes, (cudaStream_t)stream_);
 }
 
 int meb200_conv_forward_packed(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
@@ -111,6 +120,7 @@ int meb200_conv_forward_packed(const void *in, int in_dtype, uint32_t n_in, uint
                                uint32_t c_out, const int32_t *out_nbr, uint32_t n_out, void *out,
                                int out_dtype, void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
+  (void)weight_tp;   // the permuted copy: accepted for ABI stability, the kernels read weight_t
   if (n_out == 0) return MEB200_OK;
   MEB_CHECK_ARG(in_dtype >= 0 && in_dtype <= 2 && out_dtype >= 0 && out_dtype <= 2, "dtype");
   MEB_CHECK_ARG(out_dtype == MEB200_F32 || out_dtype == in_dtype,
@@ -123,8 +133,7 @@ int meb200_conv_forward_packed(const void *in, int in_dtype, uint32_t n_in, uint
   }
   // W^T[k][c_out][c_in] is operand B as the kernels want it: the "no transpose" entry
   return conv_forward_tc(in, in_dtype, n_in, c_in, weight_t, K, c_out, /*dgrad=*/true, out_nbr,
-                         n_out, out, out_dtype, nullptr, stream,
-                         c_in % 32 == 0 ? weight_tp : nullptr);
+                         n_out, out, out_dtype, nullptr, stream);
 }
 
 int meb200_conv_backward_packed(const void *in, const void *grad_out, int dtype, uint32_t n_in,
@@ -133,8 +142,10 @@ int meb200_conv_backward_packed(const void *in, const void *grad_out, int dtype,
                                 uint32_t n_out, void *grad_in, int grad_in_dtype,
                                 float *grad_weight, const int32_t *pairs_in,
                                 const int32_t *pairs_out, const int32_t *seg_start,
-                                uint32_t n_chunks, void *stream_) {
+                                uint32_t n_chunks, void *workspace, uint64_t workspace_bytes,
+                                void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
+  (void)w_cp;        // the permuted copy: accepted for ABI stability, the kernels read w_cast
   MEB_CHECK_ARG(dtype == MEB200_BF16 || dtype == MEB200_F16, "packed backward is bf16 or fp16");
   MEB_CHECK_ARG(grad_in_dtype == MEB200_F32 || grad_in_dtype == dtype,
                 "grad_in dtype must be fp32 or the feature dtype");
@@ -149,13 +160,12 @@ int meb200_conv_backward_packed(const void *in, const void *grad_out, int dtype,
   if (grad_in != nullptr && n_in > 0) {
     MEB_CHECK_ARG(in_nbr && w_cast && (grad_out || n_out == 0), "null buffer");
     int rc = conv_forward_tc(grad_out, dtype, n_out, c_out, w_cast, K, c_in, /*dgrad=*/true, in_nbr,
-                             n_in, grad_in, grad_in_dtype, nullptr, stream,
-                             c_out % 32 == 0 ? w_cp : nullptr);
+                             n_in, grad_in, grad_in_dtype, nullptr, stream);
     if (rc != MEB200_OK) return rc;
   }
   if (grad_weight != nullptr) {
     MEB_CHECK_ARG(out_nbr && (in || n_in == 0) && (grad_out || n_out == 0), "null buffer");
-    static int use_pairs = -1;    // MEB200_TC_WGRAD=dense keeps the round-1 dense kernel
+    static int use_pairs = -1;    // MEB200_TC_WGRAD=dense walks the table instead of the pair lists
     if (use_pairs < 0) {
       const char *e = getenv("MEB200_TC_WGRAD");
       use_pairs = (e && e[0] == 'd') ? 0 : 1;
@@ -163,10 +173,12 @@ int meb200_conv_backward_packed(const void *in, const void *grad_out, int dtype,
     if (use_pairs && pairs_in && pairs_out && seg_start && n_chunks > 0 &&
         conv_wgrad_pairs_supported(dtype, c_in, K, c_out)) {
       int rc = conv_wgrad_pairs(in, grad_out, dtype, c_in, K, c_out, pairs_in, pairs_out,
-                                seg_start, n_chunks, n_out, grad_weight, stream);
+                                seg_start, n_chunks, n_out, grad_weight, workspace,
+                                workspace_bytes, stream);
       if (rc != MEB200_ERR_UNSUPPORTED) return rc;
     }
-    return conv_wgrad_tc(in, grad_out, dtype, c_in, K, c_out, out_nbr, n_out, grad_weight, stream);
+    return conv_wgrad_tc(in, grad_out, dtype, c_in, K, c_out, out_nbr, n_out, grad_weight,
+                         workspace, workspace_bytes, stream);
   }
   return MEB200_OK;
 }
@@ -199,7 +211,7 @@ int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32
     MEB_CHECK_ARG(out_nbr && (in || n_in == 0) && (grad_out || n_out == 0), "null buffer");
     if (tc && conv_wgrad_tc_supported(dtype, c_in, c_out)) {
       int rc = conv_wgrad_tc(in, grad_out, dtype, c_in, K, c_out, out_nbr, n_out, grad_weight,
-                             stream);
+                             workspace, workspace_bytes, stream);
       if (rc != MEB200_ERR_UNSUPPORTED) return rc;
     }
     if (conv_small_cin_supported(c_in, c_out))

@@ -1,5 +1,5 @@
 // SIMT (CUDA-core, fp32-accumulate) sparse convolution kernels: the exact-fp32 parity
-// path and the fallback for channel counts the tcgen05 path does not take.
+// path and the fallback for channel counts the wgmma path does not take.
 #pragma once
 #include "common.cuh"
 

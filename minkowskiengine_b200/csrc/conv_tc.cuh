@@ -1,10 +1,10 @@
-// tcgen05 (5th-gen tensor core, TMEM accumulator) sparse convolution kernels.
+// wgmma (Hopper warpgroup MMA) sparse convolution kernels, bf16/fp16 operands, fp32 accumulation.
 #pragma once
 #include "common.cuh"
 
 namespace meb200 {
 
-// bf16/fp16 features with channel counts the UMMA tiles cover.
+// bf16/fp16 features with channel counts the wgmma tiles cover.
 bool conv_tc_supported(int dtype, uint32_t c_reduce, uint32_t c_cols);
 bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out);
 
@@ -13,10 +13,9 @@ bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out);
 // c_cols = c_in.  `workspace` receives the re-laid-out operand-B copy of W.
 int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *W,
                     uint32_t K, uint32_t c_cols, bool dgrad, const int32_t *nbr, uint32_t n_rows,
-                    void *out, int out_dtype, void *workspace, cudaStream_t stream,
-                    const void *Wperm = nullptr);        // operand B in ta_perm order (k_conv_ts)
+                    void *out, int out_dtype, void *workspace, cudaStream_t stream);
 
-// fp32 W[K,c_in,c_out] -> w_cast [K,c_in,c_out], w_t [K,c_out,c_in] and their k_conv_ta twins
+// fp32 W[K,c_in,c_out] -> w_cast [K,c_in,c_out], w_t [K,c_out,c_in] and the permuted copies
 // w_cp / w_tp (reduction axis permuted within 32-channel blocks; may be NULL) in bf16/fp16.
 int conv_pack_weights(const float *W, uint32_t K, uint32_t c_in, uint32_t c_out, int dtype,
                       void *w_cast, void *w_t, void *w_cp, void *w_tp, cudaStream_t stream);
@@ -33,18 +32,24 @@ int conv_pack_weights_batched(const PackJob *jobs_dev, uint32_t n_jobs, uint32_t
 
 int conv_wgrad_tc(const void *in, const void *grad_out, int dtype, uint32_t c_in, uint32_t K,
                   uint32_t c_out, const int32_t *out_nbr, uint32_t n_out, float *grad_weight,
-                  cudaStream_t stream);
+                  void *workspace, uint64_t workspace_bytes, cudaStream_t stream);
 
-// wgrad over the compacted pair lists of meb200_kernel_map_pairs (stage = 64 pairs).
+// Bytes of workspace that let wgrad over n_out rows use all its planned row splits (0: one split).
+// With less (or none) it uses fewer splits.  For a given workspace size the result never depends
+// on the order in which CTAs finish (the splits' partial sums are added in a fixed order).
+uint64_t conv_wgrad_workspace_bytes(uint32_t c_in, uint32_t c_out, uint32_t K, uint32_t n_out);
+
+// wgrad over the compacted pair lists of meb200_kernel_map_pairs.
 bool conv_wgrad_pairs_supported(int dtype, uint32_t c_in, uint32_t K, uint32_t c_out);
 int conv_wgrad_pairs(const void *in, const void *grad_out, int dtype, uint32_t c_in, uint32_t K,
                      uint32_t c_out, const int32_t *pairs_in, const int32_t *pairs_out,
                      const int32_t *seg_start, uint32_t n_chunks, uint32_t n_out,
-                     float *grad_weight, cudaStream_t stream);
+                     float *grad_weight, void *workspace, uint64_t workspace_bytes,
+                     cudaStream_t stream);
 
 // ---- network stem: rows of <= 4 channels, padded to 4 (8 bytes) ------------------------------
 // The layer is run as a K = 1 convolution over 4 * 16 ceil(K / 16) VIRTUAL channels (offset k,
-// channel c) -> 4 k + c: forward through k_conv_ts (STEM producers), wgrad through k_wgrad_stem.
+// channel c) -> 4 k + c, by the forward and wgrad kernels in their stem mode.
 bool conv_stem_tc_supported(int dtype, uint32_t K, uint32_t c_cols);
 int conv_stem_forward_tc(const void *A4, int dtype, uint32_t K, const void *Wv, uint32_t c_cols,
                          const int32_t *nbr, uint32_t n_rows, void *out, int out_dtype,
@@ -52,6 +57,6 @@ int conv_stem_forward_tc(const void *A4, int dtype, uint32_t K, const void *Wv, 
 bool conv_stem_wgrad_tc_supported(int dtype, uint32_t K, uint32_t c_out);
 int conv_stem_wgrad_tc(const void *in4, const void *grad_out, int dtype, uint32_t K,
                        uint32_t c_out, const int32_t *nbr, uint32_t n_rows, float *dWv,
-                       cudaStream_t stream);
+                       void *workspace, uint64_t workspace_bytes, cudaStream_t stream);
 
 }  // namespace meb200

@@ -3,8 +3,8 @@
 // MinkowskiEngine/MinkowskiNormalization.py:101-192; NCCL all-reduce per layer there).
 //
 // A SyncBN exchange moves 2C+1 doubles (<= 4 KB) per layer, forward and backward: ~140 latency-
-// bound NCCL launches per MinkUNet34C step, each with two cross-stream hand-offs (measured: 83 %
-// weak-scaling efficiency at 2 GPUs, profiles/r1_notes.md).  Here every rank keeps a buffer in
+// bound NCCL launches per MinkUNet34C step, each with two cross-stream hand-offs (a visible
+// share of a 2-GPU step).  Here every rank keeps a buffer in
 // symmetric memory (same layout on every GPU, peers' base pointers known); the LAST CTA of the
 // batch-norm reduction (csrc/batchnorm.cu, BnTail)
 //   1. publishes "my slot for call #seq is complete" by storing seq into each peer's flag word

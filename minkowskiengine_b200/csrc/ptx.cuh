@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the Blackwell (sm_100a) primitives the tensor-core kernels
-// use: mbarrier, cp.async, the async-proxy fence, TMEM allocation, tcgen05.mma/commit/ld.
+// Thin inline-PTX wrappers for the Hopper (sm_90a) primitives the tensor-core kernels use:
+// cp.async, the async-proxy fence, and warpgroup MMA (wgmma) with shared-memory descriptors.
 #pragma once
 #include <stdint.h>
 
@@ -10,65 +10,11 @@ __device__ __forceinline__ uint32_t smem_u32(const void *p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-// ---- mbarrier ---------------------------------------------------------------------
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_fence_init() {
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  while (!mbar_try_wait(bar, parity)) {
-  }
-}
-// Long waits (a role parked for most of a tile): try_wait with an explicit suspend-time hint, so
-// the hardware parks the warp instead of letting it poll.  (Measured, r2_run5: plain try_wait
-// loops — with or without __nanosleep between polls — returned every ~11 ns and the parked roles
-// issued 40 % of all instructions of the kernel, at higher scheduler priority than the producers.)
-__device__ __forceinline__ bool mbar_try_wait_hint(uint32_t bar, uint32_t parity, uint32_t ns) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity), "r"(ns)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_sleep(uint32_t bar, uint32_t parity, unsigned ns) {
-  while (!mbar_try_wait_hint(bar, parity, ns)) {
-  }
-}
-// default for waits that may last long: up to 20 us per suspension
-__device__ __forceinline__ void mbar_wait_park(uint32_t bar, uint32_t parity) {
-  mbar_wait_sleep(bar, parity, 20000u);
-}
-
 // ---- cp.async (LDGSTS) ------------------------------------------------------------
 // 16-byte global->shared copy; src_bytes = 0 zero-fills the destination (missing row).
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, uint32_t src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src),
                "r"(src_bytes)
-               : "memory");
-}
-// 4-byte variant (neighbour indices); src_bytes = 0 zero-fills
-__device__ __forceinline__ void cp_async4(uint32_t dst, const void *src, uint32_t src_bytes) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(src_bytes)
                : "memory");
 }
 // 8-byte variant (4-channel rows of a network stem); src_bytes = 0 zero-fills
@@ -83,165 +29,89 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
-// The mbarrier receives one arrival from this thread once all cp.async operations the thread
-// has issued so far have landed in shared memory (no wait_group / fence on the issue path;
-// the barrier's expected count must include these arrivals — ".noinc").
-__device__ __forceinline__ void cp_async_mbar_arrive(uint32_t bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
-}
-// generic-proxy shared-memory writes -> visible to the async proxy (tcgen05.mma operand reads)
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// ---- TMA (bulk tensor copies, async proxy) ------------------------------------------
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes)
-               : "memory");
+// ---- wgmma ------------------------------------------------------------------------
+// Shared-memory matrix descriptor, no swizzle: the operand is stored as 8 x 16-byte "core
+// matrices" (8 rows of 16 contiguous bytes).  lbo = byte distance between core matrices that
+// are adjacent along the reduction (K) axis, sbo = along the M / N axis.
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) |
+         ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32);
 }
-// 2-D tile load: box (c0.., c1..) of the tensor map -> swizzled shared memory.
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const void *tmap, int32_t c0, int32_t c1,
-                                            uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%2, %3}], [%4];" ::"r"(dst), "l"(tmap), "r"(c0), "r"(c1), "r"(bar)
-      : "memory");
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-// Row gather: four rows (r0..r3) x one box of columns starting at c0; rows outside the tensor
-// are zero-filled.  Lands as four consecutive rows of the (swizzled) destination tile.
-__device__ __forceinline__ void tma_gather4(uint32_t dst, const void *tmap, int32_t c0, int32_t r0,
-                                            int32_t r1, int32_t r2, int32_t r3, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%2, %3, %4, %5, %6}], [%7];" ::"r"(dst), "l"(tmap), "r"(c0), "r"(r0), "r"(r1),
-      "r"(r2), "r"(r3), "r"(bar)
-      : "memory");
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tma_prefetch_desc(const void *tmap) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
-// ---- TMEM / tcgen05 ---------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst),
-               "r"(ncols)
-               : "memory");
+// D[64 x N] (fp32, registers) += A[64 x 16] * B[16 x N], both operands in shared memory.
+// TA / TB = 1: the operand is stored MN-major (M / N contiguous), 0: K-major.
+// Accumulator layout per warp w of the warpgroup (rows 16w..16w+15), lane = 4g + t:
+//   d[4j + e] = D[16w + g + 8(e >> 1)][8j + 2t + (e & 1)]
+#define MEB_F8(d, o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), \
+    "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_16_bf16(float (&d)[8], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, "
+               "%8, %9, p, 1, 1, %11, %12;\n\t}"
+               : MEB_F8(d, 0) : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_16_f16(float (&d)[8], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, "
+               "%8, %9, p, 1, 1, %11, %12;\n\t}"
+               : MEB_F8(d, 0) : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_32_bf16(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+               "%16, %17, p, 1, 1, %19, %20;\n\t}"
+               : MEB_F8(d, 0), MEB_F8(d, 8) : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_32_f16(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+               "%16, %17, p, 1, 1, %19, %20;\n\t}"
+               : MEB_F8(d, 0), MEB_F8(d, 8) : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_64_bf16(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+               "%32, %33, p, 1, 1, %35, %36;\n\t}"
+               : MEB_F8(d, 0), MEB_F8(d, 8), MEB_F8(d, 16), MEB_F8(d, 24) : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
 }
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread for the whole CTA.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_64_f16(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+               "%32, %33, p, 1, 1, %35, %36;\n\t}"
+               : MEB_F8(d, 0), MEB_F8(d, 8), MEB_F8(d, 16), MEB_F8(d, 24) : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
 }
-// mbarrier arrives once every tcgen05 op issued so far by this thread has completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns: thread t of the warp gets lane (base_lane + t).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// One lane of a CONVERGED warp is elected (warp-uniform control flow around tcgen05 issue
-// lets the compiler keep descriptors in uniform registers).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-               : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ uint64_t pack_desc(uint32_t lo, uint32_t hi) {
-  uint64_t d;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(lo), "r"(hi));
-  return d;
-}
-// upper 32 bits of a shared-memory matrix descriptor (stride offset, version 1, swizzle mode)
-__host__ __device__ constexpr uint32_t umma_desc_hi(uint32_t sbo_bytes, uint32_t layout_type) {
-  return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14) | ((layout_type & 7u) << 29);
-}
-// lower 32 bits: start address and leading offset, both in 16-byte units
-__device__ __forceinline__ uint32_t umma_desc_lo(uint32_t saddr, uint32_t lbo_bytes) {
-  return ((saddr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
-}
-
-// ---- L2 eviction-priority hints (createpolicy + .L2::cache_hint) -----------------------
-// The plain `.L2::evict_*` qualifiers exist only for 256-bit vector accesses on sm_100; any
-// width works through a policy operand.
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-  uint64_t pol;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-  uint64_t pol;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
-__device__ __forceinline__ uint4 ldg128_hint(const void *p, uint64_t pol) {
-  uint4 v;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0, %1, %2, %3}, [%4], %5;"
-               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(pol));
-  return v;
-}
-__device__ __forceinline__ int32_t ldg32_hint(const int32_t *p, uint64_t pol) {
-  int32_t v;
-  asm volatile("ld.global.nc.L2::cache_hint.s32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
-  return v;
-}
-__device__ __forceinline__ void stg128_hint(void *p, uint4 v, uint64_t pol) {
-  asm volatile("st.global.L2::cache_hint.v4.u32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "r"(v.x),
-               "r"(v.y), "r"(v.z), "r"(v.w), "l"(pol) : "memory");
-}
-
-// ---- UMMA descriptors -------------------------------------------------------------
-// Shared-memory matrix descriptor, sm_100 format (version 1): start address, leading /
-// stride byte offsets in 16-byte units, swizzle mode in bits [61,64).
-//   layout_type: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B, 6 = SWIZZLE_32B
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes,
-                                              uint32_t sbo_bytes, uint32_t layout_type) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;  // descriptor version for Blackwell
-  d |= (uint64_t)(layout_type & 7u) << 61;
-  return d;
-}
-// Instruction descriptor of tcgen05.mma.kind::f16 with fp32 accumulation.
-//   fmt: 0 = f16, 1 = bf16;  a_mn / b_mn: 1 = operand is MN-major, 0 = K-major
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t fmt, uint32_t M, uint32_t N,
-                                                     uint32_t a_mn, uint32_t b_mn) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | (a_mn << 15) | (b_mn << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
+#undef MEB_F8
+template <int N, bool BF16, int TA, int TB>
+__device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t da, uint64_t db) {
+  static_assert(N == 16 || N == 32 || N == 64, "wgmma: N is 16, 32 or 64");
+  if constexpr (N == 16) {
+    if constexpr (BF16) wgmma_16_bf16<TA, TB>(d, da, db); else wgmma_16_f16<TA, TB>(d, da, db);
+  } else if constexpr (N == 32) {
+    if constexpr (BF16) wgmma_32_bf16<TA, TB>(d, da, db); else wgmma_32_f16<TA, TB>(d, da, db);
+  } else {
+    if constexpr (BF16) wgmma_64_bf16<TA, TB>(d, da, db); else wgmma_64_f16<TA, TB>(d, da, db);
+  }
 }
 
 }  // namespace ptx

@@ -1,292 +1,47 @@
-// Host-side launch configuration of the tcgen05 kernels (plain C++, no CUDA): tile counts,
-// TMEM accumulator packing and shared-memory pipeline depths.  Kept separate so it can be
-// unit-tested on a machine without a GPU (tests/test_tc_config.py).
+// Host-side launch configuration of the wgmma kernels (plain C++, no CUDA): stage widths,
+// shared-memory footprints and row splits.  Kept separate so it can be unit-tested on a machine
+// without a GPU (tests/test_tc_config.py).
 #pragma once
 #include <stdint.h>
 
 namespace meb200 {
 namespace tc {
 
-constexpr int kTileM = 128;
-constexpr int kMaxStages = 32;
-constexpr uint32_t kMaxLag = 16;
-constexpr uint32_t kTmemCols = 512;
-constexpr uint32_t kSmemBudget = 224 * 1024;            // of the 227 KB a CTA may opt in to
-constexpr uint32_t kBarBytes = (4 * kMaxStages + 4) * 8 + 16;
-constexpr int kWgRows = 64;                             // wgrad: reduction rows per stage
-constexpr uint32_t kBlkBytes = kWgRows * 128;           // wgrad: one 64-channel block of a stage
+constexpr uint32_t kStages = 4;             // cp.async ring depth (loads run 2 stages ahead)
+constexpr uint32_t kSmemLimit = 227 * 1024; // opt-in shared memory of one CTA on sm_90
+constexpr uint32_t kMaxCols = 256;          // accumulator columns of one CTA (one launch slice)
+constexpr uint32_t kFwdRows = 128;          // forward / dgrad: output rows per CTA (2 warpgroups)
+constexpr uint32_t kWgRows = 64;            // wgrad: reduction rows per stage
+constexpr uint32_t kWgChannels = 128;       // wgrad: input channels per CTA (2 warpgroups)
 
 inline uint32_t cdiv_u(uint64_t a, uint64_t b) { return (uint32_t)((a + b - 1) / b); }
 
-// Producers publish a stage with cp.async.mbarrier.arrive (the barrier fires when the copies
-// land), so every stage of a ring may be in flight.  `share` consecutive A stages use one B
-// stage; the number of A stages that can actually be in flight is limited by both rings:
-//   depth = min(nA, (nB - 1) * share + 1)
-// The search maximises the bytes of operand A in flight (depth * a_bytes).
-struct PipeCfg { uint32_t lag, nA, nB; };   // lag = effective depth (kept for reporting)
-inline PipeCfg pick_pipeline(uint32_t a_bytes, uint32_t b_bytes, uint32_t share, uint32_t budget) {
-  PipeCfg best{0, 0, 0};
-  uint64_t best_score = 0;
-  for (uint32_t nB = 2; nB <= (uint32_t)kMaxStages; ++nB) {
-    if ((uint64_t)nB * b_bytes + 2ull * a_bytes > budget) break;
-    uint32_t nA = (uint32_t)((budget - (uint64_t)nB * b_bytes) / a_bytes);
-    if (nA > (uint32_t)kMaxStages) nA = kMaxStages;
-    if (nA < 2) continue;
-    uint32_t depth = (nB - 1) * share + 1;
-    if (depth > nA) depth = nA;
-    uint64_t score = (uint64_t)depth * a_bytes;
-    if (score > best_score) { best_score = score; best = {depth, nA, nB}; }
-  }
-  return best;
+// forward / dgrad: reduction channels per stage (64, 32 or 16), 0 = unsupported
+inline uint32_t fwd_bk(uint32_t c_red) {
+  return c_red % 64 == 0 ? 64 : (c_red % 32 == 0 ? 32 : (c_red % 16 == 0 ? 16 : 0));
+}
+// one stage = A [128 rows x bk] + B [c_cols x bk], 16-bit elements; +1 KB for alignment
+inline uint32_t fwd_smem_bytes(uint32_t bk, uint32_t c_cols) {
+  return 1024 + kStages * (kFwdRows + c_cols) * bk * 2;
+}
+// one stage = A [64 rows x 128 channels] + B [64 rows x c_out]
+inline uint32_t wgrad_smem_bytes(uint32_t c_out) {
+  return 1024 + kStages * kWgRows * (kWgChannels + c_out) * 2;
 }
 
-// ---- forward / dgrad: out[r, 0:c_cols] over n_rows rows, reduction over c_red channels ----
-struct FwdCfg {
-  int bk;                 // channel-chunk width (64/32/16 -> 128B/64B/32B swizzle), 0 = unsupported
-  uint32_t cps;           // channel chunks per pipeline stage (one barrier round trip per stage)
-  uint32_t R;             // row tiles sharing one B slice (1, 2 or 4)
-  uint32_t n_super;       // super tiles of R*128 rows
-  uint32_t a_sub_bytes, b_sub_bytes;       // one chunk of A (128 rows) / of B (c_cols rows)
-  uint32_t a_stage_bytes, b_stage_bytes;   // cps chunks
-  PipeCfg pipe;
-  uint32_t smem_bytes;
-};
-constexpr uint32_t kRsScratchBytes = 10 * 128 * 8 + 64;  // register-staged kernel: per-warp compaction lists + counters
-
-inline FwdCfg fwd_config(uint32_t c_red, uint32_t c_cols, uint32_t n_rows, uint32_t max_stage_bytes = 32 * 1024,
-                         uint32_t extra_bytes = 0, uint32_t budget = kSmemBudget) {
-  FwdCfg c{};
-  uint32_t R = kTmemCols / (2 * c_cols);                // accumulator set is double buffered
-  R = R >= 4 ? 4 : (R >= 2 ? 2 : 1);
-  uint32_t tiles = cdiv_u(n_rows, kTileM);
-  while (R > 1 && R > tiles) R >>= 1;
-  c.R = R;
-  c.n_super = cdiv_u(tiles, R);
-  const int cands[3] = {64, 32, 16};
-  uint64_t best_score = 0;
-  for (int cand : cands) {
-    if (c_red % cand != 0) continue;
-    const uint32_t chunks = c_red / cand;
-    const uint32_t a_sub = kTileM * cand * 2;
-    const uint32_t b_sub = ((c_cols * cand * 2 + 1023) / 1024) * 1024;
-    for (uint32_t cps = chunks; cps >= 1; --cps) {
-      if (chunks % cps != 0 || (cps * a_sub > max_stage_bytes && cps > 1)) continue;
-      PipeCfg p = pick_pipeline(cps * a_sub, cps * b_sub, R, budget - kBarBytes - 1024 - extra_bytes);
-      if (p.lag < 3) continue;
-      // bytes of A in flight, with a mild preference for fat stages (fewer barrier round trips)
-      uint64_t score = (uint64_t)p.lag * cps * a_sub * 8 + (uint64_t)cps * a_sub;
-      if (score > best_score + best_score / 8) {
-        best_score = score;
-        c.pipe = p; c.bk = cand; c.cps = cps; c.a_sub_bytes = a_sub; c.b_sub_bytes = b_sub;
-        c.a_stage_bytes = cps * a_sub; c.b_stage_bytes = cps * b_sub;
-      }
-      break;  // the fattest feasible stage for this chunk width
-    }
-  }
-  c.smem_bytes = 1024 + c.pipe.nA * c.a_stage_bytes + c.pipe.nB * c.b_stage_bytes + kBarBytes + extra_bytes;
-  return c;
-}
-
-// ---- forward / dgrad with operand A in tensor memory (k_conv_ta) --------------------------
-// TMEM (512 columns): acc_sets x R accumulators of c_cols columns, then nA operand-A slots of
-// 16*nb columns (one stage = nb 32-channel blocks of a 128-row tile).  Shared memory holds only
-// the ring of packed-weight stages (nB x [c_cols x 32*nb channels]).
-struct TaCfg {
-  uint32_t nb;            // 32-channel blocks per stage (1..4); 0 = unsupported
-  int bk;                 // channel width of a B sub-tile (64 or 32)
-  uint32_t n_macro;       // stages per (tile, offset) = c_red / (32 nb)
-  uint32_t R, acc_sets, n_super, nA, nB;
-  uint32_t a_col0, b_sub_bytes, b_stage_bytes, smem_bytes;
-  uint32_t rs;            // row slots per producer thread's ring
-  uint32_t g;             // offsets per stage (narrow layers); 1 otherwise
-};
-#ifndef MEB_TS_GROUPS
-#define MEB_TS_GROUPS 3
-#endif
-constexpr uint32_t kTsGroupsCfg = MEB_TS_GROUPS;   // k_conv_ts: producer groups of 4 warps
-constexpr uint32_t kTsProducerWarpsCfg = 4 * kTsGroupsCfg;
-// counters, landing barriers (8 per warp), descriptors (8 x 128 B per warp), index rings
-// (4 stages x g offsets x 128 B per warp)
-inline uint32_t ts_tail_bytes(uint32_t g) {
-  return 64 + kTsProducerWarpsCfg * (8 * 8 + 8 * 32 * 4 + 4 * g * 32 * 4);
-}
-// One candidate: nb 32-channel blocks per stage, g offsets per stage.
-inline TaCfg ta_try(uint32_t c_red, uint32_t c_cols, uint32_t n_rows, uint32_t nb, uint32_t g,
-                    int force_R, int force_acc, uint32_t gi = 0) {
-  // gi: offsets whose neighbour indices one stage needs (index-ring rows); g unless stated
-  if (gi == 0) gi = g;
-  TaCfg c{};
-  c.g = g;
-  c.bk = (nb % 2 == 0 && (g == 1 || (32 * nb / g) % 64 == 0)) ? 64 : 32;
-  c.n_macro = g > 1 ? 1 : c_red / (32 * nb);
-  const uint32_t a_cols = 16 * nb;
-  const uint32_t tiles = cdiv_u(n_rows, kTileM);
-  uint32_t bestR = 0, bestAcc = 0;
-  for (uint32_t acc = 2; acc >= 1 && bestR == 0; --acc) {
-    if (force_acc && (int)acc != force_acc) continue;
-    for (uint32_t R = 4; R >= 1; R >>= 1) {
-      if (force_R && (int)R != force_R) continue;
-      if (R > 1 && R > tiles) continue;
-      // one A slot per producer group at least
-      if (acc * R * c_cols + kTsGroupsCfg * a_cols <= kTmemCols) { bestR = R; bestAcc = acc; break; }
-    }
-  }
-  if (bestR == 0) return c;
-  c.R = bestR; c.acc_sets = bestAcc;
-  c.n_super = cdiv_u(tiles, c.R);
-  c.a_col0 = c.acc_sets * c.R * c_cols;
-  c.nA = (kTmemCols - c.a_col0) / a_cols;
-  if (c.nA > 3 * kTsGroupsCfg) c.nA = 3 * kTsGroupsCfg;
-  c.nA = c.nA / kTsGroupsCfg * kTsGroupsCfg;   // a slot always belongs to the same producer group
-  if (c.nA < kTsGroupsCfg) return c;
-  c.b_sub_bytes = ((c_cols * (uint32_t)c.bk * 2 + 1023) / 1024) * 1024;
-  c.b_stage_bytes = (32 * nb / (uint32_t)c.bk) * c.b_sub_bytes;
-  // weights ring of 3 (2 if tight) stages, the rest of shared memory goes to the row rings
-  const uint32_t tail_bytes = ts_tail_bytes(gi);
-  if (tail_bytes + kBarBytes + 1024 >= kSmemBudget) return c;
-  const uint32_t budget = kSmemBudget - kBarBytes - 1024 - tail_bytes;
-  const uint32_t per_slot = kTsProducerWarpsCfg * nb * 512;     // bytes one more row slot costs
-  for (uint32_t nB = 3; nB >= 2; --nB) {
-    if (nB * c.b_stage_bytes + 5 * per_slot > budget) continue;
-    uint32_t rs = (budget - nB * c.b_stage_bytes) / per_slot - 1;   // one slot is the zero slot
-    if (rs > 8) rs = 8;
-    c.nB = nB; c.rs = rs;
-    c.smem_bytes = 1024 + nB * c.b_stage_bytes + (rs + 1) * per_slot + kBarBytes + tail_bytes;
-    c.nb = nb;
-    return c;
-  }
-  return c;
-}
-inline TaCfg ta_config(uint32_t c_red, uint32_t c_cols, uint32_t n_rows, int force_R = 0,
-                       int force_acc = 0) {
-  TaCfg none{};
-  if (c_red % 32 != 0 || c_cols % 16 != 0 || c_cols < 16 || c_cols > 256) return none;
-  // narrow layers: a stage spans g offsets so that it still carries 128 channels of reduction
-  if (c_red == 32) return ta_try(c_red, c_cols, n_rows, 4, 4, force_R, force_acc);
-  if (c_red == 64) return ta_try(c_red, c_cols, n_rows, 4, 2, force_R, force_acc);
-  // otherwise the fattest stage (most 32-channel blocks) whose weights + row rings fit
-  const uint32_t cands[4] = {4, 3, 2, 1};
-  for (uint32_t nb : cands) {
-    if (c_red % (32 * nb) != 0) continue;
-    TaCfg c = ta_try(c_red, c_cols, n_rows, nb, 1, force_R, force_acc);
-    if (c.nb != 0) return c;
-  }
-  return none;   // the caller falls back to k_conv_rs
-}
-
-// Network stem (rows of <= 4 channels, padded to 4 = 8 bytes): k_conv_ts<NB = 2, G = 0> treats the
-// layer as a K = 1 convolution over 4 * 16 * ceil(K / 16) virtual channels, 16 offsets per stage.
-constexpr uint32_t kStemNb = 2, kStemOffsetsPerStage = 8 * kStemNb;
-inline uint32_t stem_virtual_channels(uint32_t K) {
-  return cdiv_u(K, kStemOffsetsPerStage) * kStemOffsetsPerStage * 4;
-}
-inline TaCfg ta_stem_config(uint32_t K, uint32_t c_cols, uint32_t n_rows) {
-  TaCfg none{};
-  if (K == 0 || c_cols % 16 != 0 || c_cols < 16 || c_cols > 256) return none;
-  return ta_try(stem_virtual_channels(K), c_cols, n_rows, kStemNb, 1, 0, 0, kStemOffsetsPerStage);
-}
-
-// ---- wgrad: dW[K, c_in, c_out] reduced over n_out rows --------------------------------------
-struct WgCfg {
-  uint32_t mt_cta;        // 128-channel m-tiles of c_in per CTA (1 or 2); 0 = unsupported
-  uint32_t n_mtgroups, G, n_kgroups, blkA, blkB;
-  uint32_t a_stage_bytes, b_stage_bytes;
-  PipeCfg pipe;
-  uint32_t rows_per_split, n_splits;
-  uint32_t smem_bytes;
-};
-// First offset of k-group kg when K offsets are dealt to n_kgroups groups whose sizes differ
-// by at most one (the first K % n_kgroups groups get the extra offset).
-#ifdef __CUDACC__
-__host__ __device__
-#endif
-inline uint32_t kgroup_begin(uint32_t kg, uint32_t K, uint32_t n_kgroups) {
-  const uint32_t base = K / n_kgroups, rem = K % n_kgroups;
-  return kg * base + (kg < rem ? kg : rem);
-}
-inline WgCfg wgrad_config(uint32_t c_in, uint32_t c_out, uint32_t K, uint32_t n_out, uint32_t n_sms) {
-  WgCfg best{};
-  const uint32_t mt_total = cdiv_u(c_in, 128);
-  uint32_t mt_max = mt_total < kTmemCols / c_out ? mt_total : kTmemCols / c_out;
-  if (mt_max > 2) mt_max = 2;
-  for (uint32_t mt = mt_max; mt >= 1; --mt) {
-    WgCfg c{};
-    c.mt_cta = mt;
-    c.n_mtgroups = cdiv_u(mt_total, mt);
-    c.G = kTmemCols / (mt * c_out);
-    if (c.G > K) c.G = K;
-    if (c.G > 8) c.G = 8;
-    c.n_kgroups = cdiv_u(K, c.G);
-    c.blkA = mt * 2;
-    c.blkB = cdiv_u(c_out, 64);
-    c.a_stage_bytes = c.blkA * kBlkBytes;
-    c.b_stage_bytes = c.blkB * kBlkBytes;
-    c.pipe = pick_pipeline(c.a_stage_bytes, c.b_stage_bytes, c.G, kSmemBudget - kBarBytes - 1024);
-    if (c.pipe.lag > best.pipe.lag) best = c;
-    if (c.pipe.lag >= 3) break;
-  }
-  if (best.pipe.lag == 0) { best.mt_cta = 0; return best; }
-  // row slices: at most 2 full waves of CTAs (one CTA per SM; a third, nearly empty wave
-  // cost a third of the launch on the 96-channel layers), each slice a multiple of the stage
-  // height.  Offsets are dealt to the k-groups evenly (kgroup_begin), so CTAs differ by at
-  // most one offset of work.
-  uint32_t base = best.n_kgroups * best.n_mtgroups;
-  uint32_t want = (2u * n_sms) / base;
-  uint32_t max_splits = cdiv_u(n_out, 4 * kWgRows);
-  uint32_t splits = want < 1 ? 1 : (want > max_splits ? max_splits : want);
-  best.rows_per_split = cdiv_u(cdiv_u(n_out, splits), kWgRows) * kWgRows;
-  best.n_splits = cdiv_u(n_out, best.rows_per_split);
-  best.smem_bytes = 1024 + best.pipe.nA * best.a_stage_bytes + best.pipe.nB * best.b_stage_bytes + kBarBytes;
-  return best;
-}
-
-// ---- wgrad over compacted pair lists (k_wgrad_pairs) --------------------------------------
-// stage = 64 pairs: A = mt_cta*2 blocks of [64 rows][128 B] (this CTA's channel slice of the
-// gathered input rows), B = ceil(c_out/64) blocks (the matching dOut rows).
-struct WpCfg {
-  uint32_t mt_cta;        // 128-channel m-tiles per CTA (1 or 2); 0 = unsupported
-  uint32_t n_mtgroups, n_splits, blkB, n_stage, a_bytes, stage_bytes, acc_sets, smem_bytes;
-  uint32_t rw;            // pairs per stage: 64, or 32 when fewer than 6 stages of 64 would fit
-};
-inline WpCfg wgrad_pairs_config(uint32_t c_in, uint32_t c_out, uint32_t K, uint32_t n_chunks,
-                                uint32_t n_out, uint32_t n_sms) {
-  WpCfg c{};
-  if (c_out > 256 || c_out == 0 || n_chunks == 0 || (uint64_t)K * n_chunks > 2047) return c;
-  const uint32_t mt_total = cdiv_u(c_in, 128);
-  uint32_t mt = kTmemCols / c_out;
-  if (mt > 2) mt = 2;
-  if (mt > mt_total) mt = mt_total;
-  if (mt == 0) return c;
-  c.n_mtgroups = cdiv_u(mt_total, mt);
-  c.blkB = cdiv_u(c_out, 64);
-  c.acc_sets = 2 * mt * c_out <= kTmemCols ? 2 : 1;
-  const uint32_t tail = kBarBytes + 12 * 4 * 32 * 4 + (K * n_chunks + 1) * 4 + 64;   // barriers, index rings (12 warps x 4 stages x 32 indices), segment table
-  // 64 pairs per stage; 32 when that leaves fewer than two stages per producer group (a group
-  // with one stage cannot overlap its copies with the landing and the MMA of the previous one)
-  c.rw = 64;
-  for (;;) {
-    const uint32_t blk = c.rw * 128;
-    c.a_bytes = mt * 2 * blk;
-    c.stage_bytes = c.a_bytes + c.blkB * blk;
-    c.n_stage = (kSmemBudget - 1024 - tail) / c.stage_bytes;
-    if (c.n_stage >= 6 || c.rw == 32) break;
-    c.rw = 32;
-  }
-  if (c.n_stage > 12) c.n_stage = 12;
-  c.n_stage = c.n_stage / 3 * 3;       // a multiple of the 3 producer groups (slot ownership)
-  if (c.n_stage < 3) return c;
-  // row-range splits: two waves of CTAs at most, and enough stages per CTA to amortise its
-  // accumulator flush (mt*128 x c_out reductions into dW; ~one stage's time per 16 columns) on
-  // the estimate "a third of the K*n_out table entries are pairs"
-  const uint64_t est_stages = (uint64_t)K * n_out / (3 * 64) + 1;
-  uint32_t want = (2u * n_sms) / c.n_mtgroups;
-  if (want < 1) want = 1;
-  uint64_t by_work = est_stages / 8;
+// wgrad row splits: enough CTAs for two waves over (k, channel tile) pairs, but at least
+// 4 stages of work per CTA so the store of its 128 x c_out partial sums (and their later
+// ordered addition) stays amortised.
+// `stages` is the (estimated) number of 64-row stages one (k, channel tile) has in total.
+inline uint32_t wgrad_splits(uint32_t stages, uint32_t K, uint32_t m_tiles, uint32_t n_sms) {
+  const uint64_t base = (uint64_t)K * m_tiles;
+  uint64_t want = (2ull * n_sms + base - 1) / base;
+  uint64_t by_work = stages / 4;
   if (by_work < 1) by_work = 1;
-  c.n_splits = (uint32_t)(by_work < want ? by_work : want);
-  c.smem_bytes = 1024 + c.n_stage * c.stage_bytes + tail;
-  c.mt_cta = mt;
-  return c;
+  if (want > by_work) want = by_work;
+  if (want < 1) want = 1;
+  if (want > 65535) want = 65535;
+  return (uint32_t)want;
 }
 
 }  // namespace tc

@@ -1,4 +1,8 @@
-"""Shared test helpers: seeded inputs and oracle-side evaluation of one layer."""
+"""Shared test helpers: seeded inputs, oracle-side evaluation of one layer, stored results of the
+compiled reference (tests/golden/)."""
+import hashlib
+import os
+
 import numpy as np
 import torch
 
@@ -53,3 +57,27 @@ def oracle_conv_layer(in_coords, tensor_stride, kernel_size, stride, dilation, t
 def rel_err(a, b):
     a = np.asarray(a, np.float64); b = np.asarray(b, np.float64)
     return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
+
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+
+
+def golden(name):
+    """A results file of the compiled reference (written by tests/golden/make_reference_runs.py)."""
+    return np.load(os.path.join(GOLDEN, name))
+
+
+def digest(t):
+    """SHA-256 of a tensor's values in a fixed dtype per kind (int -> int64, float -> float32)."""
+    a = np.ascontiguousarray(np.asarray(t.detach().cpu() if torch.is_tensor(t) else t))
+    a = a.astype(np.int64) if a.dtype.kind in "iub" else a.astype(np.float32)
+    return np.frombuffer(hashlib.sha256(a.tobytes() + str(a.shape).encode()).digest(), np.uint8)
+
+
+def state_digest(module):
+    """Digest of a module's state_dict (parameters and buffers, in key order)."""
+    h = hashlib.sha256()
+    for k, v in module.state_dict().items():
+        h.update(k.encode())
+        h.update(digest(v).tobytes())
+    return np.frombuffer(h.digest(), np.uint8)

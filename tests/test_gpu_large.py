@@ -85,7 +85,7 @@ def test_cfg1_single_conv_bf16_100k(ME, cuda):
     wl = w.to(torch.bfloat16)
     before = _lib.tc_launch_count()
     y = backend._conv_forward(feats, wl, km, out_dtype=torch.float32)
-    assert _lib.tc_launch_count() > before, "forward did not take the tcgen05 path"
+    assert _lib.tc_launch_count() > before, "forward did not take the tensor-core path"
     ref = _torch_conv(feats, wl, km.out_nbr)
     assert float((y - ref).abs().max() / ref.abs().max()) < 1e-4
     # linearity: conv(a*X1 + X2) == a*conv(X1) + conv(X2) (fp32 output, exact bf16 inputs)
@@ -189,7 +189,7 @@ def test_cfg4_4d_conv_bf16_vs_oracle_20k(ME, cuda):
 
 
 def test_cfg4_4d_conv_bf16_full_size_properties(ME, cuda):
-    """configs[4] at full size (200k draws -> 131 897 coordinates, K = 81, C = 32): the tcgen05
+    """configs[4] at full size (200k draws -> 131 897 coordinates, K = 81, C = 32): the tensor-core
     path against an fp32 torch restatement on the device, and the adjoint identities."""
     from minkowskiengine_b200 import _lib, backend
     torch.backends.cuda.matmul.allow_tf32 = False
@@ -207,7 +207,7 @@ def test_cfg4_4d_conv_bf16_full_size_properties(ME, cuda):
     wl = w.bfloat16()
     before = _lib.tc_launch_count()
     y = backend._conv_forward(feats, wl, km, out_dtype=torch.float32)
-    assert _lib.tc_launch_count() > before, "4-D forward did not take the tcgen05 path"
+    assert _lib.tc_launch_count() > before, "4-D forward did not take the tensor-core path"
     ref = _torch_conv(feats, wl, km.out_nbr)
     assert float((y - ref).abs().max() / ref.abs().max()) < 1e-4
     dy = (torch.rand(n, 32, generator=g) - 0.5).bfloat16().to(cuda)

@@ -60,8 +60,8 @@ def test_stem_forward_and_wgrad(ME, cuda, dtype, cin, cout, n_in, n_out, K, dens
     (3, 96, 40000, 40001, 125, 0.2),     # many CTAs, ragged last tile / stage
 ])
 def test_stem_tensor_core_path(ME, cuda, dtype, cin, cout, n_in, n_out, K, density):
-    """The same layers through the tensor-core stem path (fp32 master weights: k_conv_ts with
-    8-byte rows forward, k_wgrad_stem backward) — must have launched tcgen05 kernels."""
+    """The same layers through the tensor-core stem path (fp32 master weights: the wgmma
+    kernels' stem mode forward and wgrad) — must have launched tensor-core kernels."""
     from minkowskiengine_b200 import backend, _lib
     lib = _lib.load()
     torch.backends.cuda.matmul.allow_tf32 = False

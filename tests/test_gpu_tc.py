@@ -1,4 +1,4 @@
-"""tcgen05 (tensor-core) convolution path: bf16 / fp16 operands, fp32 accumulation.
+"""wgmma (tensor-core) convolution path: bf16 / fp16 operands, fp32 accumulation.
 
 Parity definition for reduced-precision inputs (SURVEY.md §8a notes): the oracle is fed the
 SAME bf16/fp16-rounded features and weights; with fp32 accumulation the CUDA result then
@@ -113,7 +113,7 @@ def test_tc_wgrad_matches_fp32_reference(ME, cuda, dtype, cin, cout, n_in, n_out
     km = backend._KernelMap(nbr, torch.full((K, n_in), -1, dtype=torch.int32, device=cuda))
     before = _lib.tc_launch_count()
     _, gw = backend._conv_backward(feats, gout, w, km, need_in=False, need_w=True)
-    assert _lib.tc_launch_count() > before, "wgrad did not take the tcgen05 path"
+    assert _lib.tc_launch_count() > before, "wgrad did not take the tensor-core path"
     ref = torch.zeros(K, cin, cout, dtype=torch.float32, device=cuda)
     f32, g32 = feats.float(), gout.float()
     for k in range(K):
@@ -138,7 +138,7 @@ def test_tc_wgrad_matches_fp32_reference(ME, cuda, dtype, cin, cout, n_in, n_out
     (96, 96, 50000, 50000, 27),
 ])
 def test_ta_forward_and_dgrad_packed_weights(ME, cuda, dtype, cin, cout, n_in, n_out, K):
-    """fp32 master weights -> packed operand copies -> k_conv_ta (operand A in tensor memory):
+    """fp32 master weights -> packed operand copies -> k_conv_wg:
     forward over out_nbr and dgrad over in_nbr against the fp32 torch restatement."""
     from minkowskiengine_b200 import _lib, backend
     g = torch.Generator().manual_seed(cin * 1000 + cout + 7)
@@ -210,7 +210,7 @@ def test_pair_lists_match_table(ME, cuda, K, n, density, chunk, monkeypatch):
 
 
 def test_wgrad_pairs_many_chunks(ME, cuda, monkeypatch):
-    """k_wgrad_pairs walking several row chunks (small chunks forced) against the fp32 reference."""
+    """k_wgrad_wg walking several row chunks of the pair lists (small chunks forced) against the fp32 reference."""
     from minkowskiengine_b200 import backend
     monkeypatch.setattr(backend._KernelMap, "PAIR_CHUNK_ROWS", 4096)
     torch.backends.cuda.matmul.allow_tf32 = False
@@ -254,13 +254,9 @@ def test_batched_weight_packing_equals_single(ME, cuda):
 
     def check(k):
         got = backend._packed_weights(k, dtype)
-        ref, has_cp, has_tp = single(k)
+        ref = single(k)[0]
         assert torch.equal(got[0].flatten(), ref[0]) and torch.equal(got[1].flatten(), ref[1])
-        assert (got[2] is not None) == has_cp and (got[3] is not None) == has_tp
-        if has_cp:
-            assert torch.equal(got[2].flatten(), ref[2])
-        if has_tp:
-            assert torch.equal(got[3].flatten(), ref[3])
+        assert len(got) == 2              # the permuted copies are not built by the host
 
     for k in ks:            # first sight: packed one by one, registered
         check(k)

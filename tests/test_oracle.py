@@ -3,7 +3,8 @@
      transcribed from the reference's tests, file:line in each entry);
   2. against outputs of the compiled reference stored as fixtures (tests/golden/ref_*.npz,
      produced by tests/golden/make_fixtures.py);
-  3. live against oracle/_ref when it is built here (skipped otherwise)."""
+  3. against one strided convolution of the compiled reference on seeded inputs
+     (tests/golden/ref_live_conv.npz, produced by tests/golden/make_reference_runs.py)."""
 import glob
 import json
 import os
@@ -126,19 +127,11 @@ def test_oracle_matches_reference_transpose_fixture():
 
 
 def test_oracle_live_against_compiled_reference():
-    from oracle import ref
-    if not ref.available():
-        pytest.skip("oracle/_ref is not built in this checkout")
-    import torch
-    ME = ref.import_reference()
-    torch.manual_seed(3)
-    coords = torch.cat([torch.zeros(700, 1, dtype=torch.int32),
-                        torch.randint(-9, 9, (700, 3), dtype=torch.int32)], 1)
-    x = ME.SparseTensor(torch.rand(700, 4), coords)
-    conv = ME.MinkowskiConvolution(4, 6, kernel_size=3, stride=2, dimension=3)
-    y = conv(x)
-    oc, _ = O.stride_map_coords(x.C.numpy(), [1, 1, 1], [2, 2, 2])
-    assert (O.unique_rows(y.C.numpy()) == oc).all()
-    im, om = O.kernel_map(x.C.numpy(), y.C.numpy(), O.region_offsets(O.HYPER_CUBE, [3] * 3, [1] * 3, [1] * 3))
-    ref_out = O.conv_forward(x.F.numpy(), conv.kernel.detach().numpy(), im, om, len(y))
-    assert np.abs(ref_out - y.F.detach().numpy()).max() < 1e-5
+    """One strided convolution of the compiled reference on seeded inputs (stored in
+    tests/golden/ref_live_conv.npz by tests/golden/make_reference_runs.py)."""
+    f = np.load(os.path.join(GOLD, "ref_live_conv.npz"))
+    oc, _ = O.stride_map_coords(f["in_coords"], [1, 1, 1], [2, 2, 2])
+    assert (O.unique_rows(f["out_coords"]) == oc).all()
+    im, om = O.kernel_map(f["in_coords"], f["out_coords"], O.region_offsets(O.HYPER_CUBE, [3] * 3, [1] * 3, [1] * 3))
+    ref_out = O.conv_forward(f["in_feats"], f["kernel"], im, om, len(f["out_coords"]))
+    assert np.abs(ref_out - f["out_feats"]).max() < 1e-5

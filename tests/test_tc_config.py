@@ -1,6 +1,7 @@
-"""Host-side launch configuration of the tcgen05 kernels (csrc/tc_config.h), checked on CPU:
-every channel shape MinkUNet14/34C/... can produce must get a pipeline (lag >= 1) that fits in
-the 227 KB of shared memory a CTA may use and 512 TMEM columns."""
+"""Host-side launch configuration of the wgmma kernels (csrc/tc_config.h), checked on CPU:
+every channel shape MinkUNet14/34C/... can produce must get a stage width and a shared-memory
+ring that fit in the 227 KB a CTA may use on sm_90, and wgrad row splits that keep at most
+about two waves of CTAs on the 132 SMs of an H100 while giving every CTA enough work."""
 import os
 import subprocess
 
@@ -15,81 +16,26 @@ int main() {
   const unsigned chans[] = {16, 32, 48, 64, 96, 128, 160, 192, 256, 384, 512};
   const unsigned ncs[] = {16, 32, 48, 64, 96, 128, 192, 256};
   int bad = 0;
-  for (unsigned cr : chans) for (unsigned cc : ncs) for (unsigned rows : {1u, 129u, 5000u, 800000u}) {
-    FwdCfg f = fwd_config(cr, cc, rows);
-    bool ok = f.bk != 0 && f.pipe.lag >= 1 && f.smem_bytes <= 227 * 1024 && 2 * f.R * cc <= kTmemCols
-              && f.pipe.nA >= 3 && f.pipe.nB >= 2 && f.cps >= 1 && (cr / f.bk) % f.cps == 0
-              && f.a_stage_bytes == f.cps * f.a_sub_bytes && f.a_stage_bytes <= 32 * 1024
-              && 2 * f.pipe.nB * f.R >= f.pipe.nA + f.R - 1;  /* B-ring parity safety */
-    if (!ok) { printf("FWD BAD cr=%u cc=%u rows=%u bk=%d lag=%u\n", cr, cc, rows, f.bk, f.pipe.lag); ++bad; }
-    printf("fwd %u %u %u : bk=%d cps=%u R=%u depth=%u nA=%u nB=%u smem=%u\n", cr, cc, rows, f.bk, f.cps, f.R, f.pipe.lag, f.pipe.nA, f.pipe.nB, f.smem_bytes);
+  for (unsigned cr : chans) for (unsigned cc : ncs) {
+    const unsigned bk = fwd_bk(cr);
+    const unsigned smem = fwd_smem_bytes(bk, cc);
+    bool ok = (bk == 64 || bk == 32 || bk == 16) && cr % bk == 0 && smem <= kSmemLimit &&
+              (cr % 64 != 0 || bk == 64);
+    if (!ok) { printf("FWD BAD cr=%u cc=%u bk=%u smem=%u\n", cr, cc, bk, smem); ++bad; }
+    printf("fwd %u %u : bk=%u smem=%u\n", cr, cc, bk, smem);
   }
-  const unsigned cins[] = {16, 24, 32, 64, 96, 128, 192, 256, 384, 512};
-  for (unsigned ci : cins) for (unsigned co : ncs) for (unsigned K : {1u, 8u, 27u, 125u}) for (unsigned rows : {1u, 300u, 800000u}) {
-    WgCfg w = wgrad_config(ci, co, K, rows, 148);
-    bool ok = w.mt_cta != 0 && w.pipe.lag >= 1 && w.smem_bytes <= 227 * 1024 &&
-              w.G * w.mt_cta * co <= kTmemCols && w.G >= 1 && w.n_splits * w.rows_per_split >= rows
-              && w.pipe.nA >= 2 && w.pipe.nB >= 2;
-    /* one CTA per SM: never a third, nearly empty wave; k-groups cover K, sizes <= G, differ by <= 1 */
-    if (ok && w.n_splits > 1) ok = w.n_splits * w.n_kgroups * w.n_mtgroups <= 2 * 148;
-    if (ok) {
-      unsigned lo = K, hi = 0;
-      for (unsigned kg = 0; kg < w.n_kgroups; ++kg) {
-        unsigned g = kgroup_begin(kg + 1, K, w.n_kgroups) - kgroup_begin(kg, K, w.n_kgroups);
-        lo = g < lo ? g : lo; hi = g > hi ? g : hi;
-      }
-      ok = kgroup_begin(0, K, w.n_kgroups) == 0 && kgroup_begin(w.n_kgroups, K, w.n_kgroups) == K
-           && hi <= w.G && hi - lo <= 1 && lo >= 1;
-    }
-    if (w.mt_cta == 0 && co == 256 && K == 1) ok = true;  // declared unsupported -> SIMT fallback
-    if (!ok) { printf("WG BAD ci=%u co=%u K=%u rows=%u\n", ci, co, K, rows); ++bad; }
-    printf("wg %u %u %u %u : mt=%u G=%u lag=%u nA=%u nB=%u splits=%u smem=%u\n", ci, co, K, rows, w.mt_cta, w.G, w.pipe.lag, w.pipe.nA, w.pipe.nB, w.n_splits, w.smem_bytes);
+  if (fwd_bk(24) != 0 || fwd_bk(8) != 0) { printf("FWD BAD: widths not a multiple of 16 accepted\n"); ++bad; }
+  for (unsigned co : ncs) {
+    const unsigned smem = wgrad_smem_bytes(co);
+    if (smem > kSmemLimit) { printf("WG BAD co=%u smem=%u\n", co, smem); ++bad; }
+    printf("wg %u : smem=%u\n", co, smem);
   }
-  /* k_conv_ts: A slots in TMEM (a multiple of the 3 producer groups), accumulators, rings */
-  for (unsigned cr : chans) for (unsigned cc : ncs) for (unsigned rows : {1u, 129u, 5000u, 800000u}) {
-    TaCfg t = ta_config(cr, cc, rows);
-    if (cr % 32 != 0) { if (t.nb != 0) { printf("TA BAD (should be unsupported) cr=%u\n", cr); ++bad; } continue; }
-    if (t.nb == 0) { printf("ta %u %u %u : falls back to k_conv_rs\n", cr, cc, rows); continue; }
-    const unsigned a_cols = 16 * t.nb;
-    bool ok = t.nb * 32 * t.n_macro * (t.g > 1 ? 1 : 1) == (t.g > 1 ? t.nb * 32 : cr) &&
-              (t.g == 1 || cr * t.g == t.nb * 32) &&
-              t.acc_sets * t.R * cc + t.nA * a_cols <= kTmemCols && t.a_col0 == t.acc_sets * t.R * cc &&
-              t.nA >= 3 && t.nA % 3 == 0 && t.nB >= 2 && t.rs >= 4 && t.rs <= 8 &&
-              t.smem_bytes <= 227 * 1024 && t.b_stage_bytes == (32 * t.nb / t.bk) * t.b_sub_bytes &&
-              t.b_sub_bytes >= cc * t.bk * 2 && t.b_sub_bytes % 1024 == 0 &&
-              1024 + t.nB * t.b_stage_bytes + (t.rs + 1) * 12 * t.nb * 512 + kBarBytes + ts_tail_bytes(t.g) == t.smem_bytes;
-    if (!ok) { printf("TA BAD cr=%u cc=%u rows=%u nb=%u g=%u\n", cr, cc, rows, t.nb, t.g); ++bad; }
-    printf("ta %u %u %u : nb=%u g=%u bk=%d R=%u acc=%u nA=%u nB=%u rs=%u smem=%u\n", cr, cc, rows, t.nb, t.g, t.bk, t.R, t.acc_sets, t.nA, t.nB, t.rs, t.smem_bytes);
-  }
-  /* k_wgrad_pairs: ring a multiple of the 3 producer groups, accumulators within TMEM */
-  for (unsigned ci : cins) for (unsigned co : ncs) for (unsigned K : {1u, 8u, 27u, 125u}) for (unsigned rows : {1u, 300u, 800000u}) {
-    const unsigned chunks = (rows + 65535) / 65536;
-    WpCfg w = wgrad_pairs_config(ci, co, K, chunks, rows, 148);
-    if (K * chunks > 2047) { if (w.mt_cta != 0) { printf("WP BAD (too many segments)\n"); ++bad; } continue; }
-    bool ok = w.mt_cta >= 1 && w.mt_cta <= 2 && w.acc_sets * w.mt_cta * co <= kTmemCols &&
-              w.n_stage >= 3 && w.n_stage % 3 == 0 && w.smem_bytes <= 227 * 1024 &&
-              w.n_mtgroups * w.mt_cta * 128 >= ci && w.n_splits >= 1 &&
-              w.n_splits * w.n_mtgroups <= 2 * 148 + w.n_mtgroups &&
-              (w.rw == 64 || w.rw == 32) && w.a_bytes == w.mt_cta * 2 * w.rw * 128 &&
-              w.stage_bytes == w.a_bytes + w.blkB * w.rw * 128 && w.blkB * 64 >= co &&
-              (w.rw == 64 ? w.n_stage >= 6 : true);
-    if (!ok) { printf("WP BAD ci=%u co=%u K=%u rows=%u\n", ci, co, K, rows); ++bad; }
-    printf("wp %u %u %u %u : mt=%u groups=%u splits=%u stages=%u acc=%u smem=%u\n", ci, co, K, rows, w.mt_cta, w.n_mtgroups, w.n_splits, w.n_stage, w.acc_sets, w.smem_bytes);
-  }
-  /* network stem (k_conv_ts STEM): K = 1 layer over 4 * 16 ceil(K / 16) virtual channels, 16 offsets
-     per stage; index rings of 16 offsets per warp must fit beside the row rings */
-  for (unsigned K : {1u, 8u, 16u, 27u, 64u, 81u, 125u, 128u}) for (unsigned cc : {16u, 32u, 64u, 96u, 128u, 256u}) for (unsigned rows : {1u, 300u, 800000u}) {
-    TaCfg t = ta_stem_config(K, cc, rows);
-    const unsigned cv = stem_virtual_channels(K);
-    if (cv != 4 * 16 * ((K + 15) / 16)) { printf("STEM BAD virtual channels K=%u\n", K); ++bad; }
-    if (t.nb == 0) { printf("stem %u %u %u : unsupported\n", K, cc, rows); continue; }
-    bool ok = t.nb == kStemNb && t.g == 1 && t.bk == 64 && t.n_macro * 64 == cv &&
-              t.acc_sets * t.R * cc + t.nA * 16 * t.nb <= kTmemCols && t.nA >= 3 && t.nA % 3 == 0 &&
-              t.nB >= 2 && t.rs >= 4 && t.rs <= 8 && t.smem_bytes <= 227 * 1024 &&
-              1024 + t.nB * t.b_stage_bytes + (t.rs + 1) * 12 * t.nb * 512 + kBarBytes +
-                  ts_tail_bytes(kStemOffsetsPerStage) == t.smem_bytes;
-    if (!ok) { printf("STEM BAD K=%u cc=%u rows=%u\n", K, cc, rows); ++bad; }
-    printf("stem %u %u %u : n_macro=%u R=%u acc=%u nA=%u nB=%u rs=%u smem=%u\n", K, cc, rows, t.n_macro, t.R, t.acc_sets, t.nA, t.nB, t.rs, t.smem_bytes);
+  const unsigned sms = 132;
+  for (unsigned K : {1u, 8u, 27u, 125u}) for (unsigned mt : {1u, 2u, 4u}) for (unsigned st : {0u, 1u, 5u, 100u, 20000u}) {
+    const unsigned s = wgrad_splits(st, K, mt, sms);
+    const unsigned by_work = st / 4 > 1 ? st / 4 : 1;
+    bool ok = s >= 1 && s <= by_work && (s == 1 || (unsigned long long)(s - 1) * K * mt < 2ull * sms);
+    if (!ok) { printf("SPLIT BAD K=%u mt=%u stages=%u splits=%u\n", K, mt, st, s); ++bad; }
   }
   printf("bad=%d\n", bad);
   return bad != 0;
