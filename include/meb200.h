@@ -269,6 +269,66 @@ int meb200_pool_backward(const void *grad_out, int dtype, uint32_t n_in, uint32_
                          const int32_t *in_nbr, uint32_t K, uint32_t n_out, int mode,
                          const void *aux, void *grad_in, void *stream);
 
+/* ---- per-cloud grouping, segmented reduction, broadcast (reference: the origin map
+ *      coordinate_map_cpu.hpp:492-513,724-783; src/global_pooling_cpu.cpp;
+ *      src/broadcast_kernel.hpp).  A "segment" is the set of rows of one cloud: the rows whose
+ *      (batch, 0, ..., 0) is row s of the origin map.  Deterministic: no float atomics, no
+ *      atomics that decide an order, bit-identical results run to run. ----------------------- */
+#define MEB200_SEGMENT_TILE_ROWS 512 /* rows per reduction tile */
+
+#define MEB200_SEG_SUM 0
+#define MEB200_SEG_AVG 1
+#define MEB200_SEG_MAX 2
+
+#define MEB200_BCAST_ADD 0     /* reference BroadcastMode::ELEMENTWISE_ADDITON (src/types.hpp) */
+#define MEB200_BCAST_MUL 1     /* ELEMENTWISE_MULTIPLICATION */
+#define MEB200_BCAST_COPY 2    /* out = g[seg]  (sum / avg pooling backward, MinkowskiBroadcast) */
+#define MEB200_BCAST_MAXGRAD 3 /* out = g[seg] where argmax[seg] == i*C + c, else 0 */
+
+/* Groups the n rows of `coords` by cloud.  origin_coords / origin_table / origin_capacity: the
+ * origin map (B rows (b, 0, ..., 0) and its row-index table, as meb200_insert_and_map leaves
+ * them).  Outputs (DEVICE, no host synchronisation):
+ *   row_seg    int32 [n]    origin row of every row (-1: its batch index is not in the origin map)
+ *   order      int32 [n]    rows grouped by segment, ascending row order inside a segment
+ *   seg_start  int32 [B+1]  segment s is order[seg_start[s] .. seg_start[s+1])
+ *   tile_start int32 [B+1]  reduction tiles of segment s: [tile_start[s], tile_start[s+1]),
+ *                           ceil(rows / MEB200_SEGMENT_TILE_ROWS) each
+ * scratch: meb200_origin_group_scratch_bytes(n, B) bytes.  1 <= B <= 12288. */
+uint64_t meb200_origin_group_scratch_bytes(uint32_t n, uint32_t B);
+int meb200_origin_group(const int32_t *coords, uint32_t n, uint32_t ncols,
+                        const int32_t *origin_coords, const uint32_t *origin_table,
+                        uint32_t origin_capacity, uint32_t B, int32_t *row_seg, int32_t *order,
+                        int32_t *seg_start, int32_t *tile_start, void *scratch, void *stream);
+
+/* out[s, c] (fp32 [B, C]) = SUM / AVG / MAX over the rows i of segment s of a[i, c], or of
+ * a[i, c] * b[i, c] when b != NULL (SUM / AVG only).  Each tile of a segment stores fp32 partials
+ * into `workspace` (meb200_segment_workspace_bytes(n, C, B) bytes, 16-byte aligned) and a second
+ * pass adds them in tile order.  aux (may be NULL): SUM / AVG -> fp32 [B] row counts; MAX -> int32
+ * [B, C] flat index row*C + c of the maximum (lowest row on ties).  An empty segment gives 0 (and
+ * index -1).  a, b: [n, C] in `dtype`. */
+uint32_t meb200_segment_max_tiles(uint32_t n, uint32_t B);
+uint64_t meb200_segment_workspace_bytes(uint32_t n, uint32_t C, uint32_t B);
+int meb200_segment_reduce(const void *a, const void *b, int dtype, uint32_t n, uint32_t C,
+                          const int32_t *order, const int32_t *seg_start,
+                          const int32_t *tile_start, uint32_t B, int mode, float *out, void *aux,
+                          void *workspace, uint64_t workspace_bytes, void *stream);
+
+/* out[i, c] = x[i, c] op g[row_seg[i], c] for every row (fully written, no memset):
+ * op ADD / MUL; COPY: g[row_seg[i], c]; MAXGRAD: g[s, c] where argmax[s, c] == i*C + c, else 0
+ * (x unused for COPY / MAXGRAD).  x: [n, C] in `dtype`; g: fp32 [B, C]; argmax: int32 [B, C];
+ * out: [n, C] in out_dtype (= dtype or F32). */
+int meb200_broadcast(const void *x, int dtype, const float *g, const int32_t *argmax,
+                     const int32_t *row_seg, uint32_t n, uint32_t C, int op, void *out,
+                     int out_dtype, void *stream);
+
+/* out[i, c] = x[i, c] * g[s, c] + z[i, c] * h[s, c] + k[s, c] with s = row_seg[i]: the per-cloud
+ * affine pass of instance normalisation (forward: z = h = NULL; backward: z = the normalised
+ * features).  x, z, out: [n, C] in `dtype`; g, h, k: fp32 [B, C]; z / h (together) and k may be
+ * NULL. */
+int meb200_broadcast_fma(const void *x, const void *z, int dtype, const float *g, const float *h,
+                         const float *k, const int32_t *row_seg, uint32_t n, uint32_t C, void *out,
+                         void *stream);
+
 /* ---- batch normalisation over [n, C] feature rows (SURVEY.md 8(f) "next" row 1; the
  *      reference applies torch.nn.BatchNorm1d to `.F`: MinkowskiEngine/MinkowskiNormalization.py:51-99).
  *      C must be a multiple of 8.  sums: DEVICE double [2C]; statistics tensors fp32 [C]. ------ */

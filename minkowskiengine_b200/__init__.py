@@ -6,7 +6,8 @@ hot path of NVIDIA/MinkowskiEngine, behind the reference's own Python API.
     y = ME.MinkowskiConvolution(64, 128, kernel_size=3, stride=2, dimension=3).cuda()(x)
 
 Scope (SURVEY.md §8): SparseTensor / CoordinateManager / kernel maps, MinkowskiConvolution,
-MinkowskiConvolutionTranspose, local pooling, and the thin torch wrappers MinkUNet needs.
+MinkowskiConvolutionTranspose, local and global pooling, broadcast, batch and instance
+normalisation, and the thin torch wrappers MinkUNet and the ResNet classifiers need.
 CUDA tensors only; all device work runs in csrc/libmeb200.so (include/meb200.h).
 """
 __version__ = "0.1.0"
@@ -28,9 +29,15 @@ from .coordinate_manager import (CoordinateManager, CoordsManager, set_gpu_alloc
 from .convolution import (MinkowskiConvolution, MinkowskiConvolutionFunction,
                           MinkowskiConvolutionTranspose, MinkowskiConvolutionTransposeFunction,
                           MinkowskiGenerativeConvolutionTranspose)
-from .pooling import (MinkowskiAvgPooling, MinkowskiLocalPoolingFunction, MinkowskiMaxPooling,
+from .pooling import (MinkowskiAvgPooling, MinkowskiGlobalAvgPooling, MinkowskiGlobalMaxPooling,
+                      MinkowskiGlobalPooling, MinkowskiGlobalPoolingFunction,
+                      MinkowskiGlobalSumPooling, MinkowskiLocalPoolingFunction, MinkowskiMaxPooling,
                       MinkowskiSumPooling)
-from .normalization import MinkowskiBatchNorm, MinkowskiSyncBatchNorm, fused_bn_relu
+from .broadcast import (MinkowskiBroadcast, MinkowskiBroadcastAddition,
+                        MinkowskiBroadcastConcatenation, MinkowskiBroadcastFunction,
+                        MinkowskiBroadcastMultiplication)
+from .normalization import (MinkowskiBatchNorm, MinkowskiInstanceNorm,
+                            MinkowskiInstanceNormFunction, MinkowskiSyncBatchNorm, fused_bn_relu)
 from .nonlinearity import *  # noqa: F401,F403
 from .ops import MinkowskiLinear, cat
 from . import modules, utils  # noqa: F401

@@ -14,6 +14,8 @@ LIB_PATH = os.path.join(_HERE, "csrc", os.environ.get("MEB200_LIB", "libmeb200.s
 OK = 0
 F32, BF16, F16 = 0, 1, 2
 POOL_SUM, POOL_AVG, POOL_MAX = 0, 1, 2
+SEG_SUM, SEG_AVG, SEG_MAX = 0, 1, 2
+BCAST_ADD, BCAST_MUL, BCAST_COPY, BCAST_MAXGRAD = 0, 1, 2, 3
 
 _u32, _u64, _i32, _vp = C.c_uint32, C.c_uint64, C.c_int, C.c_void_p
 
@@ -61,6 +63,15 @@ PROTOTYPES = {
     "meb200_pool_forward": (_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _u32, _i32, _vp, _vp, _vp]),
     "meb200_pool_backward": (_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _u32, _i32, _vp, _vp,
                                     _vp]),
+    "meb200_origin_group_scratch_bytes": (_u64, [_u32, _u32]),
+    "meb200_origin_group": (_i32, [_vp, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp,
+                                   _vp]),
+    "meb200_segment_max_tiles": (_u32, [_u32, _u32]),
+    "meb200_segment_workspace_bytes": (_u64, [_u32, _u32, _u32]),
+    "meb200_segment_reduce": (_i32, [_vp, _vp, _i32, _u32, _u32, _vp, _vp, _vp, _u32, _i32, _vp, _vp,
+                                     _vp, _u64, _vp]),
+    "meb200_broadcast": (_i32, [_vp, _i32, _vp, _vp, _vp, _u32, _u32, _i32, _vp, _i32, _vp]),
+    "meb200_broadcast_fma": (_i32, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _u32, _u32, _vp, _vp]),
     "meb200_bn_workspace_bytes": (_u64, []),
     "meb200_bn_forward_train": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _vp, _i32, C.c_float,
                                        C.c_float, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -17,7 +17,7 @@ import weakref
 import torch
 
 from . import _lib
-from .enums import MinkowskiAlgorithm, PoolingMode, RegionType
+from .enums import BroadcastMode, MinkowskiAlgorithm, PoolingMode, RegionType
 from .kernel_generator import region_offsets
 
 ERROR_MAP_NOT_FOUND = "CoordinateMap not found"  # reference: src/errors.hpp:33
@@ -314,6 +314,9 @@ class CoordinateMapManagerGPU_c10:
         self._km_requests = []  # ... in order: the prediction for the next manager
         self._replaying = False
         self._hint_ncols = None
+        self._inserted = []     # keys of the maps made by insert_and_map, in order
+        self._origin_covers = 0  # ... how many of them the origin map was built from
+        self._groupings = {}    # map key -> _OriginGrouping
         _lib.load()             # fail at construction if the native library is missing
 
     # -- keys ------------------------------------------------------------------------
@@ -369,6 +372,7 @@ class CoordinateMapManagerGPU_c10:
         cmap, unique_index, inverse_map = _CoordinateMap.build(coordinates, ts)
         first = not self._maps
         self._maps[key] = cmap
+        self._inserted.append(key)
         if first:
             self._chain_tip = key
             self._hint_ncols = cmap.ncols
@@ -670,6 +674,87 @@ class CoordinateMapManagerGPU_c10:
         in_map, out_map = self._get(ik), self._get(ok)
         return self._stride_pairs(ik, ok, in_map, out_map)
 
+    # -- origin map and per-cloud grouping ---------------------------------------------
+    def _origin_key(self, ncols):
+        return (tuple([0] * (ncols - 1)), "")
+
+    def _origin(self):
+        """reference: coordinate_map_manager.cpp:474-508.  The origin map holds one row
+        (b, 0, ..., 0) per batch index of the inserted maps, in ASCENDING batch order; built once
+        (the one host read is its row count B) and cached under the key ([0]*D, "")."""
+        _assert(len(self._inserted) > 0, "No coordinate map found")
+        ncols = self._maps[self._inserted[0]].ncols
+        key = self._origin_key(ncols)
+        if key in self._maps:
+            return key
+        lib = _lib.load()
+        batch = torch.cat([self._maps[k].coords[:, 0] for k in self._inserted])
+        cand = torch.zeros((batch.numel(), ncols), dtype=torch.int32, device=batch.device)
+        cand[:, 0] = batch
+        cmap, _, _ = _CoordinateMap.build(cand, key[0])
+        # ascending batch index: rebuild the table over the sorted rows
+        coords = cmap.coords[torch.argsort(cmap.coords[:, 0])].contiguous()
+        table = torch.empty(cmap.capacity, dtype=torch.int32, device=coords.device)
+        _lib.check(lib.meb200_map_build_table(_lib.ptr(coords), coords.shape[0], ncols,
+                                              _lib.ptr(table), cmap.capacity,
+                                              _lib.current_stream()))
+        self._maps[key] = _CoordinateMap(coords, table, cmap.capacity, key[0])
+        self._origin_covers = len(self._inserted)
+        return key
+
+    def origin(self):
+        k = self._origin()
+        return CoordinateMapKey(list(k[0]), k[1])
+
+    def origin_map_size(self):
+        return self._maps[self._origin()].size
+
+    def _origin_grouping(self, in_key):
+        """Rows of map `in_key` grouped by cloud (cached per map, like kernel maps)."""
+        ik = self._k(in_key)
+        grp = self._groupings.get(ik)
+        if grp is not None:
+            return grp
+        _assert(ik in self._maps, ERROR_MAP_NOT_FOUND)
+        okey = self._origin()
+        omap, imap = self._maps[okey], self._maps[ik]
+        _assert(imap.ncols == omap.ncols, "coordinate size mismatch")
+        lib = _lib.load()
+        n, B, dev = imap.size, omap.size, imap.coords.device
+        grp = _OriginGrouping()
+        grp.n, grp.B = n, B
+        grp.row_seg = torch.empty(n, dtype=torch.int32, device=dev)
+        grp.order = torch.empty(n, dtype=torch.int32, device=dev)
+        starts = torch.empty((2, B + 1), dtype=torch.int32, device=dev)
+        grp.seg_start, grp.tile_start = starts[0], starts[1]
+        scratch = torch.empty(int(lib.meb200_origin_group_scratch_bytes(n, B)), dtype=torch.uint8,
+                              device=dev)
+        _lib.check(lib.meb200_origin_group(
+            _lib.ptr(imap.coords), n, imap.ncols, _lib.ptr(omap.coords), _lib.ptr(omap.table),
+            omap.capacity, B, _lib.ptr(grp.row_seg), _lib.ptr(grp.order), _lib.ptr(grp.seg_start),
+            _lib.ptr(grp.tile_start), _lib.ptr(scratch), _lib.current_stream()))
+        if len(self._inserted) > self._origin_covers:
+            # a map inserted after the origin map was built may hold batch indices it lacks: the
+            # one case that needs a host read (maps derived from covered ones share their batches)
+            _assert(int(grp.seg_start[B].item()) == n,
+                    "the coordinate map holds batch indices that are not in the origin map")
+        self._groupings[ik] = grp
+        return grp
+
+    def origin_map(self, key):
+        """reference: origin_map_th, coordinate_map_manager.cpp:828-885 -> (batch_indices int64
+        [B], [row indices (int64) of batch index b for b in 0..max batch index])."""
+        grp = self._origin_grouping(key)
+        okey = self._origin()
+        batch = self._maps[okey].coords[:, 0].long()
+        starts = grp.seg_start.tolist()
+        rows = [torch.empty(0, dtype=torch.int64, device=batch.device)
+                for _ in range(int(batch.max().item()) + 1 if batch.numel() else 0)]
+        order = grp.order.long()
+        for s, b in enumerate(batch.tolist()):
+            rows[b] = order[starts[s]:starts[s + 1]]
+        return batch, rows
+
     def __repr__(self):
         lines = [f"\t{list(k[0])}{':' + k[1] if k[1] else ''}:\tCoordinateMapGPU:{m.size}x{m.ncols}"
                  for k, m in self._maps.items()]
@@ -685,6 +770,19 @@ def _cell_table(ksize):
 
 
 CoordinateMapManagerGPU_default = CoordinateMapManagerGPU_c10
+
+
+class _OriginGrouping:
+    """The rows of one coordinate map grouped by cloud (meb200_origin_group): segment s = the rows
+    of origin row s, i.e. of the s-th smallest batch index."""
+
+    __slots__ = ("n", "B", "row_seg", "order", "seg_start", "tile_start", "_counts")
+
+    def counts(self):
+        """fp32 [B] rows per cloud (device; exact up to 2^24 rows)."""
+        if getattr(self, "_counts", None) is None:
+            self._counts = (self.seg_start[1:] - self.seg_start[:-1]).float()
+        return self._counts
 
 
 # ----------------------------------------------------------------------------------------
@@ -1160,3 +1258,150 @@ def LocalPoolingBackwardGPU(in_feat, grad_out_feat, num_nonzero, kernel_size, ke
         km.K, km.n_out, mode, _lib.ptr(num_nonzero) if num_nonzero.numel() else None,
         _lib.ptr(grad_in), _lib.current_stream()))
     return grad_in
+
+
+# ---- global pooling and broadcast over the origin map ------------------------------------------
+_GLOBAL_CODE = {PoolingMode.GLOBAL_SUM_POOLING_DEFAULT: _lib.SEG_SUM,
+                PoolingMode.GLOBAL_SUM_POOLING_KERNEL: _lib.SEG_SUM,
+                PoolingMode.GLOBAL_SUM_POOLING_PYTORCH_INDEX: _lib.SEG_SUM,
+                PoolingMode.GLOBAL_AVG_POOLING_DEFAULT: _lib.SEG_AVG,
+                PoolingMode.GLOBAL_AVG_POOLING_KERNEL: _lib.SEG_AVG,
+                PoolingMode.GLOBAL_AVG_POOLING_PYTORCH_INDEX: _lib.SEG_AVG,
+                PoolingMode.GLOBAL_MAX_POOLING_DEFAULT: _lib.SEG_MAX,
+                PoolingMode.GLOBAL_MAX_POOLING_KERNEL: _lib.SEG_MAX,
+                PoolingMode.GLOBAL_MAX_POOLING_PYTORCH_INDEX: _lib.SEG_MAX}
+_BCAST_CODE = {BroadcastMode.ELEMENTWISE_ADDITON: _lib.BCAST_ADD,
+               BroadcastMode.ELEMENTWISE_MULTIPLICATION: _lib.BCAST_MUL}
+
+
+def _segment_reduce(a, grp, mode, b=None, aux=None):
+    """fp32 [B, C] per-cloud SUM / AVG / MAX of a (or of a * b) over the rows of `grp`."""
+    lib = _lib.load()
+    n, C = a.shape
+    out = torch.empty((grp.B, C), dtype=torch.float32, device=a.device)
+    nbytes = int(lib.meb200_segment_workspace_bytes(n, C, grp.B))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=a.device)
+    _lib.check(lib.meb200_segment_reduce(
+        _lib.ptr(a), _lib.ptr(b), _lib.dtype_code(a.dtype), n, C, _lib.ptr(grp.order),
+        _lib.ptr(grp.seg_start), _lib.ptr(grp.tile_start), grp.B, mode, _lib.ptr(out),
+        _lib.ptr(aux), _lib.ptr(ws), nbytes, _lib.current_stream()))
+    return out
+
+
+def _broadcast(x, g32, grp, op, out_dtype=None, argmax=None, n=None, C=None):
+    """[n, C] x op g32[segment of the row] (g32: fp32 [B, C])."""
+    lib = _lib.load()
+    if x is not None:
+        n, C = x.shape
+    out_dtype = out_dtype or x.dtype
+    out = torch.empty((n, C), dtype=out_dtype, device=g32.device)
+    code = _lib.dtype_code(x.dtype if x is not None else out_dtype)
+    _lib.check(lib.meb200_broadcast(
+        _lib.ptr(x), code, _lib.ptr(g32), _lib.ptr(argmax), _lib.ptr(grp.row_seg), n, C, op,
+        _lib.ptr(out), _lib.dtype_code(out_dtype), _lib.current_stream()))
+    return out
+
+
+def _broadcast_fma(x, g32, grp, z=None, h32=None, k32=None):
+    """x * g32[s] + z * h32[s] + k32[s] per row (s = the row's cloud), in x's dtype."""
+    lib = _lib.load()
+    n, C = x.shape
+    out = torch.empty_like(x)
+    _lib.check(lib.meb200_broadcast_fma(
+        _lib.ptr(x), _lib.ptr(z), _lib.dtype_code(x.dtype), _lib.ptr(g32), _lib.ptr(h32),
+        _lib.ptr(k32), _lib.ptr(grp.row_seg), n, C, _lib.ptr(out), _lib.current_stream()))
+    return out
+
+
+def _f32c(t):
+    return t if (t.dtype == torch.float32 and t.is_contiguous()) else t.float().contiguous()
+
+
+def _check_glob(manager, in_feat, glob_feat, glob_key):
+    _assert(glob_feat.is_cuda, "in_feat_glob must be CUDA (this backend has no CPU path)")
+    _assert(glob_feat.dim() == 2, "Invalid in_feat_glob.dim():", glob_feat.dim())
+    _assert(manager.exists(glob_key), ERROR_MAP_NOT_FOUND)
+    B = manager.origin_map_size()
+    _assert(glob_feat.size(0) == B, "Invalid in_feat_glob size", glob_feat.size(0), "!=", B)
+    _assert(in_feat.size(1) == glob_feat.size(1), "Invalid feature sizes", in_feat.size(1), "!=",
+            glob_feat.size(1))
+    _assert(in_feat.dtype == glob_feat.dtype, "Incompatible scalar_type. Use the same float type "
+            "for both in_feat and in_feat_glob.")
+
+
+def GlobalPoolingForwardGPU(in_feat, pooling_mode, in_key, out_key, manager):
+    """reference: GlobalPoolingForwardCPU src/global_pooling_cpu.cpp:43-200 -> (out_feat [B, C],
+    num_nonzero [B] (sum / avg, feature dtype) | max_index int32 [B, C] (flat row*C + c)).
+    Mutates `out_key` (-> the origin key) when it is unset.  All nine GLOBAL_* modes are accepted;
+    the _DEFAULT / _KERNEL / _PYTORCH_INDEX variants select a strategy in the reference, not a
+    result, and run the same kernels here."""
+    _check_feats(in_feat, manager, in_key)
+    _assert(pooling_mode in _GLOBAL_CODE, "Invalid pooling mode", pooling_mode)
+    okey = manager._origin()
+    if not out_key.is_key_set():
+        out_key.set_key(list(okey[0]), okey[1])
+    grp = manager._origin_grouping(in_key)
+    mode = _GLOBAL_CODE[pooling_mode]
+    if mode == _lib.SEG_MAX:
+        aux = torch.empty((grp.B, in_feat.size(1)), dtype=torch.int32, device=in_feat.device)
+    else:
+        aux = torch.empty(grp.B, dtype=torch.float32, device=in_feat.device)
+    out = _segment_reduce(in_feat, grp, mode, aux=aux)
+    if mode != _lib.SEG_MAX:
+        aux = aux.to(in_feat.dtype)
+    return out.to(in_feat.dtype), aux
+
+
+def GlobalPoolingBackwardGPU(in_feat, grad_out_feat, num_nonzero, pooling_mode, in_key, out_key,
+                             manager):
+    """reference: GlobalPoolingBackwardCPU src/global_pooling_cpu.cpp:221-330.  The average's
+    divisor is the exact per-cloud row count of the grouping (num_nonzero may be rounded in
+    bf16 / fp16); the max gradient goes to the row max_index names, whatever the cloud count."""
+    _check_feats(in_feat, manager, in_key)
+    _assert(pooling_mode in _GLOBAL_CODE, "Invalid pooling mode", pooling_mode)
+    _assert(manager.exists(out_key), ERROR_MAP_NOT_FOUND)
+    grp = manager._origin_grouping(in_key)
+    _assert(grad_out_feat.dim() == 2 and grad_out_feat.size(0) == grp.B,
+            "Invalid grad_out size", tuple(grad_out_feat.shape))
+    _assert(in_feat.size(1) == grad_out_feat.size(1), "Input feature size and kernel size mismatch")
+    _assert(in_feat.dtype == grad_out_feat.dtype, "type mismatch")
+    mode = _GLOBAL_CODE[pooling_mode]
+    g = _f32c(grad_out_feat)
+    if mode == _lib.SEG_MAX:
+        _assert(num_nonzero.dtype == torch.int32 and num_nonzero.shape == grad_out_feat.shape,
+                "max_index must be int32 [B, C]")
+        return _broadcast(None, g, grp, _lib.BCAST_MAXGRAD, in_feat.dtype,
+                          argmax=num_nonzero.contiguous(), n=grp.n, C=in_feat.size(1))
+    if mode == _lib.SEG_AVG:
+        g = (g / grp.counts().clamp(min=1.0)[:, None]).contiguous()
+    return _broadcast(None, g, grp, _lib.BCAST_COPY, in_feat.dtype, n=grp.n, C=in_feat.size(1))
+
+
+def BroadcastForwardGPU(in_feat, in_feat_glob, broadcast_mode, in_key, glob_key, manager):
+    """reference: BroadcastForwardCPU src/broadcast_cpu.cpp:44-90:
+    out[i] = in_feat[i] + / * in_feat_glob[cloud of i]."""
+    _check_feats(in_feat, manager, in_key)
+    _assert(broadcast_mode in _BCAST_CODE, "Invalid broadcast mode", broadcast_mode)
+    _check_glob(manager, in_feat, in_feat_glob, glob_key)
+    grp = manager._origin_grouping(in_key)
+    return _broadcast(in_feat, _f32c(in_feat_glob), grp, _BCAST_CODE[broadcast_mode])
+
+
+def BroadcastBackwardGPU(in_feat, in_feat_glob, grad_out_feat, broadcast_mode, in_key, glob_key,
+                         manager):
+    """reference: BroadcastBackwardCPU src/broadcast_cpu.cpp:92-150 (broadcast_kernel.hpp):
+    add: dx = dy, dg[b] = sum_{i in b} dy;  mul: dx = dy * g[b(i)], dg[b] = sum_{i in b} dy * x."""
+    _check_feats(in_feat, manager, in_key)
+    _assert(broadcast_mode in _BCAST_CODE, "Invalid broadcast mode", broadcast_mode)
+    _check_glob(manager, in_feat, in_feat_glob, glob_key)
+    grad_out_feat = grad_out_feat.contiguous()
+    _assert(grad_out_feat.shape == in_feat.shape and grad_out_feat.dtype == in_feat.dtype,
+            "Incompatible grad_out_feat")
+    grp = manager._origin_grouping(in_key)
+    if broadcast_mode == BroadcastMode.ELEMENTWISE_ADDITON:
+        grad_in = grad_out_feat
+        grad_glob = _segment_reduce(grad_out_feat, grp, _lib.SEG_SUM)
+    else:
+        grad_in = _broadcast(grad_out_feat, _f32c(in_feat_glob), grp, _lib.BCAST_MUL)
+        grad_glob = _segment_reduce(grad_out_feat, grp, _lib.SEG_SUM, b=in_feat)
+    return grad_in, grad_glob.to(in_feat_glob.dtype)

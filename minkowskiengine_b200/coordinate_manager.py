@@ -131,6 +131,20 @@ class CoordinateManager:
             convert_to_int_list(stride, self.D), convert_to_int_list(dilation, self.D),
             region_type, region_offset, is_transpose, is_pool)
 
+    def origin(self) -> CoordinateMapKey:
+        """Key of the origin map: one row (b, 0, ..., 0) per batch index, ascending
+        (reference: MinkowskiCoordinateManager.py:270)."""
+        return self._manager.origin()
+
+    def origin_map(self, key: CoordinateMapKey):
+        """(batch_indices int64 [B], [row indices of batch index b, b = 0..max batch index])
+        (reference: MinkowskiCoordinateManager.py:423)."""
+        return self._manager.origin_map(key)
+
+    def origin_map_size(self) -> int:
+        """Number of clouds B (rows of the origin map)."""
+        return self._manager.origin_map_size()
+
     def stride_map(self, in_key: CoordinateMapKey, stride_key: CoordinateMapKey):
         return self._manager.stride_map(in_key, stride_key)
 

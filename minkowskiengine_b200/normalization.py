@@ -345,3 +345,79 @@ class MinkowskiSyncBatchNorm(MinkowskiBatchNorm):
             module_output.add_module(name, cls.convert_sync_batchnorm(child, process_group))
         del module
         return module_output
+
+
+class MinkowskiInstanceNormFunction(torch.autograd.Function):
+    """Per-cloud normalisation (reference: MinkowskiNormalization.py:194-310), composed from the
+    native per-cloud reduction and broadcast as the reference composes global average pooling and
+    broadcast.  Statistics stay fp32 and the centred features are kept in fp32, so a bf16 / fp16
+    output carries one rounding:
+        mean = avg(x),  var = avg((x - mean)^2),  inv_std = 1 / sqrt(var + 1e-8),
+        y = x * inv_std - mean * inv_std
+    backward (reference :254-310):
+        dx = (dy - y * avg(dy * y) - avg(dy)) * inv_std"""
+
+    @staticmethod
+    def forward(ctx, in_feat, in_coords_key, glob_coords_key=None, coords_manager=None,
+                gpooling_mode=None):
+        from . import backend as _C
+        mgr = coords_manager._manager
+        in_feat = in_feat.contiguous()
+        _C._check_feats(in_feat, mgr, in_coords_key)
+        grp = mgr._origin_grouping(in_coords_key)
+        mean = _C._segment_reduce(in_feat, grp, _lib.SEG_AVG)
+        centered = _C._broadcast(in_feat, (-mean).contiguous(), grp, _lib.BCAST_ADD, torch.float32)
+        var = _C._segment_reduce(centered, grp, _lib.SEG_AVG, b=centered)
+        del centered
+        inv_std = torch.rsqrt(var + 1e-8)
+        norm_feat = _C._broadcast_fma(in_feat, inv_std, grp, k32=(-mean * inv_std).contiguous())
+        ctx.grp = grp
+        ctx.save_for_backward(inv_std, norm_feat)
+        return norm_feat
+
+    @staticmethod
+    def backward(ctx, out_grad):
+        from . import backend as _C
+        inv_std, norm_feat = ctx.saved_tensors
+        grp = ctx.grp
+        dy = out_grad.contiguous()
+        if dy.dtype != norm_feat.dtype:
+            dy = dy.to(norm_feat.dtype)
+        mean_dout = _C._segment_reduce(dy, grp, _lib.SEG_AVG)
+        mean_dout_feat = _C._segment_reduce(dy, grp, _lib.SEG_AVG, b=norm_feat)
+        din = _C._broadcast_fma(dy, inv_std, grp, z=norm_feat,
+                                h32=(-mean_dout_feat * inv_std).contiguous(),
+                                k32=(-mean_dout * inv_std).contiguous())
+        return din, None, None, None, None
+
+
+class MinkowskiInstanceNorm(nn.Module):
+    """Instance normalisation of a sparse tensor: every cloud normalised by its own per-channel
+    statistics, then `* weight + bias` ([1, C] parameters; reference MinkowskiNormalization.py:
+    357-400).  The affine step keeps the feature dtype."""
+
+    def __init__(self, num_features):
+        nn.Module.__init__(self)
+        self.num_features = num_features
+        self.weight = nn.Parameter(torch.ones(1, num_features))
+        self.bias = nn.Parameter(torch.zeros(1, num_features))
+        self.reset_parameters()
+        self.inst_norm = MinkowskiInstanceNormFunction
+
+    def __repr__(self):
+        return self.__class__.__name__ + f"(nchannels={self.num_features})"
+
+    def reset_parameters(self):
+        self.weight.data.fill_(1)
+        self.bias.data.zero_()
+
+    def forward(self, input: SparseTensor):
+        assert isinstance(input, SparseTensor)
+        output = self.inst_norm.apply(input.F, input.coordinate_map_key, None,
+                                      input.coordinate_manager)
+        w, b = self.weight, self.bias
+        if w.dtype != output.dtype:
+            w, b = w.to(output.dtype), b.to(output.dtype)
+        output = output * w + b
+        return SparseTensor(output, coordinate_map_key=input.coordinate_map_key,
+                            coordinate_manager=input.coordinate_manager)

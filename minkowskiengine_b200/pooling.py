@@ -106,3 +106,73 @@ class MinkowskiMaxPooling(MinkowskiPoolingBase):
                                       is_transpose=False,
                                       pooling_mode=PoolingMode.LOCAL_MAX_POOLING,
                                       dimension=dimension)
+
+
+class MinkowskiGlobalPoolingFunction(Function):
+    """Per-cloud reduction to the origin map (reference: MinkowskiPooling.py:583-630)."""
+
+    @staticmethod
+    def forward(ctx, input_features: torch.Tensor, pooling_mode: PoolingMode,
+                in_coordinate_map_key: CoordinateMapKey,
+                out_coordinate_map_key: CoordinateMapKey = None,
+                coordinate_manager: CoordinateManager = None):
+        if out_coordinate_map_key is None:
+            out_coordinate_map_key = CoordinateMapKey(
+                in_coordinate_map_key.get_coordinate_size())
+        input_features = input_features.contiguous()
+        ctx.input_features = input_features
+        ctx.in_coords_key = in_coordinate_map_key
+        ctx.out_coords_key = out_coordinate_map_key
+        ctx.coordinate_manager = coordinate_manager
+        ctx.pooling_mode = pooling_mode
+        out_feat, num_nonzero = _C.GlobalPoolingForwardGPU(
+            input_features, pooling_mode, in_coordinate_map_key, out_coordinate_map_key,
+            coordinate_manager._manager)
+        ctx.num_nonzero = num_nonzero
+        return out_feat
+
+    @staticmethod
+    def backward(ctx, grad_out_feat):
+        grad_out_feat = grad_out_feat.contiguous()
+        grad_in_feat = _C.GlobalPoolingBackwardGPU(
+            ctx.input_features, grad_out_feat, ctx.num_nonzero, ctx.pooling_mode,
+            ctx.in_coords_key, ctx.out_coords_key, ctx.coordinate_manager._manager)
+        return grad_in_feat, None, None, None, None, None
+
+
+class MinkowskiGlobalPooling(MinkowskiModuleBase):
+    """Reduces every cloud to one row at its origin (b, 0, ..., 0); output row s is the cloud
+    with the s-th smallest batch index (reference: MinkowskiPooling.py:633-677)."""
+
+    def __init__(self, mode: PoolingMode = PoolingMode.GLOBAL_AVG_POOLING_PYTORCH_INDEX):
+        super().__init__()
+        assert isinstance(mode, PoolingMode), f"Mode must be an instance of PoolingMode. mode={mode}"
+        self.pooling_mode = mode
+        self.pooling = MinkowskiGlobalPoolingFunction
+
+    def forward(self, input: SparseTensor, coordinates=None):
+        out_key = _get_coordinate_map_key(input, coordinates)
+        output = self.pooling.apply(input.F, self.pooling_mode, input.coordinate_map_key, out_key,
+                                    input._manager)
+        return SparseTensor(output, coordinate_map_key=out_key,
+                            coordinate_manager=input.coordinate_manager)
+
+    def __repr__(self):
+        return self.__class__.__name__ + f"(mode={str(self.pooling_mode)})"
+
+
+class MinkowskiGlobalSumPooling(MinkowskiGlobalPooling):
+    def __init__(self, mode=PoolingMode.GLOBAL_SUM_POOLING_PYTORCH_INDEX):
+        MinkowskiGlobalPooling.__init__(self, mode=mode)
+
+
+class MinkowskiGlobalAvgPooling(MinkowskiGlobalPooling):
+    def __init__(self, mode=PoolingMode.GLOBAL_AVG_POOLING_PYTORCH_INDEX):
+        MinkowskiGlobalPooling.__init__(self, mode=mode)
+
+
+class MinkowskiGlobalMaxPooling(MinkowskiGlobalPooling):
+    """Per-cloud, per-channel maximum; the gradient goes to the lowest row holding it."""
+
+    def __init__(self, mode=PoolingMode.GLOBAL_MAX_POOLING_PYTORCH_INDEX):
+        MinkowskiGlobalPooling.__init__(self, mode=mode)
