@@ -329,6 +329,40 @@ int meb200_broadcast_fma(const void *x, const void *z, int dtype, const float *g
                          const float *k, const int32_t *row_seg, uint32_t n, uint32_t C, void *out,
                          void *stream);
 
+/* ---- pruning, union and arithmetic between different coordinate maps (reference:
+ *      src/pruning_cpu.cpp, MinkowskiUnion.py:50-82, MinkowskiTensor.py:522-540).  The maps come
+ *      from meb200_insert_and_map (pruned: valid = the keep mask; union: the inputs' rows
+ *      concatenated).  Every output element is written exactly once: no memset, no atomics,
+ *      bit-identical results run to run.  fp32 arithmetic, one rounding to the feature dtype;
+ *      16-byte accesses where C * sizeof(dtype) % 16 == 0 and the pointers allow. ------------- */
+#define MEB200_UNION_ADD 0
+#define MEB200_UNION_SUB 1
+#define MEB200_UNION_MUL 2
+#define MEB200_UNION_DIV 3
+
+/* out[j, :] = idx[j] >= 0 ? src[idx[j], :] : 0 for j < n_out; src: [n_src, C], out: [n_out, C] in
+ * `dtype`.  Pruning forward (idx = the insert's unique_index) and backward (idx = its
+ * inverse_map, -1 -> zero row). */
+int meb200_gather_rows(const void *src, int dtype, uint32_t n_src, uint32_t C, const int64_t *idx,
+                       uint32_t n_out, void *out, void *stream);
+
+/* The union fold.  inputs: DEVICE array of N feature pointers ([n_i, C] in `dtype`);
+ * inputs_align: a power of two dividing every one of them (16 enables vector loads);
+ * src: int32 [N, M], src[i, u] = row of input i with union row u's coordinate, or -1.
+ * Forward, for every union row u:  acc = 0;  for i = 0..N-1 with src[i, u] >= 0:
+ *   acc = (i == 0) ? x_i : op(acc, x_i);   out[u] = acc          (out: [M, C])
+ * Backward, for input i: grad_i[r] = grad_out[u_i[r]] * d out / d x_i at u_i[r] (u_i: int64
+ * [n_i], the union row of every row of input i), the derivative of the piecewise fold above:
+ *   ADD 1;  SUB i == 0 ? 1 : -1;  MUL the product of the other present inputs (0 when i > 0 and
+ *   input 0 is absent);  DIV i == 0: 1 / x_1 / x_2 ...,  i > 0: -(out / x_i). */
+int meb200_union_fold_forward(const void *const *inputs, uint32_t N, uint32_t inputs_align,
+                              const int32_t *src, uint32_t M, uint32_t C, int dtype, int op,
+                              void *out, void *stream);
+int meb200_union_fold_backward(const void *const *inputs, uint32_t N, uint32_t inputs_align,
+                               const int32_t *src, uint32_t M, uint32_t C, int dtype, int op,
+                               const void *grad_out, uint32_t i, const int64_t *u_i, uint32_t n_i,
+                               void *grad_i, void *stream);
+
 /* ---- batch normalisation over [n, C] feature rows (SURVEY.md 8(f) "next" row 1; the
  *      reference applies torch.nn.BatchNorm1d to `.F`: MinkowskiEngine/MinkowskiNormalization.py:51-99).
  *      C must be a multiple of 8.  sums: DEVICE double [2C]; statistics tensors fp32 [C]. ------ */

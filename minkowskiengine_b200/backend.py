@@ -12,6 +12,7 @@ import ctypes
 import os
 import random
 import string
+import warnings
 import weakref
 
 import torch
@@ -317,6 +318,8 @@ class CoordinateMapManagerGPU_c10:
         self._inserted = []     # keys of the maps made by insert_and_map, in order
         self._origin_covers = 0  # ... how many of them the origin map was built from
         self._groupings = {}    # map key -> _OriginGrouping
+        self._prunes = {}       # (in key, out key) -> (unique_index, inverse_map) of a pruned map
+        self._unions = {}       # tuple of input keys -> _UnionMap
         _lib.load()             # fail at construction if the native library is missing
 
     # -- keys ------------------------------------------------------------------------
@@ -755,6 +758,74 @@ class CoordinateMapManagerGPU_c10:
             rows[b] = order[starts[s]:starts[s + 1]]
         return batch, rows
 
+    # -- pruning and union -------------------------------------------------------------
+    def _new_map(self, cand, ts, valid=None):
+        """Insert of candidate rows (meb200_insert_and_map) -> (map, unique_index, inverse_map);
+        zero candidates or zero survivors give a 0-row map whose table is empty."""
+        dev = cand.device
+        if cand.shape[0] == 0:
+            cap = int(_lib.load().meb200_hash_capacity(0))
+            table = torch.full((cap,), -1, dtype=torch.int32, device=dev)
+            empty = torch.empty(0, dtype=torch.int64, device=dev)
+            return _CoordinateMap(cand, table, cap, ts), empty, empty
+        cmap, uidx, inv = _CoordinateMap.build(cand, ts, valid)
+        if cmap.size == 0:
+            cmap.table.fill_(-1)
+        return cmap, uidx, inv
+
+    def _prune(self, in_key, keep):
+        """reference: CoordinateMapManager::prune (coordinate_map_manager.cpp) -> out key tuple.
+        Rows of the pruned map are the kept rows in ascending input order (the insert numbers rows
+        by first occurrence).  Not cached: every call makes a new key at the input's stride."""
+        ik = self._k(in_key)
+        _assert(ik in self._maps, ERROR_MAP_NOT_FOUND)
+        in_map = self._maps[ik]
+        valid = keep if keep.dtype == torch.uint8 else keep.view(torch.uint8)
+        cmap, uidx, inv = self._new_map(in_map.coords, in_map.tensor_stride, valid.contiguous())
+        ok = self.get_random_string_id(in_map.tensor_stride, "")
+        self._maps[ok] = cmap
+        self._prunes[(ik, ok)] = (uidx, inv)
+        return ok
+
+    def _union(self, in_keys):
+        """The union map of `in_keys` (cached per ordered tuple of keys, as kernel maps are): rows of
+        input 0 in order, then the new rows of input 1 in order, and so on."""
+        iks = tuple(self._k(k) for k in in_keys)
+        um = self._unions.get(iks)
+        if um is not None:
+            return um
+        _assert(len(iks) >= 1, "union_map needs at least one input")
+        for k in iks:
+            _assert(k in self._maps, ERROR_MAP_NOT_FOUND, list(k[0]), k[1])
+        maps = [self._maps[k] for k in iks]
+        ts0, nc0 = maps[0].tensor_stride, maps[0].ncols
+        for k, m in zip(iks, maps):
+            _assert(m.tensor_stride == ts0, "union_map: tensor stride", list(m.tensor_stride),
+                    "of", list(k[0]), k[1], "!= tensor stride", list(ts0), "of the first input")
+            _assert(m.ncols == nc0, "union_map: coordinate size", m.ncols, "!=", nc0)
+        cand = torch.cat([m.coords for m in maps]).contiguous()
+        cmap, _, inv = self._new_map(cand, ts0)
+        ok = self.get_random_string_id(ts0, "")
+        self._maps[ok] = cmap
+        um = _UnionMap()
+        um.key, um.M = ok, cmap.size
+        um.sizes = [m.size for m in maps]
+        um.u = list(torch.split(inv, um.sizes))
+        um.src = torch.full((len(maps), cmap.size), -1, dtype=torch.int32, device=cand.device)
+        for i, (u, n) in enumerate(zip(um.u, um.sizes)):
+            # unique targets (coordinates are unique within an input): a deterministic scatter
+            um.src[i, u] = torch.arange(n, dtype=torch.int32, device=cand.device)
+        self._unions[iks] = um
+        return um
+
+    def union_map(self, in_keys, out_key):
+        """reference: union_map_th (coordinate_map_manager.cpp) -> per input int64 [2, n_i] of
+        (input rows, union rows); sets `out_key`."""
+        um = self._union(in_keys)
+        out_key.set_key(list(um.key[0]), um.key[1])
+        return [torch.stack([torch.arange(n, dtype=torch.int64, device=u.device), u])
+                for u, n in zip(um.u, um.sizes)]
+
     def __repr__(self):
         lines = [f"\t{list(k[0])}{':' + k[1] if k[1] else ''}:\tCoordinateMapGPU:{m.size}x{m.ncols}"
                  for k, m in self._maps.items()]
@@ -783,6 +854,13 @@ class _OriginGrouping:
         if getattr(self, "_counts", None) is None:
             self._counts = (self.seg_start[1:] - self.seg_start[:-1]).float()
         return self._counts
+
+
+class _UnionMap:
+    """The union of N coordinate maps: `key` (M rows); u[i] int64 [n_i] = union row of every row of
+    input i; src int32 [N, M] = row of input i holding union row u, or -1."""
+
+    __slots__ = ("key", "M", "sizes", "u", "src")
 
 
 # ----------------------------------------------------------------------------------------
@@ -1405,3 +1483,123 @@ def BroadcastBackwardGPU(in_feat, in_feat_glob, grad_out_feat, broadcast_mode, i
         grad_in = _broadcast(grad_out_feat, _f32c(in_feat_glob), grp, _lib.BCAST_MUL)
         grad_glob = _segment_reduce(grad_out_feat, grp, _lib.SEG_SUM, b=in_feat)
     return grad_in, grad_glob.to(in_feat_glob.dtype)
+
+
+# ---- pruning, union and arithmetic between different coordinate maps ---------------------------
+def _gather_rows(src, idx, n_out):
+    """[n_out, C] rows src[idx[j]] (zero where idx[j] < 0): meb200_gather_rows."""
+    out = torch.empty((n_out, src.size(1)), dtype=src.dtype, device=src.device)
+    _lib.check(_lib.load().meb200_gather_rows(
+        _lib.ptr(src), _lib.dtype_code(src.dtype), src.size(0), src.size(1), _lib.ptr(idx), n_out,
+        _lib.ptr(out), _lib.current_stream()))
+    return out
+
+
+def PruningForwardGPU(in_feat, keep, in_key, out_key, manager):
+    """reference: PruningForwardGPU (pybind/extern.hpp:414-421, validation of
+    src/pruning_cpu.cpp:49-69).  Mutates `out_key` (-> a new key at the input's tensor stride, rows
+    = the kept rows in ascending input order) when it is unset."""
+    _assert(in_feat.is_contiguous(), "in_feat must be contiguous")
+    _assert(keep.is_contiguous(), "keep must be contiguous")
+    _assert(keep.dtype in (torch.bool, torch.uint8), "keep must be a boolean tensor")
+    _assert(in_feat.dim() == 2, "in_feat.dim():", in_feat.dim())
+    _assert(keep.dim() == 1, "keep.dim():", keep.dim())
+    N = in_feat.size(0)
+    _assert(N == keep.size(0), "Input feature size and keep size mismatch")
+    _assert(manager.exists(in_key), ERROR_MAP_NOT_FOUND)
+    _assert(N == manager.size(in_key), "Invalid in_feat size", N, "!=", manager.size(in_key))
+    _assert(in_feat.is_cuda, "in_feat must be CUDA (this backend has no CPU path)")
+    _assert(keep.device == in_feat.device, "keep must be on the device of in_feat")
+    ik = manager._k(in_key)
+    if not out_key.is_key_set():
+        ok = manager._prune(in_key, keep)
+        out_key.set_key(list(ok[0]), ok[1])
+    ent = manager._prunes.get((ik, manager._k(out_key)))
+    _assert(ent is not None, "out_key", out_key, "is not a pruning of in_key", in_key)
+    uidx, _ = ent
+    if uidx.numel() == 0:
+        warnings.warn("MinkowskiPruning: Generating an empty SparseTensor")
+    return _gather_rows(in_feat, uidx, uidx.numel())
+
+
+def PruningBackwardGPU(grad_out_feat, in_key, out_key, manager):
+    """reference: PruningBackwardGPU (pybind/extern.hpp:423-430): grad_in[r] = grad_out[row of r in
+    the pruned map], 0 for pruned rows (fully written, no zero fill)."""
+    grad_out_feat = grad_out_feat.contiguous()
+    _assert(grad_out_feat.is_cuda, "grad_out_feat must be CUDA (this backend has no CPU path)")
+    _assert(grad_out_feat.dim() == 2, "grad_out_feat.dim():", grad_out_feat.dim())
+    ik, ok = manager._k(in_key), manager._k(out_key)
+    ent = manager._prunes.get((ik, ok))
+    _assert(ent is not None, "out_key", out_key, "is not a pruning of in_key", in_key)
+    uidx, inv = ent
+    _assert(grad_out_feat.size(0) == uidx.numel(), "Invalid grad_out_feat size",
+            grad_out_feat.size(0), "!=", uidx.numel())
+    return _gather_rows(grad_out_feat, inv, manager.size(in_key))
+
+
+def _pointer_table(feats):
+    """(DEVICE int64 [N] of the feature pointers, largest power of two <= 16 dividing all of them)."""
+    ptrs = [t.data_ptr() for t in feats]
+    align = 16
+    for p in ptrs:
+        while p % align:
+            align //= 2
+    table = torch.tensor(ptrs, dtype=torch.int64).to(feats[0].device, non_blocking=True)
+    return table, align
+
+
+def _check_union_feats(feats, um):
+    _assert(len(feats) == len(um.sizes), "The input features and keys must have the same length")
+    f0 = feats[0]
+    for i, (f, n) in enumerate(zip(feats, um.sizes)):
+        _assert(f.dim() == 2 and f.size(0) == n, "input", i, "features", tuple(f.shape),
+                "do not match its map of", n, "rows")
+        _assert(f.size(1) == f0.size(1), "input", i, "has", f.size(1), "channels,", f0.size(1),
+                "expected")
+        _assert(f.dtype == f0.dtype, "input", i, "dtype", f.dtype, "!=", f0.dtype)
+    _check_union_devices(feats)
+
+
+def _check_union_devices(feats):
+    for i, f in enumerate(feats):
+        _assert(f.is_cuda and f.device == feats[0].device, "input", i, "must be a CUDA tensor on",
+                feats[0].device, "(this backend has no CPU path)")
+
+
+def union_fold_forward(feats, um, op):
+    """[M, C] fold of the inputs over union map `um` (meb200_union_fold_forward)."""
+    feats = [f.contiguous() for f in feats]
+    _check_union_feats(feats, um)
+    C = feats[0].size(1)
+    out = torch.empty((um.M, C), dtype=feats[0].dtype, device=feats[0].device)
+    if um.M == 0 or C == 0:
+        return out
+    table, align = _pointer_table(feats)
+    _lib.check(_lib.load().meb200_union_fold_forward(
+        _lib.ptr(table), len(feats), align, _lib.ptr(um.src), um.M, C,
+        _lib.dtype_code(feats[0].dtype), op, _lib.ptr(out), _lib.current_stream()))
+    return out
+
+
+def union_fold_backward(grad_out, feats, um, op, needs=None):
+    """Gradients of union_fold_forward for every input (None where needs[i] is False)."""
+    feats = [f.contiguous() for f in feats]
+    grad_out = grad_out.contiguous()
+    _check_union_feats(feats, um)
+    C = feats[0].size(1)
+    _assert(grad_out.shape == (um.M, C) and grad_out.dtype == feats[0].dtype,
+            "Invalid grad_out_feat", tuple(grad_out.shape), grad_out.dtype)
+    table, align = _pointer_table(feats)
+    lib = _lib.load()
+    grads = []
+    for i, f in enumerate(feats):
+        if needs is not None and not needs[i]:
+            grads.append(None)
+            continue
+        g = torch.empty_like(f)
+        _lib.check(lib.meb200_union_fold_backward(
+            _lib.ptr(table), len(feats), align, _lib.ptr(um.src), um.M, C, _lib.dtype_code(f.dtype),
+            op, _lib.ptr(grad_out), i, _lib.ptr(um.u[i]), um.sizes[i], _lib.ptr(g),
+            _lib.current_stream()))
+        grads.append(g)
+    return grads

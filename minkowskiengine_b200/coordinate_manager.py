@@ -145,6 +145,13 @@ class CoordinateManager:
         """Number of clouds B (rows of the origin map)."""
         return self._manager.origin_map_size()
 
+    def union_map(self, in_keys: list, out_key):
+        """Sets `out_key` to the union of the maps `in_keys` (rows of the first map in order, then
+        the new rows of each following map in order; cached per ordered tuple of keys) and returns,
+        per input, int64 [2, n_i]: (input rows, union rows)
+        (reference: MinkowskiCoordinateManager.py:432)."""
+        return self._manager.union_map(in_keys, out_key)
+
     def stride_map(self, in_key: CoordinateMapKey, stride_key: CoordinateMapKey):
         return self._manager.stride_map(in_key, stride_key)
 

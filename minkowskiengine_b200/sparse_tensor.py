@@ -6,6 +6,8 @@ from enum import Enum
 
 import torch
 
+from ._lib import UNION_ADD as _UNION_ADD, UNION_DIV as _UNION_DIV, UNION_MUL as _UNION_MUL, \
+    UNION_SUB as _UNION_SUB
 from .backend import CoordinateMapKey
 from .common import convert_to_int_list
 from .coordinate_manager import CoordinateManager
@@ -135,32 +137,42 @@ class Tensor:
         return self.__class__(feats, coordinate_map_key=self.coordinate_map_key,
                               coordinate_manager=self._manager)
 
-    def _binary(self, other, fn):
+    def _binary(self, other, fn, op):
         if isinstance(other, Tensor):
             assert self._manager == other._manager, COORDINATE_MANAGER_DIFFERENT_ERROR
             if self.coordinate_map_key != other.coordinate_map_key:
-                raise NotImplementedError(
-                    "binary operations between sparse tensors with different coordinate maps "
-                    "(the reference's union-map path, MinkowskiTensor.py:431-481) are outside "
-                    "this package's scope")
+                return self._binary_union(other, op)
             return self._like(fn(self._F, other._F))
         return self._like(fn(self._F, other))
 
+    def _binary_union(self, other, op):
+        """op over the union of the two coordinate maps (reference: MinkowskiTensor.py:522-540):
+        rows only in self keep self's features, rows only in other give op(0, other), rows in both
+        op(self, other).  Rows: self's in order, then other's new rows in order.  Mixed dtypes are
+        computed in their promoted dtype and the result has self's dtype, as in the reference."""
+        from .union import MinkowskiBinaryFunction
+        out_key = CoordinateMapKey(self.coordinate_map_key.get_coordinate_size())
+        dt = torch.promote_types(self._F.dtype, other._F.dtype)
+        out = MinkowskiBinaryFunction.apply(op, [self.coordinate_map_key, other.coordinate_map_key],
+                                            out_key, self._manager, self._F.to(dt), other._F.to(dt))
+        return self.__class__(out.to(self._F.dtype), coordinate_map_key=out_key,
+                              coordinate_manager=self._manager)
+
     def __add__(self, other):
-        return self._binary(other, lambda a, b: a + b)
+        return self._binary(other, lambda a, b: a + b, _UNION_ADD)
 
     __radd__ = __add__
 
     def __sub__(self, other):
-        return self._binary(other, lambda a, b: a - b)
+        return self._binary(other, lambda a, b: a - b, _UNION_SUB)
 
     def __mul__(self, other):
-        return self._binary(other, lambda a, b: a * b)
+        return self._binary(other, lambda a, b: a * b, _UNION_MUL)
 
     __rmul__ = __mul__
 
     def __truediv__(self, other):
-        return self._binary(other, lambda a, b: a / b)
+        return self._binary(other, lambda a, b: a / b, _UNION_DIV)
 
     def __neg__(self):
         return self._like(-self._F)
