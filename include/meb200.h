@@ -169,7 +169,10 @@ int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_
                         void *workspace, uint64_t workspace_bytes, void *stream);
 
 /* grad_in[i,:] = sum_k grad_out[in_nbr[k,i],:] @ W[k]^T   (fully written)
- * grad_weight[k] = sum_o in[out_nbr[k,o],:]^T @ grad_out[o,:]   (fully written, fp32) */
+ * grad_weight[k] = sum_o in[out_nbr[k,o],:]^T @ grad_out[o,:]   (fully written, fp32)
+ * workspace: meb200_conv_workspace_bytes(n_in, n_out, c_in, c_out, K, dtype) bytes.  Every wgrad
+ * kernel stores its row splits' partial sums there and adds them in split order (no atomics:
+ * bit-identical run to run); less or NULL is legal and means fewer splits, down to one. */
 int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32_t n_in,
                          uint32_t c_in, const void *weight, uint32_t K, uint32_t c_out,
                          const int32_t *out_nbr, const int32_t *in_nbr, uint32_t n_out,
@@ -249,7 +252,9 @@ int meb200_conv_backward_packed(const void *in, const void *grad_out, int dtype,
                                 uint32_t n_chunks, void *workspace, uint64_t workspace_bytes,
                                 void *stream);
 
-/* Workspace the two calls above may use (0 is legal: slower fallbacks are chosen). */
+/* Workspace of meb200_conv_forward / meb200_conv_backward in any dtype: the SIMT wgrad's row
+ * splits, and for BF16/F16 the tensor-core weight copy and wgrad splits (0 is legal: slower
+ * fallbacks and fewer splits are chosen). */
 uint64_t meb200_conv_workspace_bytes(uint32_t n_in, uint32_t n_out, uint32_t c_in,
                                      uint32_t c_out, uint32_t K, int dtype);
 /* Workspace for the row-split partial sums of a wgrad over n_out rows (0: none needed).  Row
@@ -260,11 +265,14 @@ uint64_t meb200_conv_wgrad_workspace_bytes(uint32_t c_in, uint32_t c_out, uint32
 /* ---- local pooling (reference a11: src/pooling_avg_kernel.hpp:40-150,
  *      src/pooling_max_kernel.hpp:35-115, src/local_pooling_cpu.cpp:43-185) ---------- */
 /* aux: AVG -> num_nonzero [n_out] (feature dtype); MAX -> max_index int32 [n_out, C]
- * (flat index row*C + c into `in`, -1 for rows without input); SUM -> unused (NULL ok). */
+ * (flat index row*C + c into `in`, -1 for rows without input); SUM -> unused (NULL ok).
+ * MAX: an empty window holds the lowest finite value of the dtype (not -inf in bf16/fp16). */
 int meb200_pool_forward(const void *in, int dtype, uint32_t n_in, uint32_t C,
                         const int32_t *out_nbr, uint32_t K, uint32_t n_out, int mode,
                         void *out, void *aux, void *stream);
-/* grad_in fully written for SUM/AVG; for MAX the caller zero-fills grad_in first. */
+/* grad_in fully written in every mode (no pre-zeroing), accumulated in fp32 in ascending k over
+ * in_nbr (required in every mode) and rounded once; deterministic, no atomics.  MAX:
+ * grad_in[i,c] = sum over windows o = in_nbr[k,i] with max_index[o,c] == i*C + c of grad_out[o,c]. */
 int meb200_pool_backward(const void *grad_out, int dtype, uint32_t n_in, uint32_t C,
                          const int32_t *in_nbr, uint32_t K, uint32_t n_out, int mode,
                          const void *aux, void *grad_in, void *stream);

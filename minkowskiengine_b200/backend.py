@@ -1327,10 +1327,7 @@ def LocalPoolingBackwardGPU(in_feat, grad_out_feat, num_nonzero, kernel_size, ke
     lib = _lib.load()
     C = in_feat.size(1)
     mode = _POOL_CODE[pooling_mode]
-    if mode == _lib.POOL_MAX:
-        grad_in = torch.zeros_like(in_feat)
-    else:
-        grad_in = torch.empty_like(in_feat)
+    grad_in = torch.empty_like(in_feat)       # every mode writes every element once
     _lib.check(lib.meb200_pool_backward(
         _lib.ptr(grad_out_feat), _lib.dtype_code(in_feat.dtype), km.n_in, C, _lib.ptr(km.in_nbr),
         km.K, km.n_out, mode, _lib.ptr(num_nonzero) if num_nonzero.numel() else None,

@@ -2,6 +2,8 @@
 // qualifies (conv_tc.cuh) and the SIMT path otherwise.
 #include <stdlib.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 #include "conv_simt.cuh"
 #include "conv_tc.cuh"
@@ -22,12 +24,14 @@ extern "C" {
 uint64_t meb200_conv_workspace_bytes(uint32_t n_in, uint32_t n_out, uint32_t c_in,
                                      uint32_t c_out, uint32_t K, int dtype) {
   (void)n_in;
-  if (dtype == MEB200_F32) return 0;
-  // bf16/fp16 weights re-laid out for the tensor-core kernels (W^T per offset), or the row-split
-  // partial sums of wgrad (the two are never needed by the same call)
+  // the row-split partial sums of a SIMT wgrad (any dtype); for bf16/fp16 also the weights
+  // re-laid out for the tensor-core kernels (W^T per offset) or the row-split partial sums of
+  // the tensor-core wgrad (no call needs two of these at once)
+  const uint64_t ws = conv_wgrad_simt_workspace_bytes(c_in, c_out, K, n_out);
+  if (dtype == MEB200_F32) return ws;
   const uint64_t wt = (uint64_t)K * c_in * c_out * 2 + 256;
   const uint64_t wg = conv_wgrad_workspace_bytes(c_in, c_out, K, n_out);
-  return wt > wg ? wt : wg;
+  return std::max({ws, wt, wg});
 }
 
 uint64_t meb200_conv_wgrad_workspace_bytes(uint32_t c_in, uint32_t c_out, uint32_t K,
@@ -216,9 +220,9 @@ int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32
     }
     if (conv_small_cin_supported(c_in, c_out))
       return conv_small_cin_wgrad(in, grad_out, dtype, c_in, K, c_out, out_nbr, n_out,
-                                  grad_weight, stream);
+                                  grad_weight, workspace, workspace_bytes, stream);
     return conv_wgrad_simt(in, grad_out, dtype, c_in, K, c_out, out_nbr, n_out, grad_weight,
-                           stream);
+                           workspace, workspace_bytes, stream);
   }
   return MEB200_OK;
 }

@@ -97,12 +97,14 @@ k_conv_gather_gemm(const TIn *__restrict__ A, uint32_t c_a, const TIn *__restric
   }
 }
 
-// dW[k][ci][co] += sum over rows o in this CTA's slice of in[nbr[k][o]][ci] * dOut[o][co]
+// part[split][k][ci][co] = sum over rows o in this CTA's split of in[nbr[k][o]][ci] * dOut[o][co]
+// Every element of the split's slot is stored once (zeros included); with one split the slot is
+// dW itself, otherwise k_split_sum adds the slots in split order.
 template <typename T>
 __global__ void __launch_bounds__(256)
 k_conv_wgrad(const T *__restrict__ in, const T *__restrict__ grad_out, uint32_t c_in,
              uint32_t c_out, const int32_t *__restrict__ out_nbr, uint32_t n_out,
-             uint32_t rows_per_split, uint32_t tiles_n, float *__restrict__ dW) {
+             uint32_t rows_per_split, uint32_t tiles_n, float *__restrict__ part) {
   __shared__ float As[TK][TM + 4];  // [row in chunk][ci]
   __shared__ float Bs[TK][TN + 4];  // [row in chunk][co]
   __shared__ int32_t s_idx[TK];
@@ -154,7 +156,7 @@ k_conv_wgrad(const T *__restrict__ in, const T *__restrict__ grad_out, uint32_t 
         for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
     }
   }
-  float *dWk = dW + (size_t)k * c_in * c_out;
+  float *dWk = part + ((size_t)blockIdx.y * gridDim.x + k) * c_in * c_out;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     uint32_t ci = ci0 + ty * 4 + i;
@@ -162,9 +164,36 @@ k_conv_wgrad(const T *__restrict__ in, const T *__restrict__ grad_out, uint32_t 
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       uint32_t co = co0 + tx * 4 + j;
-      if (co < c_out && acc[i][j] != 0.f) atomicAdd(dWk + (size_t)ci * c_out + co, acc[i][j]);
+      if (co < c_out) dWk[(size_t)ci * c_out + co] = acc[i][j];
     }
   }
+}
+
+// dW = part[0] + part[1] + ... + part[splits - 1], in that order
+__global__ void __launch_bounds__(256)
+k_split_sum(const float *__restrict__ part, float *__restrict__ dW, size_t n, uint32_t splits) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n;
+       i += (size_t)gridDim.x * blockDim.x) {
+    float a = part[i];
+    for (uint32_t s = 1; s < splits; ++s) a += part[s * n + i];
+    dW[i] = a;
+  }
+}
+
+static int launch_split_sum(const float *part, float *dW, size_t n, uint32_t splits,
+                            cudaStream_t stream) {
+  const unsigned blocks = (unsigned)std::min<size_t>(cdiv(n, 256), 4096);
+  k_split_sum<<<blocks, 256, 0, stream>>>(part, dW, n, splits);
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
+}
+
+// Splits that fit in `workspace_bytes`: one slot of K * c_in * c_out floats each (none: one split).
+static uint64_t workspace_slots(const void *workspace, uint64_t workspace_bytes, uint32_t c_in,
+                                uint32_t c_out, uint32_t K) {
+  if (workspace == nullptr) return 1;
+  const uint64_t fit = workspace_bytes / ((uint64_t)K * c_in * c_out * sizeof(float));
+  return fit > 1 ? fit : 1;
 }
 
 // ---- tiny input-channel count (the network stem: c_in <= 4, e.g. RGB -> 32, K = 125) -------
@@ -266,7 +295,8 @@ k_conv_small_cin_fwd(const T *__restrict__ in, uint32_t c_in, const T *__restric
 // per-warp shared-memory list, and the list is consumed 32 hits at a time with lane <-> hit:
 // every lane fetches its own dOut row slab (vector loads) and input row and accumulates a private
 // [CIN][32] tile in registers, so 32 row fetches are in flight per warp instead of one.  The
-// 32 private tiles are folded with butterfly shuffles once per warp and added to dW atomically.
+// 32 private tiles are folded with butterfly shuffles once per warp and stored to the row slice's
+// slot part[slice][k][c][co] (dW itself with one slice); k_split_sum adds the slots in order.
 constexpr int WG_SCAN = 256;             // table entries scanned per round (8 per lane)
 constexpr int WG_LIST = WG_SCAN + 32;    // + carried remainder (< 32)
 
@@ -293,7 +323,7 @@ template <typename T, int CIN>
 __global__ void __launch_bounds__(256, 1)
 k_conv_small_cin_wgrad(const T *__restrict__ in, const T *__restrict__ gout, uint32_t c_out,
                        uint32_t K, const int32_t *__restrict__ nbr, uint32_t n_out,
-                       uint32_t rows_per_block, float *__restrict__ dW) {
+                       uint32_t rows_per_block, float *__restrict__ part) {
   __shared__ uint2 s_hits[8][WG_LIST];  // (output row, input row) per warp
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t k = blockIdx.y * 8 + warp;
@@ -361,13 +391,13 @@ k_conv_small_cin_wgrad(const T *__restrict__ in, const T *__restrict__ gout, uin
 
 #pragma unroll
   for (int c = 0; c < CIN; ++c) {
-    float *dst = dW + ((size_t)k * CIN + c) * c_out + co0;
+    float *dst = part + (((size_t)blockIdx.x * K + k) * CIN + c) * c_out + co0;
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
       float v = acc[c][j];
 #pragma unroll
       for (int s = 16; s > 0; s >>= 1) v += __shfl_xor_sync(0xffffffffu, v, s);
-      if (lane == (uint32_t)j && (uint32_t)j < nco && v != 0.f) atomicAdd(dst + j, v);
+      if (lane == (uint32_t)j && (uint32_t)j < nco) dst[j] = v;
     }
   }
 }
@@ -416,40 +446,54 @@ int conv_small_cin_forward(const void *in, int in_dtype, uint32_t c_in, const vo
   return MEB200_ERR_UNSUPPORTED;
 }
 
+// Row slices of k_conv_small_cin_wgrad (at most max_slices): one 8-warp CTA per SM (register
+// tiles), aiming at ~4 CTAs per SM over the whole grid; slices are whole scan rounds, >= 4 each.
+static uint32_t small_wgrad_rows(uint32_t c_out, uint32_t K, uint32_t n_out, uint64_t max_slices) {
+  const uint32_t kgroups = cdiv(K, 8), slabs = cdiv(c_out, 32);
+  uint64_t want = std::max<uint64_t>(1, cdiv(4ull * num_sms(), (uint64_t)kgroups * slabs));
+  if (want > max_slices) want = max_slices;
+  uint32_t rows_per_block = cdiv(cdiv(n_out, (uint32_t)want), WG_SCAN) * WG_SCAN;
+  return std::max<uint32_t>(rows_per_block, 4 * WG_SCAN);
+}
+
 template <typename T>
 static int launch_small_wgrad(const void *in, const void *gout, uint32_t c_in, uint32_t K,
                               uint32_t c_out, const int32_t *nbr, uint32_t n_out, float *dW,
-                              cudaStream_t stream) {
-  const uint32_t kgroups = cdiv(K, 8), slabs = cdiv(c_out, 32);
-  // one 8-warp CTA per SM (register tiles); aim at ~4 CTAs per SM over the whole grid
-  uint32_t want_slices = std::max(1u, cdiv(4ull * num_sms(), (uint64_t)kgroups * slabs));
-  uint32_t rows_per_block = cdiv(cdiv(n_out, want_slices), WG_SCAN) * WG_SCAN;
-  if (rows_per_block < 4 * WG_SCAN) rows_per_block = 4 * WG_SCAN;
-  dim3 grid(cdiv(n_out, rows_per_block), kgroups, slabs);
+                              void *workspace, uint64_t workspace_bytes, cudaStream_t stream) {
+  const uint32_t rows_per_block =
+      small_wgrad_rows(c_out, K, n_out, workspace_slots(workspace, workspace_bytes, c_in, c_out, K));
+  dim3 grid(cdiv(n_out, rows_per_block), cdiv(K, 8), cdiv(c_out, 32));
+  float *part = grid.x > 1 ? reinterpret_cast<float *>(workspace) : dW;
   const T *x = (const T *)in, *g = (const T *)gout;
   switch (c_in) {
-    case 1: k_conv_small_cin_wgrad<T, 1><<<grid, 256, 0, stream>>>(x, g, c_out, K, nbr, n_out, rows_per_block, dW); break;
-    case 2: k_conv_small_cin_wgrad<T, 2><<<grid, 256, 0, stream>>>(x, g, c_out, K, nbr, n_out, rows_per_block, dW); break;
-    case 3: k_conv_small_cin_wgrad<T, 3><<<grid, 256, 0, stream>>>(x, g, c_out, K, nbr, n_out, rows_per_block, dW); break;
-    case 4: k_conv_small_cin_wgrad<T, 4><<<grid, 256, 0, stream>>>(x, g, c_out, K, nbr, n_out, rows_per_block, dW); break;
+    case 1: k_conv_small_cin_wgrad<T, 1><<<grid, 256, 0, stream>>>(x, g, c_out, K, nbr, n_out, rows_per_block, part); break;
+    case 2: k_conv_small_cin_wgrad<T, 2><<<grid, 256, 0, stream>>>(x, g, c_out, K, nbr, n_out, rows_per_block, part); break;
+    case 3: k_conv_small_cin_wgrad<T, 3><<<grid, 256, 0, stream>>>(x, g, c_out, K, nbr, n_out, rows_per_block, part); break;
+    case 4: k_conv_small_cin_wgrad<T, 4><<<grid, 256, 0, stream>>>(x, g, c_out, K, nbr, n_out, rows_per_block, part); break;
     default: return MEB200_ERR_UNSUPPORTED;
   }
   MEB_LAUNCH_OK();
-  return MEB200_OK;
+  if (grid.x == 1) return MEB200_OK;
+  return launch_split_sum(part, dW, (size_t)K * c_in * c_out, grid.x, stream);
 }
 
 int conv_small_cin_wgrad(const void *in, const void *grad_out, int dtype, uint32_t c_in, uint32_t K,
                          uint32_t c_out, const int32_t *out_nbr, uint32_t n_out, float *grad_weight,
-                         cudaStream_t stream) {
-  MEB_CUDA(cudaMemsetAsync(grad_weight, 0, (size_t)K * c_in * c_out * sizeof(float), stream));
-  if (n_out == 0 || K == 0) return MEB200_OK;
+                         void *workspace, uint64_t workspace_bytes, cudaStream_t stream) {
+  if (n_out == 0 || K == 0) {
+    MEB_CUDA(cudaMemsetAsync(grad_weight, 0, (size_t)K * c_in * c_out * sizeof(float), stream));
+    return MEB200_OK;
+  }
   switch (dtype) {
     case MEB200_F32:
-      return launch_small_wgrad<float>(in, grad_out, c_in, K, c_out, out_nbr, n_out, grad_weight, stream);
+      return launch_small_wgrad<float>(in, grad_out, c_in, K, c_out, out_nbr, n_out, grad_weight,
+                                       workspace, workspace_bytes, stream);
     case MEB200_BF16:
-      return launch_small_wgrad<__nv_bfloat16>(in, grad_out, c_in, K, c_out, out_nbr, n_out, grad_weight, stream);
+      return launch_small_wgrad<__nv_bfloat16>(in, grad_out, c_in, K, c_out, out_nbr, n_out,
+                                               grad_weight, workspace, workspace_bytes, stream);
     case MEB200_F16:
-      return launch_small_wgrad<__half>(in, grad_out, c_in, K, c_out, out_nbr, n_out, grad_weight, stream);
+      return launch_small_wgrad<__half>(in, grad_out, c_in, K, c_out, out_nbr, n_out, grad_weight,
+                                        workspace, workspace_bytes, stream);
     default:
       return MEB200_ERR_UNSUPPORTED;
   }
@@ -490,38 +534,58 @@ int conv_forward_simt(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in
   return MEB200_ERR_UNSUPPORTED;
 }
 
+// Rows per split of k_conv_wgrad (at most max_splits splits): enough CTAs for ~4 waves, each
+// split a multiple of TK rows and at least 8 * TK.
+static uint32_t simt_wgrad_rows(uint32_t c_in, uint32_t c_out, uint32_t K, uint32_t n_out,
+                                uint64_t max_splits) {
+  const uint64_t tiles = (uint64_t)cdiv(c_in, TM) * cdiv(c_out, TN);
+  uint64_t splits = std::max<uint64_t>(1, cdiv(4ull * num_sms(), (uint64_t)K * tiles));
+  splits = std::min<uint64_t>({splits, cdiv(n_out, 8 * TK), 65535, max_splits});
+  return cdiv(cdiv(n_out, (uint32_t)splits), TK) * TK;
+}
+
+uint64_t conv_wgrad_simt_workspace_bytes(uint32_t c_in, uint32_t c_out, uint32_t K,
+                                         uint32_t n_out) {
+  if (n_out == 0 || K == 0 || c_in == 0 || c_out == 0) return 0;
+  const uint32_t rows = conv_small_cin_supported(c_in, c_out)
+                            ? small_wgrad_rows(c_out, K, n_out, UINT64_MAX)
+                            : simt_wgrad_rows(c_in, c_out, K, n_out, UINT64_MAX);
+  const uint32_t splits = cdiv(n_out, rows);
+  return splits > 1 ? (uint64_t)splits * K * c_in * c_out * sizeof(float) : 0;
+}
+
 int conv_wgrad_simt(const void *in, const void *grad_out, int dtype, uint32_t c_in, uint32_t K,
                     uint32_t c_out, const int32_t *out_nbr, uint32_t n_out, float *grad_weight,
-                    cudaStream_t stream) {
-  MEB_CUDA(cudaMemsetAsync(grad_weight, 0, (size_t)K * c_in * c_out * sizeof(float), stream));
-  if (n_out == 0 || K == 0) return MEB200_OK;
-  uint32_t tiles_m = cdiv(c_in, TM), tiles_n = cdiv(c_out, TN);
-  uint32_t tiles = tiles_m * tiles_n;
-  // enough CTAs for ~4 waves; each split covers a multiple of TK rows
-  uint32_t want = cdiv(4ull * num_sms(), (uint64_t)K * tiles);
-  uint32_t max_splits = cdiv(n_out, 8 * TK);
-  uint32_t splits = want < 1 ? 1 : (want > max_splits ? max_splits : want);
-  if (splits > 65535) splits = 65535;
-  uint32_t rows_per_split = cdiv(cdiv(n_out, splits), TK) * TK;
-  splits = cdiv(n_out, rows_per_split);
-  dim3 grid(K, splits, tiles);
+                    void *workspace, uint64_t workspace_bytes, cudaStream_t stream) {
+  if (n_out == 0 || K == 0) {
+    MEB_CUDA(cudaMemsetAsync(grad_weight, 0, (size_t)K * c_in * c_out * sizeof(float), stream));
+    return MEB200_OK;
+  }
+  const uint32_t tiles_n = cdiv(c_out, TN), tiles = cdiv(c_in, TM) * tiles_n;
   MEB_CHECK_ARG(tiles <= 65535, "too many channel tiles");
+  // a missing or small workspace leaves fewer splits (one: the CTAs store into dW directly)
+  const uint32_t rows_per_split = simt_wgrad_rows(
+      c_in, c_out, K, n_out, workspace_slots(workspace, workspace_bytes, c_in, c_out, K));
+  const uint32_t splits = cdiv(n_out, rows_per_split);
+  float *part = splits > 1 ? reinterpret_cast<float *>(workspace) : grad_weight;
+  dim3 grid(K, splits, tiles);
   switch (dtype) {
     case MEB200_F32:
-      k_conv_wgrad<float><<<grid, 256, 0, stream>>>((const float *)in, (const float *)grad_out, c_in, c_out, out_nbr, n_out, rows_per_split, tiles_n, grad_weight);
+      k_conv_wgrad<float><<<grid, 256, 0, stream>>>((const float *)in, (const float *)grad_out, c_in, c_out, out_nbr, n_out, rows_per_split, tiles_n, part);
       break;
     case MEB200_BF16:
-      k_conv_wgrad<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16 *)in, (const __nv_bfloat16 *)grad_out, c_in, c_out, out_nbr, n_out, rows_per_split, tiles_n, grad_weight);
+      k_conv_wgrad<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16 *)in, (const __nv_bfloat16 *)grad_out, c_in, c_out, out_nbr, n_out, rows_per_split, tiles_n, part);
       break;
     case MEB200_F16:
-      k_conv_wgrad<__half><<<grid, 256, 0, stream>>>((const __half *)in, (const __half *)grad_out, c_in, c_out, out_nbr, n_out, rows_per_split, tiles_n, grad_weight);
+      k_conv_wgrad<__half><<<grid, 256, 0, stream>>>((const __half *)in, (const __half *)grad_out, c_in, c_out, out_nbr, n_out, rows_per_split, tiles_n, part);
       break;
     default:
       set_error("conv wgrad (simt): unsupported dtype %d", dtype);
       return MEB200_ERR_UNSUPPORTED;
   }
   MEB_LAUNCH_OK();
-  return MEB200_OK;
+  if (splits == 1) return MEB200_OK;
+  return launch_split_sum(part, grad_weight, (size_t)K * c_in * c_out, splits, stream);
 }
 
 }  // namespace meb200

@@ -13,6 +13,15 @@
 
 namespace meb200 {
 
+// The lowest finite value of the storage type: what an empty max window holds, as the reference
+// CPU kernel fills it (-FLT_MAX would round to -inf in bf16 / fp16).
+template <typename T> __device__ __forceinline__ float lowest_finite();
+template <> __device__ __forceinline__ float lowest_finite<float>() { return -FLT_MAX; }
+template <> __device__ __forceinline__ float lowest_finite<__nv_bfloat16>() {
+  return __uint_as_float(0xff7f0000u);   // -0x1.fep+127
+}
+template <> __device__ __forceinline__ float lowest_finite<__half>() { return -65504.f; }
+
 template <typename T, int MODE>
 __global__ void __launch_bounds__(256)
 k_pool_fwd(const T *__restrict__ in, uint32_t C, const int32_t *__restrict__ out_nbr, uint32_t K,
@@ -21,7 +30,7 @@ k_pool_fwd(const T *__restrict__ in, uint32_t C, const int32_t *__restrict__ out
   if (t >= (uint64_t)n_out * C) return;
   uint32_t o = (uint32_t)(t / C), c = (uint32_t)(t % C);
   if (MODE == MEB200_POOL_MAX) {
-    float best = -FLT_MAX;
+    float best = lowest_finite<T>();
     int32_t arg = -1;
     for (uint32_t k = 0; k < K; ++k) {
       int32_t i = __ldg(out_nbr + (size_t)k * n_out + o);
@@ -74,14 +83,26 @@ k_pool_bwd_gather(const T *__restrict__ grad_out, uint32_t C, const int32_t *__r
   grad_in[t] = from_f32<T>(acc);
 }
 
+// Input-stationary: grad_in[i, c] = sum over k ascending of grad_out[o, c] where o = in_nbr[k][i]
+// picked input element (i, c) as its arg-max.  Each element is written once, summed in fp32 and
+// rounded once, whatever the number of windows it won.
 template <typename T>
 __global__ void __launch_bounds__(256)
-k_pool_bwd_max(const T *__restrict__ grad_out, uint64_t total, const int32_t *__restrict__ max_index,
+k_pool_bwd_max(const T *__restrict__ grad_out, uint32_t C, const int32_t *__restrict__ in_nbr,
+               uint32_t K, uint32_t n_in, const int32_t *__restrict__ max_index,
                T *__restrict__ grad_in) {
   uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= total) return;
-  int32_t idx = max_index[t];
-  if (idx >= 0) atomicAdd(grad_in + idx, grad_out[t]);
+  if (t >= (uint64_t)n_in * C) return;
+  uint32_t i = (uint32_t)(t / C), c = (uint32_t)(t % C);
+  const int32_t self = (int32_t)t;   // i * C + c: max_index is int32 (checked by the forward)
+  float acc = 0.f;
+  for (uint32_t k = 0; k < K; ++k) {
+    int32_t o = __ldg(in_nbr + (size_t)k * n_in + i);
+    if (o < 0) continue;
+    const size_t oc = (size_t)o * C + c;
+    if (__ldg(max_index + oc) == self) acc += to_f32<T>(grad_out[oc]);
+  }
+  grad_in[t] = from_f32<T>(acc);
 }
 
 template <typename T>
@@ -110,10 +131,11 @@ template <typename T>
 static int pool_bwd_t(const void *grad_out, uint32_t n_in, uint32_t C, const int32_t *in_nbr,
                       uint32_t K, uint32_t n_out, int mode, const void *aux, void *grad_in,
                       cudaStream_t s) {
+  (void)n_out;
   if (mode == MEB200_POOL_MAX) {
-    uint64_t total = (uint64_t)n_out * C;
-    if (total == 0) return MEB200_OK;
-    k_pool_bwd_max<T><<<cdiv(total, 256), 256, 0, s>>>((const T *)grad_out, total, (const int32_t *)aux, (T *)grad_in);
+    if (n_in == 0) return MEB200_OK;
+    k_pool_bwd_max<T><<<cdiv((uint64_t)n_in * C, 256), 256, 0, s>>>(
+        (const T *)grad_out, C, in_nbr, K, n_in, (const int32_t *)aux, (T *)grad_in);
   } else if (mode == MEB200_POOL_AVG) {
     if (n_in == 0) return MEB200_OK;
     k_pool_bwd_gather<T, MEB200_POOL_AVG><<<cdiv((uint64_t)n_in * C, 256), 256, 0, s>>>(
@@ -161,7 +183,9 @@ int meb200_pool_backward(const void *grad_out, int dtype, uint32_t n_in, uint32_
   if (C == 0) return MEB200_OK;
   MEB_CHECK_ARG(grad_in != nullptr || n_in == 0, "null grad_in");
   MEB_CHECK_ARG(mode == MEB200_POOL_SUM || aux != nullptr, "aux buffer required");
-  MEB_CHECK_ARG(mode == MEB200_POOL_MAX || in_nbr != nullptr, "in_nbr required");
+  MEB_CHECK_ARG(in_nbr != nullptr || n_in == 0, "in_nbr required");
+  MEB_CHECK_ARG((uint64_t)n_in * C < 0x7FFFFFFFull || mode != MEB200_POOL_MAX,
+                "max_index is int32: n_in*C too large");
   cudaStream_t s = (cudaStream_t)stream;
   switch (dtype) {
     case MEB200_F32: return pool_bwd_t<float>(grad_out, n_in, C, in_nbr, K, n_out, mode, aux, grad_in, s);

@@ -59,6 +59,34 @@ def rel_err(a, b):
     return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
 
 
+def one_rounding_bound(ref, A, dtype):
+    """Per-element bound for a reduction accumulated in fp32 and stored in `dtype`, against its
+    float64 value `ref`: delta = 2^-20 * A, A the same reduction over absolute values, plus half
+    an ulp of `dtype` at |ref| + delta when the result is stored in bf16 / fp16 (one rounding)."""
+    ref, A = ref.double(), A.double()
+    delta = A * 2.0 ** -20
+    if dtype == torch.float32:
+        return delta
+    p, emin = {torch.bfloat16: (7, -126), torch.float16: (10, -14)}[dtype]
+    v = ref.abs() + delta
+    _, e = torch.frexp(v)                        # v = m * 2^e, m in [0.5, 1)
+    e = torch.where(v > 0, e - 1, torch.full_like(e, emin)).clamp(min=emin)
+    return torch.ldexp(torch.full_like(v, 0.5), e - p) + delta
+
+
+def assert_one_rounding(y, ref, A, what=""):
+    """|y - ref| <= one_rounding_bound(ref, A, y.dtype), element by element."""
+    bound = one_rounding_bound(ref, A, y.dtype)
+    err = (y.double() - ref.double()).abs()
+    bad = ~(err <= bound)
+    if bool(bad.any()):
+        j = int(torch.nonzero(bad.flatten())[0])
+        raise AssertionError(
+            f"{what}: {int(bad.sum())} of {bad.numel()} elements outside one rounding; first at "
+            f"flat index {j}: got {y.flatten()[j].item()!r}, float64 {ref.flatten()[j].item()!r}, "
+            f"|err| {err.flatten()[j].item():.3e} > bound {bound.flatten()[j].item():.3e}")
+
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 

@@ -34,6 +34,11 @@ def test_library_pure_helpers_without_gpu():
     assert lib.meb200_launch_count() == 0 or lib.meb200_launch_count() > 0
     assert lib.meb200_conv_workspace_bytes(10, 10, 64, 128, 27, ME._lib.F32) == 0
     assert lib.meb200_conv_workspace_bytes(10, 10, 64, 128, 27, ME._lib.BF16) >= 27 * 64 * 128 * 2
+    # the SIMT weight gradients keep their row splits' partial sums in the workspace, in any
+    # dtype: the MinkUNet head (96 -> 20, K = 1) and a stem (3 -> 20, K = 125) at 200k rows
+    for dt in (ME._lib.F32, ME._lib.BF16, ME._lib.F16):
+        assert lib.meb200_conv_workspace_bytes(0, 200000, 96, 20, 1, dt) >= 2 * 96 * 20 * 4
+        assert lib.meb200_conv_workspace_bytes(0, 200000, 3, 20, 125, dt) >= 2 * 125 * 3 * 20 * 4
 
 
 def test_coordinate_map_key_semantics():
@@ -358,3 +363,29 @@ def test_lazy_reverse_table_does_not_keep_the_manager_alive(monkeypatch):
         assert ref() is None, "the manager is kept alive by a reference cycle"
     finally:
         gc.enable()
+
+
+def test_no_floating_point_atomic_adds_in_the_kernels():
+    """Every floating-point reduction runs in a fixed order (results are bit-identical run to
+    run), so no atomic add may target a floating-point value.  The integer counters and tickets
+    that remain are listed here by file and destination."""
+    allowed = {
+        ("global.cu", "cnt + s"),             # per-cloud row counts of the counting sort
+        ("coords.cu", "ticket"),              # last-CTA ticket
+        ("batchnorm.cu", "tail.ticket"),      # last-CTA ticket
+        ("kernel_map.cu", "num_pairs"),       # pair count of the compacted lists
+    }
+    csrc = os.path.join(ROOT, "minkowskiengine_b200", "csrc")
+    call = re.compile(r"\b(?:unsafeAtomicAdd|atomicAdd(?:_block|_system)?)\s*\(\s*([^,]+?)\s*,")
+    ptx = re.compile(r"\b(?:red|atom)(?:\.[a-z]+)*\.add\.(?:f|bf|noftz)")
+    found = set()
+    for name in sorted(os.listdir(csrc)):
+        if not name.endswith((".cu", ".cuh", ".h")):
+            continue
+        text = open(os.path.join(csrc, name)).read()
+        text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+        text = re.sub(r"//[^\n]*", "", text)
+        assert not ptx.search(text), f"{name}: floating-point atomic add in inline PTX"
+        found |= {(name, m.group(1)) for m in call.finditer(text)}
+    assert found, "no atomic add found at all: the pattern no longer matches the sources"
+    assert found <= allowed, f"atomic adds outside the integer allowlist: {sorted(found - allowed)}"
