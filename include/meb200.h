@@ -161,35 +161,50 @@ int meb200_kernel_map_pairs(const int32_t *nbr, uint32_t K, uint32_t n_rows, uin
 /*
  * out[o,:] = sum_k in[out_nbr[k,o],:] @ W[k]          (rows with out_nbr = -1 skipped)
  * Output is fully written (no pre-zeroing needed, no atomics, deterministic).
- * in_dtype: dtype of `in` and `weight`; out_dtype: dtype of `out` (F32 always allowed).
+ * in_dtype: dtype of `in`, `w_cast` and `w_t`; out_dtype: dtype of `out` (F32 always allowed).
+ *   w_cast  [K, Cin, Cout]  the weights in the feature dtype
+ *   w_t     [K, Cout, Cin]  the same, transposed per offset (BF16/F16: required; F32: not read)
+ * Both come from meb200_conv_pack_weights.  The call runs the tensor cores on w_t when the shape
+ * qualifies, otherwise the small-cin or SIMT kernels on w_cast.
  */
 int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
-                        const void *weight, uint32_t K, uint32_t c_out,
+                        const void *w_cast, const void *w_t, uint32_t K, uint32_t c_out,
                         const int32_t *out_nbr, uint32_t n_out, void *out, int out_dtype,
-                        void *workspace, uint64_t workspace_bytes, void *stream);
+                        void *stream);
 
 /* grad_in[i,:] = sum_k grad_out[in_nbr[k,i],:] @ W[k]^T   (fully written)
  * grad_weight[k] = sum_o in[out_nbr[k,o],:]^T @ grad_out[o,:]   (fully written, fp32)
- * workspace: meb200_conv_workspace_bytes(n_in, n_out, c_in, c_out, K, dtype) bytes.  Every wgrad
+ * grad_in / grad_weight may be NULL to skip dgrad / wgrad; each picks its kernel on its own.
+ * w_cast: [K, Cin, Cout] in the feature dtype.  pairs_in / pairs_out / seg_start (all three or
+ * NULL) + n_chunks: the compacted pair lists of out_nbr from meb200_kernel_map_pairs with
+ * stage = 64 and their chunk count; when meb200_conv_wgrad_uses_pairs() holds, the wgrad reduces
+ * over them instead of the dense table.
+ * workspace: meb200_conv_workspace_bytes(n_out, c_in, c_out, K, dtype) bytes.  Every wgrad
  * kernel stores its row splits' partial sums there and adds them in split order (no atomics:
  * bit-identical run to run); less or NULL is legal and means fewer splits, down to one. */
 int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32_t n_in,
-                         uint32_t c_in, const void *weight, uint32_t K, uint32_t c_out,
+                         uint32_t c_in, const void *w_cast, uint32_t K, uint32_t c_out,
                          const int32_t *out_nbr, const int32_t *in_nbr, uint32_t n_out,
                          void *grad_in, int grad_in_dtype, float *grad_weight,
-                         void *workspace, uint64_t workspace_bytes, void *stream);
+                         const int32_t *pairs_in, const int32_t *pairs_out,
+                         const int32_t *seg_start, uint32_t n_chunks, void *workspace,
+                         uint64_t workspace_bytes, void *stream);
 
-/* Weight packing for the tensor-core path, once per optimizer step instead of once per call:
- * fp32 master weight [K, Cin, Cout] -> `dtype` (BF16/F16) operand copies
- *   w_cast [K, Cin, Cout]                 w_t  [K, Cout, Cin]
- *   w_cp   [K, Cin, perm(Cout)]           w_tp [K, Cout, perm(Cin)]
- * where perm reorders the reduction axis inside every block of 32 channels (position
- * 16h+4j+2e+b holds channel 8j+4h+2e+b).  The convolution kernels read w_cast / w_t; w_cp /
- * w_tp may be NULL and are skipped when NULL or when Cout / Cin is not a multiple of 32.  The reference keeps weights in the feature dtype and needs no such step
+/* 1 when meb200_conv_backward's wgrad reads pair lists for this layer (so a caller builds them
+ * only then), else 0. */
+int meb200_conv_wgrad_uses_pairs(int dtype, uint32_t c_in, uint32_t c_out, uint32_t K);
+
+/* Workspace of meb200_conv_backward and meb200_conv_stem_wgrad in any dtype: room for the row
+ * splits of every wgrad kernel the call can pick (0: one split). */
+uint64_t meb200_conv_workspace_bytes(uint32_t n_out, uint32_t c_in, uint32_t c_out, uint32_t K,
+                                     int dtype);
+
+/* Weight packing, once per optimizer step instead of once per call: fp32 master weight
+ * [K, Cin, Cout] -> `dtype` (BF16/F16) operand copies w_cast [K, Cin, Cout] and
+ * w_t [K, Cout, Cin].  The reference keeps weights in the feature dtype and needs no such step
  * (MinkowskiConvolution.py:264-279); this is the bf16/fp16 operand cache of this backend. */
 int meb200_conv_pack_weights(const float *weight, uint32_t K, uint32_t c_in, uint32_t c_out,
-                             int dtype, void *w_cast, void *w_t, void *w_cp, void *w_tp,
-                             void *stream);
+                             int dtype, void *w_cast, void *w_t, void *stream);
 
 /* The same packing for MANY layers in one launch (all weights of a network change together, at
  * the optimizer step): `jobs_dev` is a DEVICE array of n_jobs jobs; job j owns the 32x32 tiles
@@ -198,7 +213,7 @@ int meb200_conv_pack_weights(const float *weight, uint32_t K, uint32_t c_in, uin
  * the set of tensors (or their addresses) changes. */
 typedef struct meb200_pack_job {
   const void *w;                      /* fp32 [K, c_in, c_out] */
-  void *w_cast, *w_t, *w_cp, *w_tp;   /* as meb200_conv_pack_weights; w_cp / w_tp may be NULL */
+  void *w_cast, *w_t;                 /* as meb200_conv_pack_weights */
   uint32_t K, c_in, c_out;
   uint32_t tile_begin;
 } meb200_pack_job;
@@ -214,7 +229,7 @@ int meb200_conv_pack_weights_batched(const meb200_pack_job *jobs_dev, uint32_t n
  *                              meb200_conv_pack_weights(Wv, K=1, c_in=V, c_out) where
  *                              Wv[4 k + c][n] = W[k][c][n] (zero for padded k, c)
  *   grad_weight_v  [V, c_out]  fp32, same indexing (fully written by the call)
- *   workspace      meb200_conv_wgrad_workspace_bytes(V, c_out, 1, n_out) bytes, 16-byte aligned,
+ *   workspace      meb200_conv_workspace_bytes(n_out, V, c_out, 1, dtype) bytes, 16-byte aligned,
  *                  for the row-split partial sums (less, NULL or unaligned is legal: fewer splits)
  * bf16 / fp16 only; c_out a multiple of 16, <= 256. */
 uint32_t meb200_conv_stem_virtual_channels(uint32_t K);
@@ -226,41 +241,6 @@ int meb200_conv_stem_wgrad(const void *in4, const void *grad_out, int dtype, uin
                            uint32_t c_out, const int32_t *out_nbr, uint32_t n_out,
                            float *grad_weight_v, void *workspace, uint64_t workspace_bytes,
                            void *stream);
-
-/* meb200_conv_forward with the weight already packed (tensor-core path only: returns
- * MEB200_ERR_UNSUPPORTED for shapes/dtypes outside it, the caller then uses
- * meb200_conv_forward).  Same result, no per-call cast/transpose, no workspace.
- * weight_tp (may be NULL) is accepted for compatibility and not read. */
-int meb200_conv_forward_packed(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
-                               const void *weight_t, const void *weight_tp, uint32_t K,
-                               uint32_t c_out, const int32_t *out_nbr, uint32_t n_out, void *out,
-                               int out_dtype, void *stream);
-
-/* meb200_conv_backward on packed weights (w_cast; w_cp is accepted and not read), tensor-core
- * path only;
- * grad_in / grad_weight may be NULL to skip dgrad / wgrad.  pairs_in / pairs_out / seg_start
- * (all three or NULL) + n_chunks: the compacted pair lists of out_nbr from
- * meb200_kernel_map_pairs with stage = 64 and their chunk count; with them wgrad reduces over
- * valid pairs only instead of the dense table.  workspace: as for meb200_conv_stem_wgrad, sized
- * by meb200_conv_wgrad_workspace_bytes(c_in, c_out, K, n_out). */
-int meb200_conv_backward_packed(const void *in, const void *grad_out, int dtype, uint32_t n_in,
-                                uint32_t c_in, const void *w_cast, const void *w_cp, uint32_t K,
-                                uint32_t c_out, const int32_t *out_nbr, const int32_t *in_nbr,
-                                uint32_t n_out, void *grad_in, int grad_in_dtype,
-                                float *grad_weight, const int32_t *pairs_in,
-                                const int32_t *pairs_out, const int32_t *seg_start,
-                                uint32_t n_chunks, void *workspace, uint64_t workspace_bytes,
-                                void *stream);
-
-/* Workspace of meb200_conv_forward / meb200_conv_backward in any dtype: the SIMT wgrad's row
- * splits, and for BF16/F16 the tensor-core weight copy and wgrad splits (0 is legal: slower
- * fallbacks and fewer splits are chosen). */
-uint64_t meb200_conv_workspace_bytes(uint32_t n_in, uint32_t n_out, uint32_t c_in,
-                                     uint32_t c_out, uint32_t K, int dtype);
-/* Workspace for the row-split partial sums of a wgrad over n_out rows (0: none needed).  Row
- * splits add their sums in a fixed order, so wgrad is deterministic for a given workspace size. */
-uint64_t meb200_conv_wgrad_workspace_bytes(uint32_t c_in, uint32_t c_out, uint32_t K,
-                                           uint32_t n_out);
 
 /* ---- local pooling (reference a11: src/pooling_avg_kernel.hpp:40-150,
  *      src/pooling_max_kernel.hpp:35-115, src/local_pooling_cpu.cpp:43-185) ---------- */

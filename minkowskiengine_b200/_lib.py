@@ -40,27 +40,22 @@ PROTOTYPES = {
     "meb200_map_find": (_i32, [_vp, _vp, _u32, _u32, _vp, _u32, _vp, _vp]),
     "meb200_kernel_map": (_i32, [_vp, _u32, _vp, _u32, _vp, _u32, _u32, _vp, _u32, _vp, _vp,
                                  _vp, _vp]),
-    "meb200_conv_forward": (_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _u32, _vp, _u32, _vp,
-                                   _i32, _vp, _u64, _vp]),
+    "meb200_conv_forward": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _u32, _vp,
+                                   _i32, _vp]),
     "meb200_conv_backward": (_i32, [_vp, _vp, _i32, _u32, _u32, _vp, _u32, _u32, _vp, _vp,
-                                    _u32, _vp, _i32, _vp, _vp, _u64, _vp]),
-    "meb200_conv_pack_weights": (_i32, [_vp, _u32, _u32, _u32, _i32, _vp, _vp, _vp, _vp, _vp]),
+                                    _u32, _vp, _i32, _vp, _vp, _vp, _vp, _u32, _vp, _u64, _vp]),
+    "meb200_conv_wgrad_uses_pairs": (_i32, [_i32, _u32, _u32, _u32]),
+    "meb200_conv_pack_weights": (_i32, [_vp, _u32, _u32, _u32, _i32, _vp, _vp, _vp]),
     "meb200_conv_pack_weights_batched": (_i32, [_vp, _u32, _u32, _i32, _vp]),
     "meb200_conv_stem_virtual_channels": (_u32, [_u32]),
     "meb200_conv_stem_supported": (_i32, [_i32, _u32, _u32]),
     "meb200_conv_stem_forward": (_i32, [_vp, _i32, _u32, _vp, _u32, _vp, _u32, _vp, _i32, _vp]),
     "meb200_conv_stem_wgrad": (_i32, [_vp, _vp, _i32, _u32, _u32, _vp, _u32, _vp, _vp, _u64, _vp]),
-    "meb200_conv_forward_packed": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _u32,
-                                          _vp, _i32, _vp]),
-    "meb200_conv_backward_packed": (_i32, [_vp, _vp, _i32, _u32, _u32, _vp, _vp, _u32, _u32, _vp,
-                                           _vp, _u32, _vp, _i32, _vp, _vp, _vp, _vp, _u32, _vp, _u64,
-                                           _vp]),
     "meb200_pair_list_chunks": (_u32, [_u32, _u32]),
     "meb200_pair_list_scratch_bytes": (_u64, [_u32, _u32, _u32]),
     "meb200_pair_list_capacity": (_u64, [_u32, _u32, _u32, _u32]),
     "meb200_kernel_map_pairs": (_i32, [_vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
-    "meb200_conv_workspace_bytes": (_u64, [_u32, _u32, _u32, _u32, _u32, _i32]),
-    "meb200_conv_wgrad_workspace_bytes": (_u64, [_u32, _u32, _u32, _u32]),
+    "meb200_conv_workspace_bytes": (_u64, [_u32, _u32, _u32, _u32, _i32]),
     "meb200_pool_forward": (_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _u32, _i32, _vp, _vp, _vp]),
     "meb200_pool_backward": (_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _u32, _i32, _vp, _vp,
                                     _vp]),

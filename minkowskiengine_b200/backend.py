@@ -187,7 +187,7 @@ class _KernelMap:
     PAIR_STAGE = 64   # pairs per pipeline stage of the wgrad kernel (k_wgrad_wg)
     # table rows per chunk of the pair lists (multiple of 2048): one chunk's rows of both feature
     # matrices stay L2-resident while the wgrad walks its K offsets
-    PAIR_CHUNK_ROWS = int(os.environ.get("MEB200_PAIR_CHUNK_ROWS", "262144"))
+    PAIR_CHUNK_ROWS = 262144
 
     def __init__(self, out_nbr, in_nbr, stride_pairs=None, n_in=None, in_thunk=None):
         # in_nbr may be None with (n_in, in_thunk): the reverse table of a large kernel (the
@@ -873,16 +873,9 @@ def _check_feats(in_feat, manager, in_key, name="in_feat"):
             "!=", manager.size(in_key))
 
 
-def _workspace(n_in, n_out, c_in, c_out, K, code, device):
-    nbytes = int(_lib.load().meb200_conv_workspace_bytes(n_in, n_out, c_in, c_out, K, code))
-    if nbytes == 0:
-        return None, 0
-    return torch.empty(nbytes, dtype=torch.uint8, device=device), nbytes
-
-
-def _wgrad_workspace(c_in, c_out, K, n_out, device):
+def _workspace(n_out, c_in, c_out, K, code, device):
     """Room for the row-split partial sums of a wgrad (added in a fixed order: deterministic)."""
-    nbytes = int(_lib.load().meb200_conv_wgrad_workspace_bytes(c_in, c_out, K, n_out))
+    nbytes = int(_lib.load().meb200_conv_workspace_bytes(n_out, c_in, c_out, K, code))
     if nbytes == 0:
         return None, 0
     return torch.empty(nbytes, dtype=torch.uint8, device=device), nbytes
@@ -938,17 +931,13 @@ def _conv_forward(in_feat, kernel, km, out_dtype=None):
 
 
 # ---- packed weights: one cast + transpose per optimizer step, not per call -------------------
-_PACKED = {}   # id(kernel tensor) -> (weakref, version, data_ptr, dtype, w_cast, w_t)
+_PACKED = {}   # id(kernel tensor) -> (weakref, version, data_ptr, dtype, (w_cast, w_t))
 _ERR_UNSUPPORTED = -3
-
-
-_PACK_BATCHED = os.environ.get("MEB200_PACK_BATCHED", "1") not in ("", "0")
 
 
 class _PackJob(ctypes.Structure):      # == meb200_pack_job (include/meb200.h)
     _fields_ = [("w", ctypes.c_void_p), ("w_cast", ctypes.c_void_p), ("w_t", ctypes.c_void_p),
-                ("w_cp", ctypes.c_void_p), ("w_tp", ctypes.c_void_p), ("K", ctypes.c_uint32),
-                ("c_in", ctypes.c_uint32), ("c_out", ctypes.c_uint32),
+                ("K", ctypes.c_uint32), ("c_in", ctypes.c_uint32), ("c_out", ctypes.c_uint32),
                 ("tile_begin", ctypes.c_uint32)]
 
 
@@ -979,8 +968,7 @@ class _PackTable:
                 continue
             K, c_in, c_out = k.shape
             w_cast, w_t = packed
-            jobs.append(_PackJob(ptr, _lib.ptr(w_cast), _lib.ptr(w_t), None, None, K, c_in, c_out,
-                                 tile))
+            jobs.append(_PackJob(ptr, _lib.ptr(w_cast), _lib.ptr(w_t), K, c_in, c_out, tile))
             tile += K * ((c_in + 31) // 32) * ((c_out + 31) // 32)
             self.order.append(key)
         self.n_jobs, self.total_tiles = len(jobs), tile
@@ -1015,18 +1003,31 @@ class _PackTable:
 _PACK_TABLES = {}      # (device index, dtype) -> _PackTable
 
 
-def _packed_weights(kernel, dtype):
-    """(w_cast [K,Cin,Cout], w_t [K,Cout,Cin]) of an fp32 master weight in `dtype` (the operand-B
-    layouts of dgrad and forward; the permuted copies the packing ABI can also emit are not read
-    by any kernel and are not built), rebuilt only when the tensor was modified in place (its autograd version counter moved) or
-    replaced."""
-    key = id(kernel)
+def _is_master(kernel):
+    """An fp32 contiguous master weight: re-packed with every other one by its _PackTable, and the
+    only kind of kernel the stem kernels and the pair-list wgrad are used for."""
+    return kernel.dtype == torch.float32 and kernel.is_contiguous()
+
+
+def _cached(key, kernel, dtype):
     ent = _PACKED.get(key)
     if ent is not None and ent[0]() is kernel and ent[1] == kernel._version \
             and ent[2] == kernel.data_ptr() and ent[3] == dtype:
         return ent[4]
+    return None
+
+
+def _packed_weights(kernel, dtype):
+    """(w_cast [K,Cin,Cout], w_t [K,Cout,Cin]) of a floating kernel in `dtype` (the operand-B
+    layouts of dgrad and forward), rebuilt only when the tensor was modified in place (its autograd
+    version counter moved) or replaced.  A kernel that is not an fp32 master is packed alone from
+    an fp32 copy: bf16 / fp16 values pass through fp32 exactly, so the bytes are kernel.to(dtype)."""
+    key = id(kernel)
+    packed = _cached(key, kernel, dtype)
+    if packed is not None:
+        return packed
     tbl = None
-    if _PACK_BATCHED:
+    if _is_master(kernel):
         tkey = (kernel.device.index, dtype)
         tbl = _PACK_TABLES.get(tkey)
         if tbl is None:
@@ -1037,12 +1038,12 @@ def _packed_weights(kernel, dtype):
             return _PACKED[key][4]
     lib = _lib.load()
     K, c_in, c_out = kernel.shape
-    src = kernel.detach()
+    src = kernel.detach().float().contiguous()
     buf = torch.empty((2, K * c_in * c_out), dtype=dtype, device=kernel.device)
     w_cast, w_t = buf[0].view(K, c_in, c_out), buf[1].view(K, c_out, c_in)
     _lib.check(lib.meb200_conv_pack_weights(
         _lib.ptr(src), K, c_in, c_out, _lib.dtype_code(dtype), _lib.ptr(w_cast), _lib.ptr(w_t),
-        None, None, _lib.current_stream()))
+        _lib.current_stream()))
     if len(_PACKED) > 4096:      # dead entries of discarded networks
         for k in [k for k, e in _PACKED.items() if e[0]() is None]:
             del _PACKED[k]
@@ -1053,13 +1054,17 @@ def _packed_weights(kernel, dtype):
     return packed
 
 
-_STEM = os.environ.get("MEB200_STEM_TC", "1") not in ("", "0")
+def _feature_weights(kernel, dtype):
+    """(w_cast, w_t) for features of `dtype`; fp32 features read the kernel itself (no w_t)."""
+    if dtype == torch.float32:
+        return kernel.float().contiguous(), None
+    return _packed_weights(kernel, dtype)
 
 
 def _is_stem(kernel, feat_dtype):
     """Layers with <= 4 input channels (the stem of a network) on the bf16/fp16 path: run over
     virtual channels (offset, channel) by the stem kernels (include/meb200.h)."""
-    if not (_STEM and kernel.dim() == 3 and kernel.shape[1] <= 4 and _can_pack(kernel, feat_dtype)):
+    if not (kernel.dim() == 3 and kernel.shape[1] <= 4 and _is_master(kernel)):
         return False
     return bool(_lib.load().meb200_conv_stem_supported(_lib.dtype_code(feat_dtype), kernel.shape[0],
                                                        kernel.shape[2]))
@@ -1068,10 +1073,9 @@ def _is_stem(kernel, feat_dtype):
 def _stem_weights(kernel, dtype):
     """Packed weights of the stem's virtual K = 1 layer, [c_out, V] (cached like _packed_weights)."""
     key = (id(kernel), "stem")
-    ent = _PACKED.get(key)
-    if ent is not None and ent[0]() is kernel and ent[1] == kernel._version \
-            and ent[2] == kernel.data_ptr() and ent[3] == dtype:
-        return ent[4]
+    w_v = _cached(key, kernel, dtype)
+    if w_v is not None:
+        return w_v
     lib = _lib.load()
     K, c_in, c_out = kernel.shape
     V = int(lib.meb200_conv_stem_virtual_channels(K))
@@ -1080,7 +1084,7 @@ def _stem_weights(kernel, dtype):
     buf = torch.empty((2, V * c_out), dtype=dtype, device=kernel.device)
     _lib.check(lib.meb200_conv_pack_weights(
         _lib.ptr(wv), 1, V, c_out, _lib.dtype_code(dtype), _lib.ptr(buf[0]), _lib.ptr(buf[1]),
-        None, None, _lib.current_stream()))
+        _lib.current_stream()))
     w_v = buf[1].view(c_out, V)
     _PACKED[key] = (weakref.ref(kernel), kernel._version, kernel.data_ptr(), dtype, w_v)
     return w_v
@@ -1091,19 +1095,13 @@ def _pad4(feat):
     return feat.contiguous() if c == 4 else torch.nn.functional.pad(feat, (0, 4 - c))
 
 
-def _can_pack(kernel, feat_dtype):
-    return (kernel.dtype == torch.float32 and feat_dtype in (torch.bfloat16, torch.float16)
-            and kernel.is_contiguous() and kernel.dim() == 3)
-
-
 def _conv_forward_impl(in_feat, kernel, km, out_dtype=None):
     lib = _lib.load()
     code = _lib.dtype_code(in_feat.dtype)
+    K, c_in, c_out = kernel.shape
+    _assert(K == km.K, "kernel volume", K, "does not match the kernel map", km.K)
+    out = torch.empty((km.n_out, c_out), dtype=out_dtype or in_feat.dtype, device=in_feat.device)
     if _is_stem(kernel, in_feat.dtype):
-        K, c_in, c_out = kernel.shape
-        _assert(K == km.K, "kernel volume", K, "does not match the kernel map", km.K)
-        out = torch.empty((km.n_out, c_out), dtype=out_dtype or in_feat.dtype,
-                          device=in_feat.device)
         # (named, so that they outlive the argument list: a temporary freed before the call can
         # be handed by the allocator to the next temporary and overwritten before the kernel runs)
         in4, w_v = _pad4(in_feat), _stem_weights(kernel, in_feat.dtype)
@@ -1113,30 +1111,10 @@ def _conv_forward_impl(in_feat, kernel, km, out_dtype=None):
         if rc != _ERR_UNSUPPORTED:
             _lib.check(rc)
             return out
-    if _can_pack(kernel, in_feat.dtype):
-        K, c_in, c_out = kernel.shape
-        _assert(K == km.K, "kernel volume", K, "does not match the kernel map", km.K)
-        _, w_t = _packed_weights(kernel, in_feat.dtype)
-        out = torch.empty((km.n_out, c_out), dtype=out_dtype or in_feat.dtype,
-                          device=in_feat.device)
-        rc = lib.meb200_conv_forward_packed(
-            _lib.ptr(in_feat), code, km.n_in, c_in, _lib.ptr(w_t), None, K, c_out,
-            _lib.ptr(km.out_nbr), km.n_out, _lib.ptr(out), _lib.dtype_code(out.dtype),
-            _lib.current_stream())
-        if rc != _ERR_UNSUPPORTED:
-            _lib.check(rc)
-            return out
-    if kernel.dtype != in_feat.dtype:
-        kernel = kernel.to(in_feat.dtype)
-    kernel = kernel.contiguous()
-    K, c_in, c_out = kernel.shape
-    _assert(K == km.K, "kernel volume", K, "does not match the kernel map", km.K)
-    n_out, n_in = km.n_out, km.n_in
-    out = torch.empty((n_out, c_out), dtype=out_dtype or in_feat.dtype, device=in_feat.device)
-    ws, ws_bytes = _workspace(n_in, n_out, c_in, c_out, K, code, in_feat.device)
+    w_cast, w_t = _feature_weights(kernel, in_feat.dtype)
     _lib.check(lib.meb200_conv_forward(
-        _lib.ptr(in_feat), code, n_in, c_in, _lib.ptr(kernel), K, c_out, _lib.ptr(km.out_nbr),
-        n_out, _lib.ptr(out), _lib.dtype_code(out.dtype), _lib.ptr(ws), ws_bytes,
+        _lib.ptr(in_feat), code, km.n_in, c_in, _lib.ptr(w_cast), _lib.ptr(w_t), K, c_out,
+        _lib.ptr(km.out_nbr), km.n_out, _lib.ptr(out), _lib.dtype_code(out.dtype),
         _lib.current_stream()))
     return out
 
@@ -1177,37 +1155,28 @@ def _conv_backward_impl(in_feat, grad_out, kernel, km, need_in=True, need_w=True
         V = int(lib.meb200_conv_stem_virtual_channels(K))
         gwv = torch.empty((V // 4, 4, c_out), dtype=torch.float32, device=in_feat.device)
         in4 = _pad4(in_feat)
-        ws, ws_bytes = _wgrad_workspace(V, c_out, 1, n_out, in_feat.device)
+        ws, ws_bytes = _workspace(n_out, V, c_out, 1, code, in_feat.device)
         rc = lib.meb200_conv_stem_wgrad(
             _lib.ptr(in4), _lib.ptr(grad_out), code, K, c_out, _lib.ptr(km.out_nbr),
             n_out, _lib.ptr(gwv), _lib.ptr(ws), ws_bytes, _lib.current_stream())
         if rc != _ERR_UNSUPPORTED:
             _lib.check(rc)
             return None, gwv[:K, :c_in].contiguous()
-    if _can_pack(kernel, in_feat.dtype):
-        w, _ = _packed_weights(kernel, in_feat.dtype)
-        pin = pout = seg = None
-        nch = 0
-        if need_w and c_in % 8 == 0 and c_in >= 16 and K <= 1023:
+    w_cast, _ = _feature_weights(kernel, in_feat.dtype)
+    pin = pout = seg = None
+    nch = 0
+    ws, ws_bytes = None, 0
+    if need_w:
+        # a kernel that is not an fp32 master keeps the dense-table wgrad: the two reduce in
+        # different orders, so switching would change its bits
+        if _is_master(kernel) and lib.meb200_conv_wgrad_uses_pairs(code, c_in, c_out, K):
             pin, pout, seg, nch = km.pair_lists()
-        ws, ws_bytes = _wgrad_workspace(c_in, c_out, K, n_out, in_feat.device) if need_w \
-            else (None, 0)
-        rc = lib.meb200_conv_backward_packed(
-            _lib.ptr(in_feat), _lib.ptr(grad_out), code, n_in, c_in, _lib.ptr(w), None,
-            K, c_out, _lib.ptr(km.out_nbr), _lib.ptr(km.in_nbr) if need_in else None, n_out,
-            _lib.ptr(grad_in), code, _lib.ptr(grad_w), _lib.ptr(pin), _lib.ptr(pout), _lib.ptr(seg), nch,
-            _lib.ptr(ws), ws_bytes, _lib.current_stream())
-        if rc != _ERR_UNSUPPORTED:
-            _lib.check(rc)
-            return grad_in, grad_w
-    else:
-        w = kernel if kernel.dtype == in_feat.dtype else kernel.to(in_feat.dtype)
-        w = w.contiguous()
-    ws, ws_bytes = _workspace(n_in, n_out, c_in, c_out, K, code, in_feat.device)
+        ws, ws_bytes = _workspace(n_out, c_in, c_out, K, code, in_feat.device)
     _lib.check(lib.meb200_conv_backward(
-        _lib.ptr(in_feat), _lib.ptr(grad_out), code, n_in, c_in, _lib.ptr(w), K, c_out,
+        _lib.ptr(in_feat), _lib.ptr(grad_out), code, n_in, c_in, _lib.ptr(w_cast), K, c_out,
         _lib.ptr(km.out_nbr), _lib.ptr(km.in_nbr) if need_in else None, n_out, _lib.ptr(grad_in),
-        code, _lib.ptr(grad_w), _lib.ptr(ws), ws_bytes, _lib.current_stream()))
+        code, _lib.ptr(grad_w), _lib.ptr(pin), _lib.ptr(pout), _lib.ptr(seg), nch, _lib.ptr(ws),
+        ws_bytes, _lib.current_stream()))
     if grad_w is not None and grad_w.dtype != kernel.dtype:
         grad_w = grad_w.to(kernel.dtype)
     return grad_in, grad_w

@@ -348,39 +348,16 @@ k_wgrad_sum(const float4 *__restrict__ partial, float4 *__restrict__ dW, size_t 
 }
 
 // ---- weight packing ----------------------------------------------------------------------------
-// Wb[k][n][c] = W[k][c][n]  (forward operand B: reduction dim contiguous)
+// Per-optimizer-step weight packing: fp32 master W[k][ci][co] -> feature dtype in the two
+// operand-B layouts of the wgmma kernels, in one pass:
+//   Wc [k][ci][co]  dgrad operand B            Wt [k][co][ci]  forward operand B
+// One CTA packs the 32 x 32 tile (k, ci0.., co0..).
 template <typename T>
-__global__ void __launch_bounds__(256)
-k_transpose_w(const T *__restrict__ W, T *__restrict__ Wb, uint32_t c_in, uint32_t c_out) {
-  __shared__ T tile[32][33];
-  const T *Wk = W + (size_t)blockIdx.z * c_in * c_out;
-  T *Wbk = Wb + (size_t)blockIdx.z * c_in * c_out;
-  uint32_t ci0 = blockIdx.y * 32, co0 = blockIdx.x * 32;
-  uint32_t tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  for (uint32_t i = ty; i < 32; i += 8)
-    if (ci0 + i < c_in && co0 + tx < c_out) tile[i][tx] = Wk[(size_t)(ci0 + i) * c_out + co0 + tx];
-  __syncthreads();
-  for (uint32_t i = ty; i < 32; i += 8)
-    if (co0 + i < c_out && ci0 + tx < c_in) Wbk[(size_t)(co0 + i) * c_in + ci0 + tx] = tile[tx][i];
-}
-
-// Per-optimizer-step weight packing: fp32 master W[k][ci][co] -> feature dtype in the operand-B
-// layouts of the packed-weight ABI (include/meb200.h), in one pass (replaces a torch cast plus
-// k_transpose_w on EVERY forward call):
-//   Wc  [k][ci][co]     dgrad operand B          Wt  [k][co][ci]     forward operand B
-//   Wcp [k][ci][perm(co)]                        Wtp [k][co][perm(ci)]
-// perm permutes each 32-channel block of the reduction axis; the wgmma kernels read Wc / Wt, the
-// permuted copies are produced only when the caller asks for them (non-NULL w_cp / w_tp).
-__host__ __device__ constexpr uint32_t ta_perm(uint32_t pos) {   // position -> channel, within 32
-  return 8u * ((pos >> 2) & 3u) + 4u * ((pos >> 4) & 1u) + (pos & 3u);
-}
-template <typename T>
-__global__ void __launch_bounds__(256)
-k_pack_w(const float *__restrict__ W, T *__restrict__ Wc, T *__restrict__ Wt, T *__restrict__ Wcp,
-         T *__restrict__ Wtp, uint32_t c_in, uint32_t c_out) {
+__device__ __forceinline__ void pack_tile(const float *__restrict__ W, T *__restrict__ Wc,
+                                          T *__restrict__ Wt, uint32_t c_in, uint32_t c_out,
+                                          uint32_t k, uint32_t ci0, uint32_t co0) {
   __shared__ float tile[32][33];
-  const size_t base = (size_t)blockIdx.z * c_in * c_out;
-  const uint32_t ci0 = blockIdx.y * 32, co0 = blockIdx.x * 32;
+  const size_t base = (size_t)k * c_in * c_out;
   const uint32_t tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   for (uint32_t i = ty; i < 32; i += 8)
     if (ci0 + i < c_in && co0 + tx < c_out) {
@@ -389,15 +366,16 @@ k_pack_w(const float *__restrict__ W, T *__restrict__ Wc, T *__restrict__ Wt, T 
       Wc[base + (size_t)(ci0 + i) * c_out + co0 + tx] = from_f32<T>(v);
     }
   __syncthreads();
-  const uint32_t px = ta_perm(tx);
-  for (uint32_t i = ty; i < 32; i += 8) {
+  for (uint32_t i = ty; i < 32; i += 8)
     if (co0 + i < c_out && ci0 + tx < c_in)
       Wt[base + (size_t)(co0 + i) * c_in + ci0 + tx] = from_f32<T>(tile[tx][i]);
-    if (Wtp != nullptr && co0 + i < c_out)      // c_in % 32 == 0: the tile is a full block
-      Wtp[base + (size_t)(co0 + i) * c_in + ci0 + tx] = from_f32<T>(tile[px][i]);
-    if (Wcp != nullptr && ci0 + i < c_in)       // c_out % 32 == 0
-      Wcp[base + (size_t)(ci0 + i) * c_out + co0 + tx] = from_f32<T>(tile[i][px]);
-  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256)
+k_pack_w(const float *__restrict__ W, T *__restrict__ Wc, T *__restrict__ Wt, uint32_t c_in,
+         uint32_t c_out) {
+  pack_tile<T>(W, Wc, Wt, c_in, c_out, blockIdx.z, blockIdx.y * 32, blockIdx.x * 32);
 }
 
 // All layers of a network in ONE launch (the weights of every layer change together, at the
@@ -406,7 +384,6 @@ k_pack_w(const float *__restrict__ W, T *__restrict__ Wc, T *__restrict__ Wt, T 
 template <typename T>
 __global__ void __launch_bounds__(256)
 k_pack_w_batched(const PackJob *__restrict__ jobs, uint32_t n_jobs) {
-  __shared__ float tile[32][33];
   uint32_t lo = 0, hi = n_jobs - 1;
   while (lo < hi) {                       // last job whose tile_begin <= blockIdx.x
     const uint32_t mid = (lo + hi + 1) >> 1;
@@ -418,28 +395,8 @@ k_pack_w_batched(const PackJob *__restrict__ jobs, uint32_t n_jobs) {
   uint32_t t = blockIdx.x - job.tile_begin;
   const uint32_t bx = t % tx_n; t /= tx_n;
   const uint32_t by = t % ty_n, bz = t / ty_n;
-  const float *W = reinterpret_cast<const float *>(job.w);
-  T *Wc = reinterpret_cast<T *>(job.w_cast), *Wt = reinterpret_cast<T *>(job.w_t);
-  T *Wcp = reinterpret_cast<T *>(job.w_cp), *Wtp = reinterpret_cast<T *>(job.w_tp);
-  const size_t base = (size_t)bz * c_in * c_out;
-  const uint32_t ci0 = by * 32, co0 = bx * 32;
-  const uint32_t tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  for (uint32_t i = ty; i < 32; i += 8)
-    if (ci0 + i < c_in && co0 + tx < c_out) {
-      const float v = W[base + (size_t)(ci0 + i) * c_out + co0 + tx];
-      tile[i][tx] = v;
-      Wc[base + (size_t)(ci0 + i) * c_out + co0 + tx] = from_f32<T>(v);
-    }
-  __syncthreads();
-  const uint32_t px = ta_perm(tx);
-  for (uint32_t i = ty; i < 32; i += 8) {
-    if (co0 + i < c_out && ci0 + tx < c_in)
-      Wt[base + (size_t)(co0 + i) * c_in + ci0 + tx] = from_f32<T>(tile[tx][i]);
-    if (Wtp != nullptr && co0 + i < c_out)
-      Wtp[base + (size_t)(co0 + i) * c_in + ci0 + tx] = from_f32<T>(tile[px][i]);
-    if (Wcp != nullptr && ci0 + i < c_in)
-      Wcp[base + (size_t)(ci0 + i) * c_out + co0 + tx] = from_f32<T>(tile[i][px]);
-  }
+  pack_tile<T>(reinterpret_cast<const float *>(job.w), reinterpret_cast<T *>(job.w_cast),
+               reinterpret_cast<T *>(job.w_t), c_in, c_out, bz, by * 32, bx * 32);
 }
 
 int conv_pack_weights_batched(const PackJob *jobs_dev, uint32_t n_jobs, uint32_t total_tiles,
@@ -454,17 +411,13 @@ int conv_pack_weights_batched(const PackJob *jobs_dev, uint32_t n_jobs, uint32_t
 }
 
 int conv_pack_weights(const float *W, uint32_t K, uint32_t c_in, uint32_t c_out, int dtype,
-                      void *w_cast, void *w_t, void *w_cp, void *w_tp, cudaStream_t stream) {
-  if (c_out % 32 != 0) w_cp = nullptr;
-  if (c_in % 32 != 0) w_tp = nullptr;
+                      void *w_cast, void *w_t, cudaStream_t stream) {
   dim3 grid(cdiv(c_out, 32), cdiv(c_in, 32), K);
   if (dtype == MEB200_BF16)
-    k_pack_w<__nv_bfloat16><<<grid, 256, 0, stream>>>(
-        W, (__nv_bfloat16 *)w_cast, (__nv_bfloat16 *)w_t, (__nv_bfloat16 *)w_cp,
-        (__nv_bfloat16 *)w_tp, c_in, c_out);
+    k_pack_w<__nv_bfloat16><<<grid, 256, 0, stream>>>(W, (__nv_bfloat16 *)w_cast,
+                                                      (__nv_bfloat16 *)w_t, c_in, c_out);
   else
-    k_pack_w<__half><<<grid, 256, 0, stream>>>(W, (__half *)w_cast, (__half *)w_t, (__half *)w_cp,
-                                               (__half *)w_tp, c_in, c_out);
+    k_pack_w<__half><<<grid, 256, 0, stream>>>(W, (__half *)w_cast, (__half *)w_t, c_in, c_out);
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
@@ -582,30 +535,17 @@ bool conv_tc_supported(int dtype, uint32_t c_reduce, uint32_t c_cols) {
   return c_cols % 16 == 0 && c_cols >= 16 && c_cols <= 1024;
 }
 
-int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *W,
-                    uint32_t K, uint32_t c_cols, bool dgrad, const int32_t *nbr, uint32_t n_rows,
-                    void *out, int out_dtype, void *workspace, cudaStream_t stream) {
+int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *B,
+                    uint32_t K, uint32_t c_cols, const int32_t *nbr, uint32_t n_rows, void *out,
+                    int out_dtype, cudaStream_t stream) {
   if (n_rows == 0) return MEB200_OK;
   MEB_CHECK_ARG(conv_tc_supported(dtype, c_reduce, c_cols), "shape not supported by tc path");
-  if (!aligned16(A) || !aligned16(W) || (!dgrad && !aligned16(workspace))) {
+  if (!aligned16(A) || !aligned16(B)) {
     set_error("conv tc: operands must be 16-byte aligned");
     return MEB200_ERR_UNSUPPORTED;
   }
-  const uint8_t *Wb = reinterpret_cast<const uint8_t *>(W);
-  if (!dgrad) {
-    // forward: B_k = W[k]^T so that the reduction dim (c_in) is contiguous
-    MEB_CHECK_ARG(workspace != nullptr, "workspace required");
-    dim3 grid(cdiv(c_cols, 32), cdiv(c_reduce, 32), K);
-    if (dtype == MEB200_BF16)
-      k_transpose_w<__nv_bfloat16><<<grid, 256, 0, stream>>>(
-          (const __nv_bfloat16 *)W, (__nv_bfloat16 *)workspace, c_reduce, c_cols);
-    else
-      k_transpose_w<__half><<<grid, 256, 0, stream>>>((const __half *)W, (__half *)workspace,
-                                                     c_reduce, c_cols);
-    MEB_LAUNCH_OK();
-    Wb = reinterpret_cast<const uint8_t *>(workspace);
-  }
-  // operand B is [K, c_cols, c_reduce]; one launch per slice of <= 256 output columns
+  const uint8_t *Wb = reinterpret_cast<const uint8_t *>(B);
+  // one launch per slice of <= 256 output columns
   const size_t out_esz = out_dtype == MEB200_F32 ? 4 : 2;
   for (uint32_t n0 = 0; n0 < c_cols; n0 += tc::kMaxCols) {
     FwdParams p{};
@@ -695,8 +635,9 @@ int conv_wgrad_tc(const void *in, const void *grad_out, int dtype, uint32_t c_in
   return run_wgrad(dtype, p, K, cdiv(n_out, tc::kWgRows), workspace, workspace_bytes, stream);
 }
 
-bool conv_wgrad_pairs_supported(int dtype, uint32_t c_in, uint32_t K, uint32_t c_out) {
-  return K >= 1 && K <= 65535 && conv_wgrad_tc_supported(dtype, c_in, c_out);
+// K <= 1023 keeps the segment count (chunks * K) of the chunked lists in range
+bool conv_wgrad_uses_pairs(int dtype, uint32_t c_in, uint32_t c_out, uint32_t K) {
+  return K >= 1 && K <= 1023 && conv_wgrad_tc_supported(dtype, c_in, c_out);
 }
 
 int conv_wgrad_pairs(const void *in, const void *grad_out, int dtype, uint32_t c_in, uint32_t K,
@@ -704,7 +645,7 @@ int conv_wgrad_pairs(const void *in, const void *grad_out, int dtype, uint32_t c
                      const int32_t *seg_start, uint32_t n_chunks, uint32_t n_out,
                      float *grad_weight, void *workspace, uint64_t workspace_bytes,
                      cudaStream_t stream) {
-  if (!conv_wgrad_pairs_supported(dtype, c_in, K, c_out) || !aligned16(in) || !aligned16(grad_out)) {
+  if (!conv_wgrad_uses_pairs(dtype, c_in, c_out, K) || !aligned16(in) || !aligned16(grad_out)) {
     set_error("wgrad pairs: shape or alignment outside the tensor-core path (c_in=%u c_out=%u K=%u)",
               c_in, c_out, K);
     return MEB200_ERR_UNSUPPORTED;

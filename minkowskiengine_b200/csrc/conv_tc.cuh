@@ -8,22 +8,20 @@ namespace meb200 {
 bool conv_tc_supported(int dtype, uint32_t c_reduce, uint32_t c_cols);
 bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out);
 
-// out[r,:] = sum_k A[nbr[k][r],:] @ Wk  with Wk = W[k] (forward) or W[k]^T (dgrad).
-// W is always the layer's [K, c_in, c_out] tensor; for dgrad c_reduce = c_out and
-// c_cols = c_in.  `workspace` receives the re-laid-out operand-B copy of W.
-int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *W,
-                    uint32_t K, uint32_t c_cols, bool dgrad, const int32_t *nbr, uint32_t n_rows,
-                    void *out, int out_dtype, void *workspace, cudaStream_t stream);
+// out[r,:] = sum_k A[nbr[k][r],:] @ B[k]^T with B [K, c_cols, c_reduce] (reduction contiguous):
+// the forward passes w_t [K, c_out, c_in], the dgrad the layer's w_cast [K, c_in, c_out].
+int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *B,
+                    uint32_t K, uint32_t c_cols, const int32_t *nbr, uint32_t n_rows, void *out,
+                    int out_dtype, cudaStream_t stream);
 
-// fp32 W[K,c_in,c_out] -> w_cast [K,c_in,c_out], w_t [K,c_out,c_in] and the permuted copies
-// w_cp / w_tp (reduction axis permuted within 32-channel blocks; may be NULL) in bf16/fp16.
+// fp32 W[K,c_in,c_out] -> w_cast [K,c_in,c_out] and w_t [K,c_out,c_in] in bf16/fp16.
 int conv_pack_weights(const float *W, uint32_t K, uint32_t c_in, uint32_t c_out, int dtype,
-                      void *w_cast, void *w_t, void *w_cp, void *w_tp, cudaStream_t stream);
+                      void *w_cast, void *w_t, cudaStream_t stream);
 
 // One job of conv_pack_weights_batched == one meb200_pack_job of include/meb200.h.
 struct PackJob {
   const void *w;                      // fp32 [K, c_in, c_out]
-  void *w_cast, *w_t, *w_cp, *w_tp;   // as conv_pack_weights (w_cp / w_tp may be NULL)
+  void *w_cast, *w_t;                 // as conv_pack_weights
   uint32_t K, c_in, c_out;
   uint32_t tile_begin;                // first 32x32 tile of this job in the launch
 };
@@ -39,8 +37,8 @@ int conv_wgrad_tc(const void *in, const void *grad_out, int dtype, uint32_t c_in
 // on the order in which CTAs finish (the splits' partial sums are added in a fixed order).
 uint64_t conv_wgrad_workspace_bytes(uint32_t c_in, uint32_t c_out, uint32_t K, uint32_t n_out);
 
-// wgrad over the compacted pair lists of meb200_kernel_map_pairs.
-bool conv_wgrad_pairs_supported(int dtype, uint32_t c_in, uint32_t K, uint32_t c_out);
+// wgrad over the compacted pair lists of meb200_kernel_map_pairs (meb200_conv_wgrad_uses_pairs).
+bool conv_wgrad_uses_pairs(int dtype, uint32_t c_in, uint32_t c_out, uint32_t K);
 int conv_wgrad_pairs(const void *in, const void *grad_out, int dtype, uint32_t c_in, uint32_t K,
                      uint32_t c_out, const int32_t *pairs_in, const int32_t *pairs_out,
                      const int32_t *seg_start, uint32_t n_chunks, uint32_t n_out,

@@ -135,16 +135,17 @@ def test_route_forward_dgrad_wgrad(ME, cuda, case, dtype):
     with _Route(False, f"{case} wgrad"):
         _, gw = backend._conv_backward(feats, gout, w, km, need_in=False, need_w=True)
         _, gw2 = backend._conv_backward(feats, gout, w, km, need_in=False, need_w=True)
+    assert km._pairs is None, f"{case}: pair lists built for a wgrad that does not read them"
     assert gw.dtype == torch.float32
     assert_one_rounding(gw, gw_ref, gw_A, f"{case} wgrad")
     assert torch.equal(gw, gw2), f"{case} wgrad differs run to run"
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16], ids=["bf16", "fp16"])
-def test_simt_dgrad_with_dense_table_tc_wgrad(ME, cuda, dtype):
-    """24 -> 32: the dgrad (24 output columns) is off the grid, the wgrad is not.  The packed
-    backward is all-or-nothing, so the layer falls back to meb200_conv_backward: SIMT dgrad and
-    `k_wgrad_wg` over the dense table (not the pair lists)."""
+def test_simt_dgrad_with_tc_wgrad(ME, cuda, dtype):
+    """24 -> 32: the dgrad (24 output columns) is off the grid, the wgrad is not.  Each picks its
+    kernel on its own: SIMT dgrad, `k_wgrad_wg` over the pair lists, whose bits do not depend on
+    whether the dgrad ran in the same call."""
     from minkowskiengine_b200 import backend
     cin, cout, n_in, n_out, K = 24, 32, 30_000, 30_000, 27
     feats, gout, w = _inputs(cin, cout, n_in, n_out, K, dtype, cuda, seed=2432)
@@ -154,13 +155,35 @@ def test_simt_dgrad_with_dense_table_tc_wgrad(ME, cuda, dtype):
     km = backend._KernelMap(out_nbr, in_nbr)
     with _Route(False, "24->32 dgrad alone"):
         backend._conv_backward(feats, gout, w, km, need_in=True, need_w=False)
+    with _Route(True, "24->32 wgrad alone"):
+        _, gw_alone = backend._conv_backward(feats, gout, w, km, need_in=False, need_w=True)
     with _Route(True, "24->32 dgrad + wgrad"):
         gi, gw = backend._conv_backward(feats, gout, w, km, need_in=True, need_w=True)
         _, gw2 = backend._conv_backward(feats, gout, w, km, need_in=True, need_w=True)
+    assert km._pairs is not None
     gi_ref, gi_A = ref_conv(gout, wl.transpose(1, 2), _pairs(in_nbr), n_in)
     assert_one_rounding(gi, gi_ref, gi_A, "24->32 dgrad")
     gw_ref, gw_A = ref_wgrad(feats, gout, _pairs(out_nbr))
-    assert_one_rounding(gw, gw_ref, gw_A, "24->32 dense-table wgrad")
+    assert_one_rounding(gw, gw_ref, gw_A, "24->32 pair-list wgrad")
+    assert torch.equal(gw, gw2)
+    assert torch.equal(gw, gw_alone), "the wgrad depends on whether dgrad was requested"
+
+
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16], ids=["bf16", "fp16"])
+def test_dense_table_tc_wgrad_large_kernel(ME, cuda, dtype):
+    """32 -> 32 with an 11^3 kernel: K > 1023 is past the pair lists' range, so the wgrad is
+    `k_wgrad_wg` over the dense neighbour table (thousands of pairs per offset, as in a layer)."""
+    from minkowskiengine_b200 import backend
+    cin, cout, n, K = 32, 32, 3_000, 11 ** 3
+    feats, gout, w = _inputs(cin, cout, n, n, K, dtype, cuda, seed=1331)
+    out_nbr = _table(K, n, n, 0.9, seed=7, device=cuda)
+    km = backend._KernelMap(out_nbr, torch.full((K, n), -1, dtype=torch.int32, device=cuda))
+    with _Route(True, "11^3 wgrad"):
+        _, gw = backend._conv_backward(feats, gout, w, km, need_in=False, need_w=True)
+        _, gw2 = backend._conv_backward(feats, gout, w, km, need_in=False, need_w=True)
+    assert km._pairs is None
+    gw_ref, gw_A = ref_wgrad(feats, gout, _pairs(out_nbr))
+    assert_one_rounding(gw, gw_ref, gw_A, "11^3 dense-table wgrad")
     assert torch.equal(gw, gw2)
 
 

@@ -231,13 +231,13 @@ def test_wgrad_pairs_many_chunks(ME, cuda, monkeypatch):
     assert (gw - ref).abs().max().item() / ref.abs().max().item() < 2e-5
 
 
-def test_batched_weight_packing_equals_single(ME, cuda):
+def test_batched_weight_packing_equals_single_and_cast(ME, cuda):
     """The one-launch re-pack of every registered kernel (backend._PackTable,
     meb200_conv_pack_weights_batched) must leave exactly the bytes the per-kernel packing leaves,
-    for ragged and 32-aligned channel counts, and track tensors that die or move."""
+    which are the kernel cast to the feature dtype (and its per-offset transpose), for ragged and
+    32-aligned channel counts, and track tensors that die or move."""
     from minkowskiengine_b200 import backend, _lib
     lib = _lib.load()
-    assert backend._PACK_BATCHED
     dtype = torch.bfloat16
     g = torch.Generator().manual_seed(5)
     shapes = [(27, 32, 64), (8, 96, 96), (1, 5, 7), (27, 48, 20), (125, 64, 32), (3, 256, 128)]
@@ -245,18 +245,18 @@ def test_batched_weight_packing_equals_single(ME, cuda):
 
     def single(k):
         K, ci, co = k.shape
-        buf = torch.empty((4, K * ci * co), dtype=dtype, device=cuda)
+        buf = torch.empty((2, K * ci * co), dtype=dtype, device=cuda)
         _lib.check(lib.meb200_conv_pack_weights(
-            _lib.ptr(k.detach()), K, ci, co, _lib.dtype_code(dtype), _lib.ptr(buf[0]), _lib.ptr(buf[1]),
-            _lib.ptr(buf[2]) if co % 32 == 0 else None, _lib.ptr(buf[3]) if ci % 32 == 0 else None,
-            _lib.current_stream()))
-        return buf, co % 32 == 0, ci % 32 == 0
+            _lib.ptr(k.detach()), K, ci, co, _lib.dtype_code(dtype), _lib.ptr(buf[0]),
+            _lib.ptr(buf[1]), _lib.current_stream()))
+        return buf
 
     def check(k):
         got = backend._packed_weights(k, dtype)
-        ref = single(k)[0]
+        ref = single(k)
         assert torch.equal(got[0].flatten(), ref[0]) and torch.equal(got[1].flatten(), ref[1])
-        assert len(got) == 2              # the permuted copies are not built by the host
+        assert torch.equal(got[0], k.detach().to(dtype))
+        assert torch.equal(got[1], k.detach().to(dtype).transpose(1, 2))
 
     for k in ks:            # first sight: packed one by one, registered
         check(k)

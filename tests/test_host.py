@@ -25,20 +25,19 @@ def test_library_exports_every_declared_symbol():
     assert ME._lib.load().meb200_build_arch() == b"sm_90a"
 
 
-def test_library_pure_helpers_without_gpu():
+def test_library_helpers_and_wgrad_workspace_without_gpu():
     import minkowskiengine_b200 as ME
     lib = ME._lib.load()
     cap = lib.meb200_hash_capacity(100000)
     assert cap >= 200000 and cap & (cap - 1) == 0
     assert lib.meb200_insert_scratch_bytes(1000) >= 8000
     assert lib.meb200_launch_count() == 0 or lib.meb200_launch_count() > 0
-    assert lib.meb200_conv_workspace_bytes(10, 10, 64, 128, 27, ME._lib.F32) == 0
-    assert lib.meb200_conv_workspace_bytes(10, 10, 64, 128, 27, ME._lib.BF16) >= 27 * 64 * 128 * 2
+    assert lib.meb200_conv_workspace_bytes(10, 64, 128, 27, ME._lib.F32) == 0
     # the SIMT weight gradients keep their row splits' partial sums in the workspace, in any
     # dtype: the MinkUNet head (96 -> 20, K = 1) and a stem (3 -> 20, K = 125) at 200k rows
     for dt in (ME._lib.F32, ME._lib.BF16, ME._lib.F16):
-        assert lib.meb200_conv_workspace_bytes(0, 200000, 96, 20, 1, dt) >= 2 * 96 * 20 * 4
-        assert lib.meb200_conv_workspace_bytes(0, 200000, 3, 20, 125, dt) >= 2 * 125 * 3 * 20 * 4
+        assert lib.meb200_conv_workspace_bytes(200000, 96, 20, 1, dt) >= 2 * 96 * 20 * 4
+        assert lib.meb200_conv_workspace_bytes(200000, 3, 20, 125, dt) >= 2 * 125 * 3 * 20 * 4
 
 
 def test_coordinate_map_key_semantics():
@@ -253,7 +252,7 @@ def test_batchnorm_host_path_runs_against_a_stub_library(monkeypatch):
     assert isinstance(ME.MinkowskiSyncBatchNorm(16).bn, torch.nn.SyncBatchNorm)
 
 
-def test_pack_table_bookkeeping_against_a_stub_library(monkeypatch):
+def test_two_copy_pack_table_against_a_stub_library(monkeypatch):
     """backend._PackTable (one batched re-pack launch for every registered kernel) driven with CPU
     tensors and the native library replaced by a recorder: first sight packs a kernel alone and
     registers it; a stale registered kernel triggers ONE batched call that refreshes every entry;
@@ -272,7 +271,6 @@ def test_pack_table_bookkeeping_against_a_stub_library(monkeypatch):
 
     monkeypatch.setattr(_lib, "load", lambda: Stub())
     monkeypatch.setattr(_lib, "current_stream", lambda: None)
-    monkeypatch.setattr(B, "_PACK_BATCHED", True)
     B._PACKED.clear()
     B._PACK_TABLES.clear()
     dtype = torch.bfloat16
@@ -282,8 +280,6 @@ def test_pack_table_bookkeeping_against_a_stub_library(monkeypatch):
         p = B._packed_weights(k, dtype)
         assert p[0].shape == k.shape and p[1].shape == (k.shape[0], k.shape[2], k.shape[1])
     assert [c[0] for c in calls] == ["meb200_conv_pack_weights"] * 3
-    assert all(len(B._packed_weights(k, dtype)) == 2 for k in ks)         # no permuted copies built
-    assert all(c[1][7] is None and c[1][8] is None for c in calls)
     tbl = B._PACK_TABLES[(None, dtype)]
     assert len(tbl.entries) == 3 and tbl.jobs_dev is None                  # table built lazily
     calls.clear()
@@ -299,8 +295,8 @@ def test_pack_table_bookkeeping_against_a_stub_library(monkeypatch):
     assert n_jobs == 3 and total_tiles == 27 * 1 * 2 + 8 * 1 * 1 + 1 * 3 * 3
     jobs = (B._PackJob * 3).from_buffer_copy(bytes(tbl.jobs_dev.numpy().tobytes()))
     assert [j.tile_begin for j in jobs] == [0, 54, 62] and [j.K for j in jobs] == [27, 8, 1]
-    assert all(j.w_cp is None and j.w_tp is None for j in jobs) and jobs[0].w == ks[0].data_ptr()
-    assert ctypes.sizeof(B._PackJob) == 56
+    assert jobs[0].w == ks[0].data_ptr()
+    assert ctypes.sizeof(B._PackJob) == 40
     calls.clear()
     for k in ks:                                                           # every entry was refreshed
         B._packed_weights(k, dtype)
