@@ -15,83 +15,10 @@ bit-identical run to run: every split's partial sums are added in a fixed order.
 import pytest
 import torch
 
-from helpers import assert_one_rounding
+from helpers import _Route, _inputs, _pairs, _table, assert_one_rounding, ref_conv, ref_wgrad
 from oracle import oracle_np as O
 
 pytestmark = pytest.mark.gpu
-
-
-def _table(K, n_rows, n_other, density, seed, device):
-    """Random k-major neighbour table [K, n_rows] with fully empty rows and an all-empty offset."""
-    g = torch.Generator().manual_seed(seed)
-    idx = torch.randint(0, n_other, (K, n_rows), generator=g, dtype=torch.int32)
-    idx[torch.rand((K, n_rows), generator=g) > density] = -1
-    idx[:, ::97] = -1                     # rows without any neighbour
-    if K > 1:
-        idx[K // 2] = -1                  # an offset without any pair
-    return idx.to(device)
-
-
-def _pairs(nbr):
-    """[(rows of the other side, table rows)] per offset of a k-major table."""
-    out = []
-    for k in range(nbr.shape[0]):
-        o = torch.nonzero(nbr[k] >= 0).flatten()
-        out.append((nbr[k][o].long(), o))
-    return out
-
-
-def ref_conv(x, w, pairs, n_out):
-    """float64 y[o] = sum over offsets k and pairs (i, o) of x[i] @ w[k]; and the same reduction
-    over |x| and |w| (the scale of the accumulation error)."""
-    x, w = x.double(), w.double()
-    y = torch.zeros((n_out, w.shape[2]), dtype=torch.float64, device=x.device)
-    A = torch.zeros_like(y)
-    for k, (i, o) in enumerate(pairs):
-        if len(i):
-            y.index_add_(0, o, x[i] @ w[k])
-            A.index_add_(0, o, x[i].abs() @ w[k].abs())
-    return y, A
-
-
-def ref_wgrad(x, g, pairs):
-    """float64 dW[k] = sum over pairs (i, o) of x[i]^T g[o], and over |x|, |g|."""
-    x, g = x.double(), g.double()
-    K = len(pairs)
-    gw = torch.zeros((K, x.shape[1], g.shape[1]), dtype=torch.float64, device=x.device)
-    A = torch.zeros_like(gw)
-    for k, (i, o) in enumerate(pairs):
-        if len(i):
-            gw[k] = x[i].t() @ g[o]
-            A[k] = x[i].abs().t() @ g[o].abs()
-    return gw, A
-
-
-def _inputs(cin, cout, n_in, n_out, K, dtype, device, seed):
-    g = torch.Generator().manual_seed(seed)
-    feats = (torch.rand(n_in, cin, generator=g) - 0.5).to(dtype).to(device)
-    gout = (torch.rand(n_out, cout, generator=g) - 0.5).to(dtype).to(device)
-    w = ((torch.rand(K, cin, cout, generator=g) - 0.5) / (cin ** 0.5)).to(device)  # fp32 master
-    return feats, gout, w
-
-
-class _Route:
-    """Counts tensor-core launches over a block and checks the route the case is meant to take."""
-
-    def __init__(self, tc, what):
-        self.tc, self.what = tc, what
-
-    def __enter__(self):
-        from minkowskiengine_b200 import _lib
-        self.n0 = _lib.tc_launch_count()
-        return self
-
-    def __exit__(self, *exc):
-        from minkowskiengine_b200 import _lib
-        if exc[0] is None:
-            n = _lib.tc_launch_count() - self.n0
-            assert (n > 0) == self.tc, \
-                f"{self.what}: {n} tensor-core launches, expected {'some' if self.tc else 'none'}"
 
 
 # (cin, cout, n_in, n_out, K, forward on tensor cores, dgrad on tensor cores)

@@ -1,30 +1,18 @@
 """wgmma (tensor-core) convolution path: bf16 / fp16 operands, fp32 accumulation.
 
-Parity definition for reduced-precision inputs (SURVEY.md §8a notes): the oracle is fed the
-SAME bf16/fp16-rounded features and weights; with fp32 accumulation the CUDA result then
-differs only by summation order (asserted 2e-5 relative with fp32 output) plus one final
-rounding when the output is stored in bf16/fp16 (2^-8 relative, asserted 6e-3 of max)."""
+Every output is checked element by element against a float64 restatement fed the same
+bf16 / fp16-rounded features and weights (tests/helpers.py): |y - ref| <= TC_ACC * 2^-20 * A,
+A the same reduction over absolute values, plus one rounding when the output is stored in
+bf16 / fp16.  Forward and dgrad write every element once and the wgrad adds its row splits in a
+fixed order, so every result must also be bit-identical run to run."""
 import pytest
 import torch
 
-from helpers import rel_err, unique_cloud
+from helpers import (TC_ACC, _pairs, assert_one_rounding, lib_conv_backward, ref_conv, ref_wgrad,
+                     unique_cloud)
 from oracle import oracle_np as O
 
 pytestmark = pytest.mark.gpu
-
-
-def _torch_ref_forward(feats, w, nbr):
-    """fp32 torch restatement on the device: sum_k feats[nbr[k]] @ w[k] (missing rows = 0)."""
-    torch.backends.cuda.matmul.allow_tf32 = False
-    K, n_out = nbr.shape
-    out = torch.zeros((n_out, w.shape[2]), dtype=torch.float32, device=feats.device)
-    f32, w32 = feats.float(), w.float()
-    for k in range(K):
-        idx = nbr[k].long()
-        valid = idx >= 0
-        g = f32[idx.clamp(min=0)] * valid.unsqueeze(1)
-        out += g @ w32[k]
-    return out
 
 
 def _random_table(K, n_out, n_in, density, seed, device):
@@ -33,6 +21,15 @@ def _random_table(K, n_out, n_in, density, seed, device):
     drop = torch.rand((K, n_out), generator=g) > density
     idx[drop] = -1
     return idx.to(device)
+
+
+def _tc(fn):
+    """fn() with the tensor-core launches it made asserted non-zero."""
+    from minkowskiengine_b200 import _lib
+    n0 = _lib.tc_launch_count()
+    out = fn()
+    assert _lib.tc_launch_count() > n0, "did not take the tensor-core path"
+    return out
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
@@ -48,45 +45,62 @@ def _random_table(K, n_out, n_in, density, seed, device):
     (32, 64, 90000, 90000, 8),       # more super tiles than SMs: persistent loop + phases
 ])
 def test_tc_forward_matches_fp32_reference(ME, cuda, dtype, cin, cout, n_in, n_out, K):
+    """A kernel already in the feature dtype (packed alone, not an fp32 master)."""
     from minkowskiengine_b200 import backend
     g = torch.Generator().manual_seed(cin * 1000 + cout)
     feats = (torch.rand(n_in, cin, generator=g) - 0.5).to(dtype).to(cuda)
     w = ((torch.rand(K, cin, cout, generator=g) - 0.5) / (cin ** 0.5)).to(dtype).to(cuda)
     nbr = _random_table(K, n_out, n_in, 0.35, seed=K + n_out, device=cuda)
     km = backend._KernelMap(nbr, torch.empty((K, n_in), dtype=torch.int32, device=cuda))
-    ref = _torch_ref_forward(feats, w, nbr)
-    out32 = backend._conv_forward(feats, w, km, out_dtype=torch.float32)
-    scale = ref.abs().max().item()
-    assert (out32 - ref).abs().max().item() / scale < 2e-5
-    out_lp = backend._conv_forward(feats, w, km)
+    ref, A = ref_conv(feats, w, _pairs(nbr), n_out)
+    out32 = _tc(lambda: backend._conv_forward(feats, w, km, out_dtype=torch.float32))
+    assert_one_rounding(out32, ref, A, "forward, fp32 output", TC_ACC)
+    out_lp = _tc(lambda: backend._conv_forward(feats, w, km))
     assert out_lp.dtype == dtype
-    assert (out_lp.float() - ref).abs().max().item() / scale < 6e-3
+    assert_one_rounding(out_lp, ref, A, "forward", TC_ACC)
+    assert torch.equal(out_lp, backend._conv_forward(feats, w, km)), "forward differs run to run"
+    assert torch.equal(out32, backend._conv_forward(feats, w, km, out_dtype=torch.float32))
+
+
+def _to_pairs(im, om, device):
+    return [(torch.as_tensor(i, dtype=torch.long, device=device),
+             torch.as_tensor(o, dtype=torch.long, device=device)) for i, o in zip(im, om)]
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16])
 @pytest.mark.parametrize("cin,cout,ks,stride", [(32, 64, 3, 1), (64, 96, 3, 2), (96, 32, 2, 2)])
 def test_tc_layer_vs_oracle(ME, cuda, dtype, cin, cout, ks, stride):
     """Through the public API (SparseTensor + MinkowskiConvolution, bf16 features), forward
-    and backward, against the numpy oracle fed the same rounded values."""
+    and backward, against float64 on the oracle's kernel maps, fed the same rounded values."""
     D = 3
     coords = unique_cloud(6000, 24, seed=5, allow_negative=True)
     g = torch.Generator().manual_seed(9)
     feats = torch.rand(len(coords), cin, generator=g).to(dtype)
     conv = ME.MinkowskiConvolution(cin, cout, kernel_size=ks, stride=stride, dimension=D).to(cuda)
-    x = ME.SparseTensor(feats, coords, device=cuda, requires_grad=True)
-    y = conv(x)
-    assert y.F.dtype == dtype
+    gout = None
+    runs = []
+    for _ in range(2):
+        conv.kernel.grad = None
+        x = ME.SparseTensor(feats, coords, device=cuda, requires_grad=True)
+        y = _tc(lambda: conv(x))
+        assert y.F.dtype == dtype
+        if gout is None:
+            gout = (torch.rand(y.F.shape, generator=g) - 0.5).to(dtype).to(cuda)
+        _tc(lambda: y.F.backward(gout))
+        runs.append((x, y, x.F.grad.clone(), conv.kernel.grad.clone()))
+    (x, y, gi, gw), (_, y2, gi2, gw2) = runs
+    assert torch.equal(y.F, y2.F) and torch.equal(gi, gi2) and torch.equal(gw, gw2), \
+        "layer differs run to run"
     in_c, out_c = x.C.cpu().numpy(), y.C.cpu().numpy()
-    im, om = O.kernel_map(in_c, out_c, O.region_offsets(O.HYPER_CUBE, [ks] * D, [1] * D, [1] * D))
-    w = conv.kernel.detach().to(dtype).float().cpu().numpy()
-    f = feats.float().numpy()
-    ref = O.conv_forward(f, w, im, om, len(out_c))
-    assert rel_err(y.F.detach().float().cpu().numpy(), ref) < 6e-3
-    gout = (torch.rand(y.F.shape, generator=g) - 0.5).to(dtype)
-    y.F.backward(gout.to(cuda))
-    gi, gw = O.conv_backward(f, gout.float().numpy(), w, im, om)
-    assert rel_err(x.F.grad.float().cpu().numpy(), gi) < 6e-3       # bf16-stored dgrad
-    assert rel_err(conv.kernel.grad.float().cpu().numpy(), gw) < 1e-4   # fp32 wgrad
+    offs = O.region_offsets(O.HYPER_CUBE, [ks] * D, [1] * D, [1] * D)
+    pairs = _to_pairs(*O.kernel_map(in_c, out_c, offs), cuda)
+    w = conv.kernel.detach().to(dtype)
+    y_ref, y_A = ref_conv(x.F.detach(), w, pairs, len(out_c))
+    assert_one_rounding(y.F.detach(), y_ref, y_A, "layer forward", TC_ACC)
+    gi_ref, gi_A = ref_conv(gout, w.transpose(1, 2), [(o, i) for i, o in pairs], len(in_c))
+    assert_one_rounding(gi, gi_ref, gi_A, "layer dgrad (bf16)", TC_ACC)
+    gw_ref, gw_A = ref_wgrad(x.F.detach(), gout, pairs)
+    assert_one_rounding(gw, gw_ref, gw_A, "layer wgrad (fp32)", TC_ACC)
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
@@ -103,24 +117,19 @@ def test_tc_layer_vs_oracle(ME, cuda, dtype, cin, cout, ks, stride):
     (32, 64, 60000, 60000, 8),
 ])
 def test_tc_wgrad_matches_fp32_reference(ME, cuda, dtype, cin, cout, n_in, n_out, K):
-    from minkowskiengine_b200 import _lib, backend
-    torch.backends.cuda.matmul.allow_tf32 = False
+    from minkowskiengine_b200 import backend
     g = torch.Generator().manual_seed(cin * 77 + cout)
     feats = (torch.rand(n_in, cin, generator=g) - 0.5).to(dtype).to(cuda)
     gout = (torch.rand(n_out, cout, generator=g) - 0.5).to(dtype).to(cuda)
     w = torch.zeros(K, cin, cout, dtype=torch.float32, device=cuda)   # fp32 master weights
     nbr = _random_table(K, n_out, n_in, 0.35, seed=K + n_out + 1, device=cuda)
     km = backend._KernelMap(nbr, torch.full((K, n_in), -1, dtype=torch.int32, device=cuda))
-    before = _lib.tc_launch_count()
-    _, gw = backend._conv_backward(feats, gout, w, km, need_in=False, need_w=True)
-    assert _lib.tc_launch_count() > before, "wgrad did not take the tensor-core path"
-    ref = torch.zeros(K, cin, cout, dtype=torch.float32, device=cuda)
-    f32, g32 = feats.float(), gout.float()
-    for k in range(K):
-        idx = nbr[k].long()
-        valid = (idx >= 0).unsqueeze(1)
-        ref[k] = (f32[idx.clamp(min=0)] * valid).t() @ g32
-    assert (gw.float() - ref).abs().max().item() / ref.abs().max().item() < 2e-5
+    _, gw = _tc(lambda: backend._conv_backward(feats, gout, w, km, need_in=False, need_w=True))
+    _, gw2 = backend._conv_backward(feats, gout, w, km, need_in=False, need_w=True)
+    ref, A = ref_wgrad(feats, gout, _pairs(nbr))
+    assert gw.dtype == torch.float32
+    assert_one_rounding(gw, ref, A, "wgrad", TC_ACC)
+    assert torch.equal(gw, gw2), "wgrad differs run to run"
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
@@ -139,36 +148,38 @@ def test_tc_wgrad_matches_fp32_reference(ME, cuda, dtype, cin, cout, n_in, n_out
 ])
 def test_ta_forward_and_dgrad_packed_weights(ME, cuda, dtype, cin, cout, n_in, n_out, K):
     """fp32 master weights -> packed operand copies -> k_conv_wg:
-    forward over out_nbr and dgrad over in_nbr against the fp32 torch restatement."""
-    from minkowskiengine_b200 import _lib, backend
+    forward over out_nbr and dgrad over in_nbr against float64, in the feature dtype and in fp32."""
+    from minkowskiengine_b200 import backend
     g = torch.Generator().manual_seed(cin * 1000 + cout + 7)
     feats = (torch.rand(n_in, cin, generator=g) - 0.5).to(dtype).to(cuda)
     w = ((torch.rand(K, cin, cout, generator=g) - 0.5) / (cin ** 0.5)).to(cuda)   # fp32 master
-    wl = w.to(dtype)
     out_nbr = _random_table(K, n_out, n_in, 0.35, seed=K + n_out, device=cuda)
     in_nbr = _random_table(K, n_in, n_out, 0.3, seed=K + n_in + 3, device=cuda)
     km = backend._KernelMap(out_nbr, in_nbr)
-    before = _lib.tc_launch_count()
-    out32 = backend._conv_forward(feats, w, km, out_dtype=torch.float32)
-    assert _lib.tc_launch_count() > before
-    ref = _torch_ref_forward(feats, wl, out_nbr)
-    scale = ref.abs().max().item()
-    assert (out32 - ref).abs().max().item() / scale < 2e-5
+    ref, A = ref_conv(feats, w.to(dtype), _pairs(out_nbr), n_out)
+    out32 = _tc(lambda: backend._conv_forward(feats, w, km, out_dtype=torch.float32))
+    assert_one_rounding(out32, ref, A, "forward, fp32 output", TC_ACC)
     out_lp = backend._conv_forward(feats, w, km)
     assert out_lp.dtype == dtype
-    assert (out_lp.float() - ref).abs().max().item() / scale < 6e-3
+    assert_one_rounding(out_lp, ref, A, "forward", TC_ACC)
+    assert torch.equal(out_lp, backend._conv_forward(feats, w, km)), "forward differs run to run"
     # weights modified in place -> the packed copies must be rebuilt
     with torch.no_grad():
         w.mul_(0.5)
     out_half = backend._conv_forward(feats, w, km, out_dtype=torch.float32)
-    ref_half = _torch_ref_forward(feats, w.to(dtype), out_nbr)
-    assert (out_half - ref_half).abs().max().item() / scale < 2e-5
+    ref, A = ref_conv(feats, w.to(dtype), _pairs(out_nbr), n_out)
+    assert_one_rounding(out_half, ref, A, "forward after an in-place weight update", TC_ACC)
     # dgrad: rows = input rows, reduction over c_out, W_k^T
     gout = (torch.rand(n_out, cout, generator=g) - 0.5).to(dtype).to(cuda)
-    gi, _ = backend._conv_backward(feats, gout, w, km, need_in=True, need_w=False)
-    ref_gi = _torch_ref_forward(gout, w.to(dtype).transpose(1, 2).contiguous(), in_nbr)
+    ref, A = ref_conv(gout, w.to(dtype).transpose(1, 2), _pairs(in_nbr), n_in)
+    gi, _ = _tc(lambda: backend._conv_backward(feats, gout, w, km, need_in=True, need_w=False))
+    gi2, _ = backend._conv_backward(feats, gout, w, km, need_in=True, need_w=False)
     assert gi.dtype == dtype
-    assert (gi.float() - ref_gi).abs().max().item() / ref_gi.abs().max().item() < 6e-3
+    assert_one_rounding(gi, ref, A, "dgrad", TC_ACC)
+    assert torch.equal(gi, gi2), "dgrad differs run to run"
+    gi32, _ = _tc(lambda: lib_conv_backward(feats, gout, w, km, grad_in_dtype=torch.float32))
+    assert_one_rounding(gi32, ref, A, "dgrad, fp32 output", TC_ACC)
+    assert torch.equal(gi32, lib_conv_backward(feats, gout, w, km, grad_in_dtype=torch.float32)[0])
 
 
 @pytest.mark.parametrize("K,n,density,chunk", [(27, 5000, 0.3, 2048), (8, 70000, 0.125, 65536),
@@ -210,10 +221,9 @@ def test_pair_lists_match_table(ME, cuda, K, n, density, chunk, monkeypatch):
 
 
 def test_wgrad_pairs_many_chunks(ME, cuda, monkeypatch):
-    """k_wgrad_wg walking several row chunks of the pair lists (small chunks forced) against the fp32 reference."""
+    """k_wgrad_wg walking several row chunks of the pair lists (small chunks forced) against float64."""
     from minkowskiengine_b200 import backend
     monkeypatch.setattr(backend._KernelMap, "PAIR_CHUNK_ROWS", 4096)
-    torch.backends.cuda.matmul.allow_tf32 = False
     K, n_in, n_out, cin, cout = 27, 30000, 33000, 96, 96
     g = torch.Generator().manual_seed(5)
     feats = (torch.rand(n_in, cin, generator=g) - 0.5).bfloat16().to(cuda)
@@ -221,14 +231,12 @@ def test_wgrad_pairs_many_chunks(ME, cuda, monkeypatch):
     w = torch.zeros(K, cin, cout, device=cuda)
     nbr = _random_table(K, n_out, n_in, 0.3, seed=11, device=cuda)
     km = backend._KernelMap(nbr, torch.full((K, n_in), -1, dtype=torch.int32, device=cuda))
-    _, gw = backend._conv_backward(feats, gout, w, km, need_in=False, need_w=True)
+    _, gw = _tc(lambda: backend._conv_backward(feats, gout, w, km, need_in=False, need_w=True))
     assert km.pair_lists()[3] == 9
-    ref = torch.zeros(K, cin, cout, device=cuda)
-    f32, g32 = feats.float(), gout.float()
-    for k in range(K):
-        idx = nbr[k].long()
-        ref[k] = (f32[idx.clamp(min=0)] * (idx >= 0).unsqueeze(1)).t() @ g32
-    assert (gw - ref).abs().max().item() / ref.abs().max().item() < 2e-5
+    ref, A = ref_wgrad(feats, gout, _pairs(nbr))
+    assert_one_rounding(gw, ref, A, "chunked pair-list wgrad", TC_ACC)
+    _, gw2 = backend._conv_backward(feats, gout, w, km, need_in=False, need_w=True)
+    assert torch.equal(gw, gw2), "wgrad differs run to run"
 
 
 def test_batched_weight_packing_equals_single_and_cast(ME, cuda):
