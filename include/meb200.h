@@ -351,6 +351,78 @@ int meb200_union_fold_backward(const void *const *inputs, uint32_t N, uint32_t i
                                const void *grad_out, uint32_t i, const int64_t *u_i, uint32_t n_i,
                                void *grad_i, void *stream);
 
+/* ---- tensor fields: points with float coordinates, quantised to voxels (reference:
+ *      MinkowskiTensorField.py, CoordinateFieldMapCPU::quantize_coordinates
+ *      coordinate_map_cpu.hpp:994-1037, interpolation_map_weight_kernel :139-240,
+ *      src/interpolation_cpu.cpp, src/direct_max_pool.cpp).  Every output element is written
+ *      exactly once: no memset, no float atomics, bit-identical results run to run.  fp32
+ *      accumulation with one rounding to the feature dtype; 16-byte accesses where
+ *      C * sizeof(dtype) % 16 == 0 and the pointers allow.
+ *   field   float32 [n, ncols]: column 0 the batch index (rounded with lroundf), then the axes;
+ *           a point lies in the voxel floorf(x / s) * s of tensor stride s (float division). ---- */
+#define MEB200_ERR_DOMAIN (-4) /* a field coordinate is not finite or its voxel is outside int32 */
+
+#define MEB200_FIELD_SUM 0       /* SparseTensorQuantizationMode.UNWEIGHTED_SUM */
+#define MEB200_FIELD_AVG 1       /* UNWEIGHTED_AVERAGE */
+#define MEB200_FIELD_MAX 2       /* MAX_POOL */
+#define MEB200_FIELD_SUBSAMPLE 3 /* RANDOM_SUBSAMPLE (the first point of a voxel) */
+
+/* Quantises the field at `tensor_stride` (HOST int32 [ncols-1]) into out (int32 [n, ncols]) and,
+ * when d_bad != NULL, sets *d_bad (DEVICE uint32 status word, cleared by the call) to 1 when a
+ * coordinate is not finite or its voxel falls outside int32 (NULL: the field is known valid). */
+int meb200_quantize_field(const float *field, uint32_t n, uint32_t ncols,
+                          const int32_t *tensor_stride, int32_t *out, uint32_t *d_bad,
+                          void *stream);
+/* Quantisation followed by meb200_insert_and_map on the quantised rows (qcoords: int32 [n, ncols]
+ * buffer; the other arguments as meb200_insert_and_map): the first point of a voxel is its
+ * unique_index.  The validity of the coordinates reaches the host with the unique count, in the
+ * same read; invalid coordinates return MEB200_ERR_DOMAIN. */
+int meb200_field_insert_and_map(const float *field, uint32_t n, uint32_t ncols,
+                                const int32_t *tensor_stride, int32_t *qcoords, uint32_t *table,
+                                uint32_t capacity, int32_t *unique_coords, int64_t *unique_index,
+                                int64_t *inverse_map, void *scratch, uint32_t *h_num_unique,
+                                void *stream);
+
+/* Deterministic grouping of P entries by an int32 key in [0, M) (keys outside are left out):
+ * entries of key r are perm[start[r] .. start[r+1]), in ascending entry order (a stable radix
+ * sort).  start: int32 [M+1], perm: int32 [P] (entries past start[M] are the left-out ones).
+ * scratch: meb200_group_by_row_scratch_bytes(P, M) bytes. */
+uint64_t meb200_group_by_row_scratch_bytes(uint32_t P, uint32_t M);
+int meb200_group_by_row(const int32_t *keys, uint32_t P, uint32_t M, int32_t *start, int32_t *perm,
+                        void *scratch, uint64_t scratch_bytes, void *stream);
+
+/* Points -> voxels.  For every output row r < M, over its entries j = perm[start[r] ..
+ * start[r+1]) in order, with source row s = j / src_div and x = src[s, :] (times weight[j] when
+ * weight != NULL): SUM the fp32 sum, AVG the sum over the exact count, MAX the maximum (the first
+ * entry wins ties) with argmax[r, c] = s (int32 [M, C]).  A row without entries gives 0 (argmax
+ * -1).  src: [n_src, C] in `dtype`, out: [M, C] in `dtype`.  Also the backward of a slice (SUM) and
+ * of interpolation (SUM, weight = the interpolation weights, src_div = 2^D). */
+int meb200_field_reduce(const void *src, int dtype, uint32_t n_src, uint32_t C, const int32_t *perm,
+                        const int32_t *start, uint32_t M, const float *weight, uint32_t src_div,
+                        int mode, void *out, int32_t *argmax, void *stream);
+
+/* Voxels -> points: out[i, :] = g[inv[i], :] scaled per mode (inv: int64 [n]; -1 -> 0):
+ * AVG  times 1 / (start[r+1] - start[r]);  MAX  kept where argmax[r, c] == i, else 0;
+ * SUBSAMPLE  kept where unique_index[r] == i, else 0.  The backward of meb200_field_reduce (the
+ * plain copy is meb200_gather_rows).  g: [M, C], out: [n, C] in `dtype`. */
+int meb200_field_expand(const void *g, int dtype, uint32_t M, uint32_t C, const int64_t *inv,
+                        uint32_t n, int mode, const int32_t *start, const int32_t *argmax,
+                        const int64_t *unique_index, void *out, void *stream);
+
+/* Trilinear (multilinear) interpolation map of n query points (float32 [n, ncols]) into a
+ * coordinate map of tensor stride `tensor_stride` (HOST int32 [ncols-1]): the corners
+ * floorf(x / s) * s + b * s (b in {0, 1} per axis; bit ncols-1-j of corner k selects the upper
+ * end of axis j) are probed in the map; rows int32 [n, 2^D] = the corner's row or -1, weights
+ * fp32 [n, 2^D] = prod_j (1 - |x_j - corner_j| / s_j) (0 where absent; not normalised).
+ * A query with a non-finite coordinate has no corners. */
+int meb200_interp_map(const float *query, uint32_t n, uint32_t ncols, const int32_t *tensor_stride,
+                      const int32_t *map_coords, const uint32_t *table, uint32_t capacity,
+                      int32_t *rows, float *weights, void *stream);
+/* out[q, :] = sum_k weights[q, k] * F[rows[q, k], :] over the present corners in ascending k
+ * (fp32, one rounding).  F: [M, C], out: [n, C] in `dtype`; K = 2^D. */
+int meb200_interp_forward(const void *F, int dtype, uint32_t M, uint32_t C, const int32_t *rows,
+                          const float *weights, uint32_t n, uint32_t K, void *out, void *stream);
+
 /* ---- batch normalisation over [n, C] feature rows (SURVEY.md 8(f) "next" row 1; the
  *      reference applies torch.nn.BatchNorm1d to `.F`: MinkowskiEngine/MinkowskiNormalization.py:51-99).
  *      C must be a multiple of 8.  sums: DEVICE double [2C]; statistics tensors fp32 [C]. ------ */

@@ -8,7 +8,8 @@ hot path of NVIDIA/MinkowskiEngine, behind the reference's own Python API.
 Scope (SURVEY.md §8): SparseTensor / CoordinateManager / kernel maps, MinkowskiConvolution,
 MinkowskiConvolutionTranspose, local and global pooling, broadcast, batch and instance
 normalisation, pruning, union and arithmetic between sparse tensors on different coordinate maps,
-and the thin torch wrappers MinkUNet, the ResNet classifiers and generative networks need.
+TensorField (point features quantised to voxels, sliced back and interpolated), and the thin torch
+wrappers MinkUNet, the ResNet classifiers and generative networks need.
 CUDA tensors only; all device work runs in csrc/libmeb200.so (include/meb200.h).
 """
 __version__ = "0.1.0"
@@ -40,7 +41,9 @@ from .broadcast import (MinkowskiBroadcast, MinkowskiBroadcastAddition,
 from .normalization import (MinkowskiBatchNorm, MinkowskiInstanceNorm,
                             MinkowskiInstanceNormFunction, MinkowskiSyncBatchNorm, fused_bn_relu)
 from .nonlinearity import *  # noqa: F401,F403
-from .ops import MinkowskiLinear, cat
+from .ops import MinkowskiLinear, MinkowskiToSparseTensor, cat
+from .tensor_field import TensorField
+from .interpolation import MinkowskiInterpolation, MinkowskiInterpolationFunction
 from .pruning import MinkowskiPruning, MinkowskiPruningFunction
 from .union import MinkowskiUnion, MinkowskiUnionFunction
 from . import modules, utils  # noqa: F401

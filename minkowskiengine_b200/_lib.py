@@ -17,6 +17,8 @@ POOL_SUM, POOL_AVG, POOL_MAX = 0, 1, 2
 SEG_SUM, SEG_AVG, SEG_MAX = 0, 1, 2
 BCAST_ADD, BCAST_MUL, BCAST_COPY, BCAST_MAXGRAD = 0, 1, 2, 3
 UNION_ADD, UNION_SUB, UNION_MUL, UNION_DIV = 0, 1, 2, 3
+FIELD_SUM, FIELD_AVG, FIELD_MAX, FIELD_SUBSAMPLE = 0, 1, 2, 3
+ERR_DOMAIN = -4
 
 _u32, _u64, _i32, _vp = C.c_uint32, C.c_uint64, C.c_int, C.c_void_p
 
@@ -72,6 +74,17 @@ PROTOTYPES = {
     "meb200_union_fold_forward": (_i32, [_vp, _u32, _u32, _vp, _u32, _u32, _i32, _i32, _vp, _vp]),
     "meb200_union_fold_backward": (_i32, [_vp, _u32, _u32, _vp, _u32, _u32, _i32, _i32, _vp, _u32,
                                           _vp, _u32, _vp, _vp]),
+    "meb200_quantize_field": (_i32, [_vp, _u32, _u32, C.POINTER(C.c_int32), _vp, _vp, _vp]),
+    "meb200_field_insert_and_map": (_i32, [_vp, _u32, _u32, C.POINTER(C.c_int32), _vp, _vp, _u32,
+                                           _vp, _vp, _vp, _vp, C.POINTER(_u32), _vp]),
+    "meb200_group_by_row_scratch_bytes": (_u64, [_u32, _u32]),
+    "meb200_group_by_row": (_i32, [_vp, _u32, _u32, _vp, _vp, _vp, _u64, _vp]),
+    "meb200_field_reduce": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _u32, _vp, _u32, _i32, _vp, _vp,
+                                   _vp]),
+    "meb200_field_expand": (_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "meb200_interp_map": (_i32, [_vp, _u32, _u32, C.POINTER(C.c_int32), _vp, _vp, _u32, _vp, _vp,
+                                 _vp]),
+    "meb200_interp_forward": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _vp]),
     "meb200_bn_workspace_bytes": (_u64, []),
     "meb200_bn_forward_train": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _vp, _i32, C.c_float,
                                        C.c_float, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -320,6 +320,10 @@ class CoordinateMapManagerGPU_c10:
         self._groupings = {}    # map key -> _OriginGrouping
         self._prunes = {}       # (in key, out key) -> (unique_index, inverse_map) of a pruned map
         self._unions = {}       # tuple of input keys -> _UnionMap
+        self._fields = {}       # field key -> float32 [N, D+1] point coordinates
+        self._field_maps = {}   # (field key, map key) -> _FieldToSparse
+        self._field_quant = {}  # (field key, tensor stride, string id) -> map key it quantised to
+        self._field_valid = set()  # field keys whose coordinates a quantisation has checked
         _lib.load()             # fail at construction if the native library is missing
 
     # -- keys ------------------------------------------------------------------------
@@ -373,6 +377,17 @@ class CoordinateMapManagerGPU_c10:
         if key in self._maps:
             key = self.get_random_string_id(ts, string_id)
         cmap, unique_index, inverse_map = _CoordinateMap.build(coordinates, ts)
+        self._add_inserted(key, cmap)
+        if cmap.size == coordinates.size(0):
+            # no duplicates: the reference GPU path returns an empty inverse map here
+            # (coordinate_map_manager.cu:94-112) and Python substitutes arange
+            inverse_map = inverse_map[:0]
+        return CoordinateMapKey(list(key[0]), key[1]), (unique_index, inverse_map)
+
+    def _add_inserted(self, key, cmap):
+        """Registers a map made from input coordinates (insert_and_map, or the quantisation of a
+        tensor field): the first one starts the predicted pyramid and kernel maps, and every one
+        counts towards the origin map."""
         first = not self._maps
         self._maps[key] = cmap
         self._inserted.append(key)
@@ -381,11 +396,6 @@ class CoordinateMapManagerGPU_c10:
             self._hint_ncols = cmap.ncols
             self._prefetch_pyramid(key, cmap)
             self._prefetch_kernel_maps(cmap.ncols)
-        if cmap.size == coordinates.size(0):
-            # no duplicates: the reference GPU path returns an empty inverse map here
-            # (coordinate_map_manager.cu:94-112) and Python substitutes arange
-            inverse_map = inverse_map[:0]
-        return CoordinateMapKey(list(key[0]), key[1]), (unique_index, inverse_map)
 
     def _stride(self, in_key, kernel_stride, string_id=""):
         """reference: coordinate_map_manager.cpp:406-429 -> (out key tuple, created?)"""
@@ -826,6 +836,161 @@ class CoordinateMapManagerGPU_c10:
         return [torch.stack([torch.arange(n, dtype=torch.int64, device=u.device), u])
                 for u, n in zip(um.u, um.sizes)]
 
+    # -- tensor fields -------------------------------------------------------------------
+    def insert_field(self, coordinates, tensor_stride, string_id=""):
+        """reference: coordinate_map_manager.cpp:145-181.  The field keeps the float32 points."""
+        _assert(coordinates.dim() == 2, "coordinates must be 2-dimensional")
+        _assert(coordinates.dtype == torch.float32, "field coordinates must be a FloatTensor")
+        _assert(coordinates.is_contiguous(), "coordinates must be contiguous")
+        _assert(coordinates.is_cuda,
+                "coordinates must be a CUDA tensor: minkowskiengine_b200 implements the GPU "
+                "coordinate manager only (no CPU backend, no fallback)")
+        ts = [int(v) for v in tensor_stride]
+        _assert(coordinates.size(1) - 1 == len(ts),
+                "The coordinate dimension (coordinate_size - 1):", coordinates.size(1) - 1,
+                " must match the size of tensor stride:", ts)
+        key = (tuple(ts), string_id)
+        while key in self._fields:
+            key = (key[0], self.get_random_string_id(ts, string_id)[1])
+        self._fields[key] = coordinates
+        return CoordinateMapKey(list(key[0]), key[1])
+
+    def _field(self, field_key):
+        fk = self._k(field_key)
+        _assert(fk in self._fields, "field", ERROR_MAP_NOT_FOUND)
+        return fk, self._fields[fk]
+
+    def get_coordinate_field(self, field_key):
+        return self._field(field_key)[1]
+
+    def _field_to_sparse(self, field_key, tensor_stride, string_id=""):
+        """Quantises the field at `tensor_stride` into a new inserted map (meb200_field_insert_and_map)
+        -> map key tuple.  Cached per (field, stride, string id): quantising again returns the same
+        map and grouping."""
+        fk, field = self._field(field_key)
+        ts = tuple(int(v) for v in tensor_stride)
+        _assert(len(ts) + 1 == field.size(1), "The coordinate dimension (coordinate_size - 1):",
+                field.size(1) - 1, " must match the size of tensor stride:", list(ts))
+        ck = (fk, ts, string_id)
+        sk = self._field_quant.get(ck)
+        if sk is not None:
+            return sk
+        lib = _lib.load()
+        n, ncols = field.shape
+        dev = field.device
+        cap = int(lib.meb200_hash_capacity(n))
+        table = torch.empty(cap, dtype=torch.int32, device=dev)
+        q = torch.empty((n, ncols), dtype=torch.int32, device=dev)
+        uniq = torch.empty((n, ncols), dtype=torch.int32, device=dev)
+        uidx = torch.empty(n, dtype=torch.int64, device=dev)
+        inv = torch.empty(n, dtype=torch.int64, device=dev)
+        scratch = torch.empty(int(lib.meb200_insert_scratch_bytes(n)), dtype=torch.uint8, device=dev)
+        m = ctypes.c_uint32(0)
+        rc = lib.meb200_field_insert_and_map(
+            _lib.ptr(field), n, ncols, (ctypes.c_int32 * len(ts))(*ts), _lib.ptr(q), _lib.ptr(table),
+            cap, _lib.ptr(uniq), _lib.ptr(uidx), _lib.ptr(inv), _lib.ptr(scratch), ctypes.byref(m),
+            _lib.current_stream())
+        if rc == _lib.ERR_DOMAIN:
+            raise ValueError("TensorField coordinates must be finite and quantise to int32 voxels")
+        _lib.check(rc)
+        self._field_valid.add(fk)
+        m = int(m.value)
+        key = (ts, string_id)
+        if key in self._maps:
+            key = self.get_random_string_id(ts, string_id)
+        self._add_inserted(key, _CoordinateMap(uniq[:m], table, cap, ts))
+        self._field_maps[(fk, key)] = _FieldToSparse(inv, m, uidx[:m])
+        self._field_quant[ck] = key
+        return key
+
+    def field_to_sparse_insert_and_map(self, field_key, tensor_stride, string_id=""):
+        """reference: coordinate_map_manager.cpp:188-254 -> (map key, (unique_index, inverse_map));
+        the inverse map is empty when no two points share a voxel, as for insert_and_map."""
+        fk = self._k(field_key)
+        sk = self._field_to_sparse(field_key, tensor_stride, string_id)
+        f2s = self._field_maps[(fk, sk)]
+        inv = f2s.inverse if f2s.M < f2s.inverse.numel() else f2s.inverse[:0]
+        return CoordinateMapKey(list(sk[0]), sk[1]), (f2s.unique_index, inv)
+
+    def field_to_sparse_map(self, field_key, sparse_key):
+        """reference: coordinate_map_manager.cpp:282-330.  The points of the field quantised at the
+        map's stride and looked up in it -> (inverse_map int64 [N]: row of every point, -1 where the
+        map lacks its voxel; unique_index int64 [M]: the first point of every row, -1 for a row
+        without points).  A field that no quantisation has checked yet costs one host read (the
+        validity of its coordinates), once."""
+        f2s = self._field_sparse_record(field_key, sparse_key)
+        return f2s.inverse, f2s.first_points()
+
+    def _field_sparse_record(self, field_key, sparse_key):
+        fk, field = self._field(field_key)
+        sk = self._k(sparse_key)
+        f2s = self._field_maps.get((fk, sk))
+        if f2s is not None:
+            return f2s
+        cmap = self._get(sk)
+        _assert(cmap.ncols == field.size(1), "The coordinate dimension mismatch.", field.size(1),
+                "!=", cmap.ncols)
+        lib = _lib.load()
+        n, ncols = field.shape
+        stream = _lib.current_stream()
+        q = torch.empty((n, ncols), dtype=torch.int32, device=field.device)
+        # the validity of the coordinates reaches the host with the row count of the first map made
+        # from the field; only a field never quantised before pays a read here, once
+        bad = None if fk in self._field_valid else \
+            torch.empty(1, dtype=torch.int32, device=field.device)
+        ts = cmap.tensor_stride
+        _lib.check(lib.meb200_quantize_field(_lib.ptr(field), n, ncols,
+                                             (ctypes.c_int32 * len(ts))(*ts), _lib.ptr(q),
+                                             _lib.ptr(bad), stream))
+        if bad is not None:
+            if int(bad.item()) != 0:
+                raise ValueError("TensorField coordinates must be finite and quantise to int32 "
+                                 "voxels")
+            self._field_valid.add(fk)
+        res = torch.empty(n, dtype=torch.int32, device=field.device)
+        _lib.check(lib.meb200_map_find(_lib.ptr(cmap.coords), _lib.ptr(cmap.table), cmap.capacity,
+                                       ncols, _lib.ptr(q), n, _lib.ptr(res), stream))
+        f2s = _FieldToSparse(res.long(), cmap.size)
+        self._field_maps[(fk, sk)] = f2s
+        return f2s
+
+    def exists_field_to_sparse(self, field_key, sparse_key):
+        return (self._k(field_key), self._k(sparse_key)) in self._field_maps
+
+    def get_field_to_sparse_map(self, field_key, sparse_key):
+        """reference: coordinate_map_manager.cpp:260-276 -> (unique_index, inverse_map)."""
+        ent = self._field_maps.get((self._k(field_key), self._k(sparse_key)))
+        _assert(ent is not None, "Field To Sparse Map doesn't exist")
+        return ent.first_points(), ent.inverse
+
+    def field_to_sparse_keys(self, field_key):
+        fk = self._k(field_key)
+        return [CoordinateMapKey(list(sk[0]), sk[1]) for f, sk in self._field_maps if f == fk]
+
+    def _interp_map(self, key, query):
+        """Dense interpolation map of float32 query points into map `key` (meb200_interp_map) ->
+        (rows int32 [n, 2^D], weights fp32 [n, 2^D])."""
+        cmap = self._get(key)
+        _assert(query.dim() == 2 and query.size(1) == cmap.ncols, "query coordinates",
+                tuple(query.shape), "do not have", cmap.ncols, "columns")
+        n, ncols = query.shape
+        K = 1 << (ncols - 1)
+        rows = torch.empty((n, K), dtype=torch.int32, device=query.device)
+        w = torch.empty((n, K), dtype=torch.float32, device=query.device)
+        ts = cmap.tensor_stride
+        _lib.check(_lib.load().meb200_interp_map(
+            _lib.ptr(query), n, ncols, (ctypes.c_int32 * len(ts))(*ts), _lib.ptr(cmap.coords),
+            _lib.ptr(cmap.table), cmap.capacity, _lib.ptr(rows), _lib.ptr(w), _lib.current_stream()))
+        return rows, w
+
+    def interpolation_map_weight(self, key, query):
+        """reference: coordinate_map_manager.cpp:1080 -> [in rows int32, out rows int32, weights fp32]
+        of every present corner, ordered by query row, then corner."""
+        rows, w = self._interp_map(key, query.float().contiguous())
+        hit = rows >= 0
+        q = torch.nonzero(hit)[:, 0].int()
+        return [rows[hit], q, w[hit]]
+
     def __repr__(self):
         lines = [f"\t{list(k[0])}{':' + k[1] if k[1] else ''}:\tCoordinateMapGPU:{m.size}x{m.ncols}"
                  for k, m in self._maps.items()]
@@ -854,6 +1019,32 @@ class _OriginGrouping:
         if getattr(self, "_counts", None) is None:
             self._counts = (self.seg_start[1:] - self.seg_start[:-1]).float()
         return self._counts
+
+
+class _FieldToSparse:
+    """How the points of a tensor field fall into the M rows of a coordinate map: inverse int64 [N]
+    (row of every point, -1 where the map lacks it) and, for a map made by quantising the field,
+    unique_index int64 [M] (first point of every row).  The grouping of the points by row
+    (meb200_group_by_row: start int32 [M+1], perm int32 [N]) is built on first use and cached."""
+
+    __slots__ = ("inverse", "M", "unique_index", "_group")
+
+    def __init__(self, inverse, M, unique_index=None):
+        self.inverse, self.M, self.unique_index, self._group = inverse, int(M), unique_index, None
+
+    def group(self):
+        if self._group is None:
+            self._group = group_by_row(self.inverse.int(), self.M)
+        return self._group
+
+    def first_points(self):
+        if self.unique_index is None:
+            start, perm = self.group()
+            cnt = start[1:] - start[:-1]
+            first = perm[start[:-1].clamp(max=max(perm.numel() - 1, 0)).long()].long() \
+                if perm.numel() else torch.zeros(self.M, dtype=torch.int64, device=start.device)
+            self.unique_index = torch.where(cnt > 0, first, torch.full_like(first, -1))
+        return self.unique_index
 
 
 class _UnionMap:
@@ -1569,3 +1760,61 @@ def union_fold_backward(grad_out, feats, um, op, needs=None):
             _lib.current_stream()))
         grads.append(g)
     return grads
+
+
+# ---- tensor fields: points <-> voxels, interpolation ----------------------------------------------
+def group_by_row(keys, M):
+    """(start int32 [M+1], perm int32 [P]): the entries of int32 keys grouped by key in [0, M),
+    ascending entry order inside a key (meb200_group_by_row)."""
+    lib = _lib.load()
+    P = keys.numel()
+    dev = keys.device
+    start = torch.empty(M + 1, dtype=torch.int32, device=dev)
+    perm = torch.empty(P, dtype=torch.int32, device=dev)
+    nbytes = int(lib.meb200_group_by_row_scratch_bytes(P, M)) if P else 0
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev) if P else None
+    _lib.check(lib.meb200_group_by_row(_lib.ptr(keys), P, M, _lib.ptr(start), _lib.ptr(perm),
+                                       _lib.ptr(scratch), nbytes, _lib.current_stream()))
+    return start, perm
+
+
+def field_reduce(src, group, M, mode, weight=None, src_div=1):
+    """[M, C] reduction of the rows of `src` over a grouping (meb200_field_reduce) -> (out, argmax
+    int32 [M, C] for MAX else None)."""
+    src = src.contiguous()
+    start, perm = group
+    C = src.size(1)
+    out = torch.empty((M, C), dtype=src.dtype, device=src.device)
+    argmax = torch.empty((M, C), dtype=torch.int32, device=src.device) \
+        if mode == _lib.FIELD_MAX else None
+    _lib.check(_lib.load().meb200_field_reduce(
+        _lib.ptr(src), _lib.dtype_code(src.dtype), src.size(0), C, _lib.ptr(perm), _lib.ptr(start),
+        M, _lib.ptr(weight), src_div, mode, _lib.ptr(out), _lib.ptr(argmax), _lib.current_stream()))
+    return out, argmax
+
+
+def field_expand(g, inv, mode, start=None, argmax=None, unique_index=None):
+    """[N, C] rows g[inv[i]] scaled per mode (meb200_field_expand): the backward of field_reduce."""
+    g = g.contiguous()
+    n, C = inv.numel(), g.size(1)
+    out = torch.empty((n, C), dtype=g.dtype, device=g.device)
+    _lib.check(_lib.load().meb200_field_expand(
+        _lib.ptr(g), _lib.dtype_code(g.dtype), g.size(0), C, _lib.ptr(inv), n, mode, _lib.ptr(start),
+        _lib.ptr(argmax), _lib.ptr(unique_index), _lib.ptr(out), _lib.current_stream()))
+    return out
+
+
+def gather_rows(src, idx, n_out):
+    """Public name of the row gather (meb200_gather_rows) for the tensor-field functions."""
+    return _gather_rows(src.contiguous(), idx, n_out)
+
+
+def interp_forward(F, rows, w):
+    """[n, C] = sum_k w[q, k] * F[rows[q, k]] in ascending k (meb200_interp_forward)."""
+    F = F.contiguous()
+    n, K = rows.shape
+    out = torch.empty((n, F.size(1)), dtype=F.dtype, device=F.device)
+    _lib.check(_lib.load().meb200_interp_forward(
+        _lib.ptr(F), _lib.dtype_code(F.dtype), F.size(0), F.size(1), _lib.ptr(rows), _lib.ptr(w), n,
+        K, _lib.ptr(out), _lib.current_stream()))
+    return out

@@ -155,6 +155,44 @@ class CoordinateManager:
     def stride_map(self, in_key: CoordinateMapKey, stride_key: CoordinateMapKey):
         return self._manager.stride_map(in_key, stride_key)
 
+    # -- tensor fields (reference: MinkowskiCoordinateManager.py, coordinate_map_manager.cpp:145-343)
+    def insert_field(self, coordinates: torch.Tensor, tensor_stride=1,
+                     string_id: str = "") -> CoordinateMapKey:
+        """Registers float32 point coordinates [N, D+1] and returns the field key."""
+        return self._manager.insert_field(coordinates, convert_to_int_list(tensor_stride, self.D),
+                                          string_id)
+
+    def get_coordinate_field(self, field_key: CoordinateMapKey) -> torch.Tensor:
+        return self._manager.get_coordinate_field(field_key)
+
+    def field_to_sparse_insert_and_map(self, field_key: CoordinateMapKey, tensor_stride=1,
+                                       string_id: str = ""):
+        """Quantises the field at `tensor_stride` into a coordinate map -> (map key, (unique_index,
+        inverse_mapping)); quantising the same field at the same stride again returns the same
+        map.  Raises ValueError for non-finite coordinates."""
+        return self._manager.field_to_sparse_insert_and_map(
+            field_key, convert_to_int_list(tensor_stride, self.D), string_id)
+
+    def field_to_sparse_map(self, field_key: CoordinateMapKey, sparse_key: CoordinateMapKey):
+        """(inverse_mapping int64 [N], unique_index int64 [M]) of the field's points in an existing
+        map (-1 where the map lacks a point's voxel / a row has no point)."""
+        return self._manager.field_to_sparse_map(field_key, sparse_key)
+
+    def exists_field_to_sparse(self, field_key: CoordinateMapKey, sparse_key: CoordinateMapKey):
+        return self._manager.exists_field_to_sparse(field_key, sparse_key)
+
+    def get_field_to_sparse_map(self, field_key: CoordinateMapKey, sparse_key: CoordinateMapKey):
+        """(unique_index, inverse_mapping) of a field-to-map relation made before."""
+        return self._manager.get_field_to_sparse_map(field_key, sparse_key)
+
+    def field_to_sparse_keys(self, field_key: CoordinateMapKey):
+        return self._manager.field_to_sparse_keys(field_key)
+
+    def interpolation_map_weight(self, key: CoordinateMapKey, samples: torch.Tensor):
+        """[in rows, out rows, weights] of the multilinear interpolation of the map's rows at the
+        float sample points (every present corner, ordered by sample, then corner)."""
+        return self._manager.interpolation_map_weight(key, samples)
+
     def __repr__(self):
         return (self._CoordinateManagerClass.__name__ + "(\n" + str(self._manager)
                 + f"\talgorithm={self.minkowski_algorithm}\n  )\n")

@@ -52,6 +52,15 @@ inline unsigned cdiv(uint64_t a, uint64_t b) { return (unsigned)((a + b - 1) / b
 
 int num_sms();
 
+// The deduplicating insert behind meb200_insert_and_map (coords.cu).  Its one blocking read copies
+// h_words words to the host: the unique count, and with h_words = 2 the word beside it in the
+// scratch (insert_flag_word), which kernels enqueued before the insert may set.
+int insert_and_map(const int32_t *coords, const uint8_t *valid, uint32_t n, uint32_t ncols,
+                   uint32_t *table, uint32_t capacity, int32_t *unique_coords,
+                   int64_t *unique_index, int64_t *inverse_map, void *scratch,
+                   uint32_t *h_num_unique, uint32_t h_words, cudaStream_t stream);
+uint32_t *insert_flag_word(void *scratch, uint32_t n);
+
 // ---- coordinate rows ---------------------------------------------------------------
 struct IntVec {  // small by-value parameter block (tensor strides, etc.)
   int32_t v[MEB200_MAX_NCOLS];
@@ -170,5 +179,32 @@ template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(flo
 template <> __device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half_rn(v); }
 
 inline size_t dtype_size(int dt) { return dt == MEB200_F32 ? 4 : 2; }
+
+// V elements of T per access: 16 bytes when V = 16 / sizeof(T), one element when V = 1
+template <typename T, int V>
+__device__ __forceinline__ void load_f32(const T *p, float (&f)[V]) {
+  if constexpr (V == 1) {
+    f[0] = to_f32<T>(*p);
+  } else {
+    static_assert(V * sizeof(T) == 16, "16-byte vectors");
+    uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
+    const T *e = reinterpret_cast<const T *>(&v);
+#pragma unroll
+    for (int j = 0; j < V; ++j) f[j] = to_f32<T>(e[j]);
+  }
+}
+
+template <typename T, int V>
+__device__ __forceinline__ void store_f32(T *p, const float (&f)[V]) {
+  if constexpr (V == 1) {
+    *p = from_f32<T>(f[0]);
+  } else {
+    uint4 v;
+    T *e = reinterpret_cast<T *>(&v);
+#pragma unroll
+    for (int j = 0; j < V; ++j) e[j] = from_f32<T>(f[j]);
+    *reinterpret_cast<uint4 *>(p) = v;
+  }
+}
 
 }  // namespace meb200

@@ -248,28 +248,12 @@ k_find(const int32_t *__restrict__ map_coords, const uint32_t *__restrict__ tabl
   result[i] = table_find<NC>(map_coords, table, mask, key);
 }
 
-}  // namespace meb200
+uint32_t *insert_flag_word(void *scratch, uint32_t n) { return carve(scratch, n).total + 1; }
 
-using namespace meb200;
-
-extern "C" {
-
-uint32_t meb200_hash_capacity(uint32_t n) {
-  uint64_t want = (uint64_t)n * 3u;
-  uint64_t cap = 1024;
-  while (cap < want) cap <<= 1;
-  return (uint32_t)(cap > 0x80000000ull ? 0x80000000ull : cap);
-}
-
-uint64_t meb200_insert_scratch_bytes(uint32_t n) {
-  return 4ull * (2ull * n + scan_blocks(n) + 8);
-}
-
-int meb200_insert_and_map(const int32_t *coords, const uint8_t *valid, uint32_t n,
-                          uint32_t ncols, uint32_t *table, uint32_t capacity,
-                          int32_t *unique_coords, int64_t *unique_index, int64_t *inverse_map,
-                          void *scratch, uint32_t *h_num_unique, void *stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
+int insert_and_map(const int32_t *coords, const uint8_t *valid, uint32_t n, uint32_t ncols,
+                   uint32_t *table, uint32_t capacity, int32_t *unique_coords,
+                   int64_t *unique_index, int64_t *inverse_map, void *scratch,
+                   uint32_t *h_num_unique, uint32_t h_words, cudaStream_t stream) {
   MEB_CHECK_ARG(h_num_unique != nullptr, "h_num_unique");
   MEB_CHECK_ARG(table != nullptr && capacity >= 2 && (capacity & (capacity - 1)) == 0,
                 "capacity must be a power of two (got %u)", capacity);
@@ -296,7 +280,7 @@ int meb200_insert_and_map(const int32_t *coords, const uint8_t *valid, uint32_t 
   MEB_LAUNCH_OK();
   k_inverse<<<cdiv(n, 256), 256, 0, stream>>>(table, s.slot_of, s.rank_of, n, inverse_map);
   MEB_LAUNCH_OK();
-  MEB_CUDA(cudaMemcpyAsync(h_num_unique, s.total, 4, cudaMemcpyDeviceToHost, stream));
+  MEB_CUDA(cudaMemcpyAsync(h_num_unique, s.total, 4 * h_words, cudaMemcpyDeviceToHost, stream));
   MEB_CUDA(cudaStreamSynchronize(stream));
   uint32_t m = *h_num_unique;
   if (m != n) {  // duplicates or masked rows: rebuild the table over the compacted rows
@@ -308,6 +292,32 @@ int meb200_insert_and_map(const int32_t *coords, const uint8_t *valid, uint32_t 
     }
   }
   return MEB200_OK;
+}
+
+}  // namespace meb200
+
+using namespace meb200;
+
+extern "C" {
+
+uint32_t meb200_hash_capacity(uint32_t n) {
+  uint64_t want = (uint64_t)n * 3u;
+  uint64_t cap = 1024;
+  while (cap < want) cap <<= 1;
+  return (uint32_t)(cap > 0x80000000ull ? 0x80000000ull : cap);
+}
+
+uint64_t meb200_insert_scratch_bytes(uint32_t n) {
+  return 4ull * (2ull * n + scan_blocks(n) + 8);
+}
+
+int meb200_insert_and_map(const int32_t *coords, const uint8_t *valid, uint32_t n,
+                          uint32_t ncols, uint32_t *table, uint32_t capacity,
+                          int32_t *unique_coords, int64_t *unique_index, int64_t *inverse_map,
+                          void *scratch, uint32_t *h_num_unique, void *stream_) {
+  return meb200::insert_and_map(coords, valid, n, ncols, table, capacity, unique_coords,
+                                unique_index, inverse_map, scratch, h_num_unique, 1,
+                                (cudaStream_t)stream_);
 }
 
 int meb200_insert_and_map_enqueue(const int32_t *coords, const uint8_t *valid,

@@ -11,33 +11,6 @@
 
 namespace meb200 {
 
-// V elements of T per access: 16 bytes when V = 16 / sizeof(T), one element when V = 1
-template <typename T, int V>
-__device__ __forceinline__ void load_f32(const T *p, float (&f)[V]) {
-  if constexpr (V == 1) {
-    f[0] = to_f32<T>(*p);
-  } else {
-    static_assert(V * sizeof(T) == 16, "16-byte vectors");
-    uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
-    const T *e = reinterpret_cast<const T *>(&v);
-#pragma unroll
-    for (int j = 0; j < V; ++j) f[j] = to_f32<T>(e[j]);
-  }
-}
-
-template <typename T, int V>
-__device__ __forceinline__ void store_f32(T *p, const float (&f)[V]) {
-  if constexpr (V == 1) {
-    *p = from_f32<T>(f[0]);
-  } else {
-    uint4 v;
-    T *e = reinterpret_cast<T *>(&v);
-#pragma unroll
-    for (int j = 0; j < V; ++j) e[j] = from_f32<T>(f[j]);
-    *reinterpret_cast<uint4 *>(p) = v;
-  }
-}
-
 template <int OP>
 __device__ __forceinline__ float fold_op(float a, float b) {
   if (OP == MEB200_UNION_ADD) return a + b;

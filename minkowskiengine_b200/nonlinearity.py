@@ -3,7 +3,7 @@
 import torch
 
 from .common import MinkowskiModuleBase
-from .sparse_tensor import SparseTensor
+from .tensor_field import same_kind as _same_kind
 
 
 class MinkowskiNonlinearityBase(MinkowskiModuleBase):
@@ -15,8 +15,7 @@ class MinkowskiNonlinearityBase(MinkowskiModuleBase):
 
     def forward(self, input):
         output = self.module(input.F)
-        return SparseTensor(output, coordinate_map_key=input.coordinate_map_key,
-                            coordinate_manager=input.coordinate_manager)
+        return _same_kind(input, output)
 
     def __repr__(self):
         return self.__class__.__name__ + "()"

@@ -23,6 +23,7 @@ import torch.nn as nn
 
 from . import _lib
 from .sparse_tensor import SparseTensor
+from .tensor_field import same_kind as _same_kind
 
 _USE_TORCH = os.environ.get("MEB200_TORCH_BN", "0") not in ("", "0")
 _USE_PEER = os.environ.get("MEB200_SYNCBN_PEER", "1") not in ("", "0")
@@ -292,8 +293,7 @@ class MinkowskiBatchNorm(nn.Module):
 
     def forward(self, input):
         output = _batch_norm(self.bn, input.F)
-        return SparseTensor(output, coordinate_map_key=input.coordinate_map_key,
-                            coordinate_manager=input.coordinate_manager)
+        return _same_kind(input, output)
 
     def __repr__(self):
         s = "({}, eps={}, momentum={}, affine={}, track_running_stats={})".format(
@@ -321,8 +321,7 @@ class MinkowskiSyncBatchNorm(MinkowskiBatchNorm):
 
     def forward(self, input):
         output = _batch_norm(self.bn, input.F, self._group())
-        return SparseTensor(output, coordinate_map_key=input.coordinate_map_key,
-                            coordinate_manager=input.coordinate_manager)
+        return _same_kind(input, output)
 
     @classmethod
     def convert_sync_batchnorm(cls, module, process_group=None):

@@ -1,10 +1,12 @@
-"""Feature-level helpers used by the networks on the path: `cat`, `MinkowskiLinear`
-(reference: MinkowskiOps.py:40-160)."""
+"""Feature-level helpers used by the networks on the path: `cat`, `MinkowskiLinear`,
+`MinkowskiToSparseTensor` (reference: MinkowskiOps.py:40-160, :276-352)."""
 import torch
 from torch.nn import Module
 
 from .sparse_tensor import (COORDINATE_KEY_DIFFERENT_ERROR, COORDINATE_MANAGER_DIFFERENT_ERROR,
                             SparseTensor)
+from .tensor_field import TensorField
+from .tensor_field import same_kind as _same_kind
 
 
 class MinkowskiLinear(Module):
@@ -14,8 +16,7 @@ class MinkowskiLinear(Module):
 
     def forward(self, input):
         output = self.linear(input.F)
-        return SparseTensor(output, coordinate_map_key=input.coordinate_map_key,
-                            coordinate_manager=input.coordinate_manager)
+        return _same_kind(input, output)
 
     def __repr__(self):
         return (f"{self.__class__.__name__}(in_features={self.linear.in_features}, "
@@ -23,16 +24,30 @@ class MinkowskiLinear(Module):
 
 
 def cat(*sparse_tensors):
-    """Concatenate features of tensors living on the SAME coordinate map
-    (reference: MinkowskiOps.py:70-110)."""
+    """Concatenate features of tensors living on the SAME coordinate map, or of TensorFields on the
+    same field key (reference: MinkowskiOps.py:70-110)."""
     assert len(sparse_tensors) > 1, f"Invalid number of inputs. The input must be at least two len(sparse_tensors) > 1"
     first = sparse_tensors[0]
-    assert isinstance(first, SparseTensor), "Inputs must be SparseTensors"
+    assert isinstance(first, (SparseTensor, TensorField)), \
+        "Inputs must be either SparseTensors or TensorFields."
     for s in sparse_tensors:
-        assert isinstance(s, SparseTensor), "Inputs must be either SparseTensors or TensorFields."
+        assert isinstance(s, type(first)), "Inputs must be either SparseTensors or TensorFields."
         assert first.coordinate_manager == s.coordinate_manager, COORDINATE_MANAGER_DIFFERENT_ERROR
         assert first.coordinate_map_key == s.coordinate_map_key, \
             COORDINATE_KEY_DIFFERENT_ERROR + str(first.coordinate_map_key) + " != " + str(s.coordinate_map_key)
     feats = torch.cat([s.F for s in sparse_tensors], dim=1)
-    return SparseTensor(feats, coordinate_map_key=first.coordinate_map_key,
-                        coordinate_manager=first.coordinate_manager)
+    return _same_kind(first, feats)
+
+
+class MinkowskiToSparseTensor(Module):
+    """TensorField -> SparseTensor through `TensorField.sparse()` (a SparseTensor passes through)
+    (reference: MinkowskiOps.py:276-352)."""
+
+    def forward(self, input):
+        if isinstance(input, TensorField):
+            return input.sparse()
+        assert isinstance(input, SparseTensor), "Input must be a TensorField or a SparseTensor"
+        return input
+
+    def __repr__(self):
+        return self.__class__.__name__ + "()"

@@ -359,6 +359,33 @@ class SparseTensor(Tensor):
             features = features[unique_index]
         return coordinates, features, coordinate_map_key
 
+    # -- tensor fields (reference: MinkowskiSparseTensor.py:559-718) -----------------------
+    def slice(self, X):
+        """Features of this tensor on the points of X (a TensorField or the SparseTensor whose
+        quantisation made this map), as a TensorField in X's point order."""
+        from .tensor_field import slice_sparse
+        return slice_sparse(self, X)
+
+    def cat_slice(self, X):
+        """slice(X) with X's own features concatenated after this tensor's."""
+        from .tensor_field import cat_slice_sparse
+        return cat_slice_sparse(self, X)
+
+    def interpolate(self, X):
+        """Features interpolated multilinearly at the points of TensorField X."""
+        from .tensor_field import TensorField
+        assert isinstance(X, TensorField)
+        return TensorField(self.features_at_coordinates(X.C),
+                           coordinate_field_map_key=X.coordinate_field_map_key,
+                           coordinate_manager=X.coordinate_manager)
+
+    def features_at_coordinates(self, query_coordinates: torch.Tensor):
+        """[N, C] features interpolated at float32 / float64 points [N, D+1] (rows of zeros where no
+        corner of a point is in the map)."""
+        from .interpolation import MinkowskiInterpolationFunction
+        return MinkowskiInterpolationFunction.apply(self._F, query_coordinates,
+                                                    self.coordinate_map_key, self._manager)[0]
+
     def dense(self, shape=None, min_coordinate=None, contract_stride=True):
         """Dense [B, C, X1..XD] tensor (reference: MinkowskiSparseTensor.py:347-448)."""
         ts = torch.tensor(self.tensor_stride, device=self.device, dtype=torch.int64)
