@@ -242,6 +242,27 @@ int meb200_conv_stem_wgrad(const void *in4, const void *grad_out, int dtype, uin
                            float *grad_weight_v, void *workspace, uint64_t workspace_bytes,
                            void *stream);
 
+/* ---- channel-wise (depthwise) convolution (reference: MinkowskiChannelwiseConvolution.py:142-191,
+ *      a per-offset torch loop with an autograd backward).  W: fp32 [K, C], one weight per offset
+ *      and channel.  Every output element is written once: no memset, no atomics, bit-identical
+ *      results run to run; fp32 accumulation, one rounding to the feature dtype; 16-byte accesses
+ *      where C * sizeof(dtype) % 16 == 0 and the pointers allow, any C >= 1 otherwise. --------- */
+/* y[r, c] = sum over k ascending with nbr[k, r] >= 0 of W[k, c] * x[nbr[k, r], c] (0 for a row
+ * without neighbours), r < n_rows.  x: [n_x, C], y: [n_rows, C] in `dtype`; nbr: [K, n_rows].
+ * Forward: nbr = out_nbr, x = the input features.  Input gradient: nbr = in_nbr, x = the output
+ * gradient, the same W. */
+int meb200_chwise_gather(const void *x, int dtype, uint32_t n_x, uint32_t C, const float *W,
+                         const int32_t *nbr, uint32_t K, uint32_t n_rows, void *y, void *stream);
+/* dW[k, c] (fp32 [K, C], fully written) = sum over o with out_nbr[k, o] >= 0 of
+ * x[out_nbr[k, o], c] * g[o, c].  x: [n_x, C], g: [n_out, C] in `dtype`.  workspace:
+ * meb200_chwise_wgrad_workspace_bytes(n_out, C, K, dtype) bytes, 16-byte aligned, for the row
+ * splits' partial sums, added in split order; less, NULL or unaligned is legal and means fewer
+ * splits, down to one. */
+uint64_t meb200_chwise_wgrad_workspace_bytes(uint32_t n_out, uint32_t C, uint32_t K, int dtype);
+int meb200_chwise_wgrad(const void *x, const void *g, int dtype, uint32_t n_x, uint32_t C,
+                        const int32_t *out_nbr, uint32_t K, uint32_t n_out, float *dW,
+                        void *workspace, uint64_t workspace_bytes, void *stream);
+
 /* ---- local pooling (reference a11: src/pooling_avg_kernel.hpp:40-150,
  *      src/pooling_max_kernel.hpp:35-115, src/local_pooling_cpu.cpp:43-185) ---------- */
 /* aux: AVG -> num_nonzero [n_out] (feature dtype); MAX -> max_index int32 [n_out, C]

@@ -6,7 +6,7 @@ hot path of NVIDIA/MinkowskiEngine, behind the reference's own Python API.
     y = ME.MinkowskiConvolution(64, 128, kernel_size=3, stride=2, dimension=3).cuda()(x)
 
 Scope (SURVEY.md §8): SparseTensor / CoordinateManager / kernel maps, MinkowskiConvolution,
-MinkowskiConvolutionTranspose, local and global pooling, broadcast, batch and instance
+MinkowskiConvolutionTranspose, MinkowskiChannelwiseConvolution (depthwise), local and global pooling, broadcast, batch and instance
 normalisation, pruning, union and arithmetic between sparse tensors on different coordinate maps,
 TensorField (point features quantised to voxels, sliced back and interpolated), and the thin torch
 wrappers MinkUNet, the ResNet classifiers and generative networks need.
@@ -31,6 +31,8 @@ from .coordinate_manager import (CoordinateManager, CoordsManager, set_gpu_alloc
 from .convolution import (MinkowskiConvolution, MinkowskiConvolutionFunction,
                           MinkowskiConvolutionTranspose, MinkowskiConvolutionTransposeFunction,
                           MinkowskiGenerativeConvolutionTranspose)
+from .channelwise_convolution import (MinkowskiChannelwiseConvolution,
+                                      MinkowskiChannelwiseConvolutionFunction)
 from .pooling import (MinkowskiAvgPooling, MinkowskiGlobalAvgPooling, MinkowskiGlobalMaxPooling,
                       MinkowskiGlobalPooling, MinkowskiGlobalPoolingFunction,
                       MinkowskiGlobalSumPooling, MinkowskiLocalPoolingFunction, MinkowskiMaxPooling,

@@ -58,7 +58,11 @@ PROTOTYPES = {
     "meb200_pair_list_capacity": (_u64, [_u32, _u32, _u32, _u32]),
     "meb200_kernel_map_pairs": (_i32, [_vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "meb200_conv_workspace_bytes": (_u64, [_u32, _u32, _u32, _u32, _i32]),
-    "meb200_pool_forward": (_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _u32, _i32, _vp, _vp, _vp]),
+    "meb200_chwise_gather": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _vp]),
+    "meb200_chwise_wgrad_workspace_bytes": (_u64, [_u32, _u32, _u32, _i32]),
+    "meb200_chwise_wgrad": (_i32, [_vp, _vp, _i32, _u32, _u32, _vp, _u32, _u32, _vp, _vp, _u64,
+                                   _vp]),
+    "meb200_pool_forward":(_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _u32, _i32, _vp, _vp, _vp]),
     "meb200_pool_backward": (_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _u32, _i32, _vp, _vp,
                                     _vp]),
     "meb200_origin_group_scratch_bytes": (_u64, [_u32, _u32]),

@@ -1495,6 +1495,77 @@ def LocalPoolingBackwardGPU(in_feat, grad_out_feat, num_nonzero, kernel_size, ke
     return grad_in
 
 
+# ---- channel-wise (depthwise) convolution ------------------------------------------------------
+def _chwise_map(in_feat, kernel, kernel_size, kernel_stride, kernel_dilation, region_type, offset,
+                in_key, out_key, manager):
+    """The convolution's own kernel map (is_transpose = is_pool = False): a MinkowskiConvolution
+    of the same geometry shares the cache entry, and the map prefetch predicts it."""
+    km = manager._kernel_map(in_key, out_key, kernel_size, kernel_stride, kernel_dilation,
+                             region_type, offset, False, False)
+    _assert(kernel.dim() == 2 and kernel.size(0) == km.K, "kernel shape", list(kernel.shape),
+            "does not match the kernel volume", km.K)
+    _assert(kernel.size(1) == in_feat.size(1), "Input feature size and kernel size mismatch")
+    return km
+
+
+def ChannelwiseConvolutionForwardGPU(in_feat, kernel, kernel_size, kernel_stride, kernel_dilation,
+                                     region_type, offset, in_key, out_key, manager):
+    """y[o, c] = sum_k kernel[k, c] * in_feat[out_nbr[k, o], c] in the feature dtype (reference:
+    MinkowskiChannelwiseConvolution.py:142-191, a per-offset torch loop).  The kernel is read as
+    fp32 [K, C] whatever its dtype.  Mutates `out_key` when it is unset."""
+    _check_feats(in_feat, manager, in_key)
+    _assert(kernel.is_cuda, "kernel must be CUDA")
+    if not out_key.is_key_set():
+        ok, _ = manager._stride(in_key, kernel_stride)
+        out_key.set_key(list(ok[0]), ok[1])
+    km = _chwise_map(in_feat, kernel, kernel_size, kernel_stride, kernel_dilation, region_type,
+                     offset, in_key, out_key, manager)
+    lib = _lib.load()
+    C = in_feat.size(1)
+    w = kernel.detach().float().contiguous()
+    out = torch.empty((km.n_out, C), dtype=in_feat.dtype, device=in_feat.device)
+    _lib.check(lib.meb200_chwise_gather(
+        _lib.ptr(in_feat), _lib.dtype_code(in_feat.dtype), km.n_in, C, _lib.ptr(w),
+        _lib.ptr(km.out_nbr), km.K, km.n_out, _lib.ptr(out), _lib.current_stream()))
+    return out
+
+
+def ChannelwiseConvolutionBackwardGPU(in_feat, grad_out_feat, kernel, kernel_size, kernel_stride,
+                                      kernel_dilation, region_type, offset, in_key, out_key,
+                                      manager, need_in=True, need_w=True):
+    """(grad_in in the feature dtype, grad_kernel in the kernel's dtype; None where not needed).
+    grad_in[i, c] = sum_k kernel[k, c] * grad_out[in_nbr[k, i], c] (the forward's gather over the
+    reverse table, built only when asked for); grad_kernel[k, c] = sum_o in[out_nbr[k, o], c] *
+    grad_out[o, c], accumulated in fp32."""
+    _check_feats(in_feat, manager, in_key)
+    _assert(kernel.is_cuda, "kernel must be CUDA")
+    _assert(manager.exists(out_key), ERROR_MAP_NOT_FOUND)
+    _assert(grad_out_feat.size(0) == manager.size(out_key), "Invalid grad_out size")
+    km = _chwise_map(in_feat, kernel, kernel_size, kernel_stride, kernel_dilation, region_type,
+                     offset, in_key, out_key, manager)
+    lib = _lib.load()
+    code = _lib.dtype_code(in_feat.dtype)
+    grad_out = grad_out_feat.to(in_feat.dtype).contiguous()
+    K, C = kernel.shape
+    grad_in = grad_w = None
+    if need_in:
+        w = kernel.detach().float().contiguous()
+        grad_in = torch.empty_like(in_feat)
+        _lib.check(lib.meb200_chwise_gather(
+            _lib.ptr(grad_out), code, km.n_out, C, _lib.ptr(w), _lib.ptr(km.in_nbr), K, km.n_in,
+            _lib.ptr(grad_in), _lib.current_stream()))
+    if need_w:
+        grad_w = torch.empty((K, C), dtype=torch.float32, device=in_feat.device)
+        nbytes = int(lib.meb200_chwise_wgrad_workspace_bytes(km.n_out, C, K, code))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=in_feat.device) if nbytes else None
+        _lib.check(lib.meb200_chwise_wgrad(
+            _lib.ptr(in_feat), _lib.ptr(grad_out), code, km.n_in, C, _lib.ptr(km.out_nbr), K,
+            km.n_out, _lib.ptr(grad_w), _lib.ptr(ws), nbytes, _lib.current_stream()))
+        if grad_w.dtype != kernel.dtype:
+            grad_w = grad_w.to(kernel.dtype)
+    return grad_in, grad_w
+
+
 # ---- global pooling and broadcast over the origin map ------------------------------------------
 _GLOBAL_CODE = {PoolingMode.GLOBAL_SUM_POOLING_DEFAULT: _lib.SEG_SUM,
                 PoolingMode.GLOBAL_SUM_POOLING_KERNEL: _lib.SEG_SUM,

@@ -180,8 +180,8 @@ k_split_sum(const float *__restrict__ part, float *__restrict__ dW, size_t n, ui
   }
 }
 
-static int launch_split_sum(const float *part, float *dW, size_t n, uint32_t splits,
-                            cudaStream_t stream) {
+int launch_split_sum(const float *part, float *dW, size_t n, uint32_t splits,
+                     cudaStream_t stream) {
   const unsigned blocks = (unsigned)std::min<size_t>(cdiv(n, 256), 4096);
   k_split_sum<<<blocks, 256, 0, stream>>>(part, dW, n, splits);
   MEB_LAUNCH_OK();
