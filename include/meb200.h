@@ -179,9 +179,10 @@ int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_
  * NULL) + n_chunks: the compacted pair lists of out_nbr from meb200_kernel_map_pairs with
  * stage = 64 and their chunk count; when meb200_conv_wgrad_uses_pairs() holds, the wgrad reduces
  * over them instead of the dense table.
- * workspace: meb200_conv_workspace_bytes(n_out, c_in, c_out, K, dtype) bytes.  Every wgrad
- * kernel stores its row splits' partial sums there and adds them in split order (no atomics:
- * bit-identical run to run); less or NULL is legal and means fewer splits, down to one. */
+ * workspace: meb200_conv_workspace_bytes(n_out, c_in, c_out, K, dtype) bytes, 16-byte aligned.
+ * Every wgrad kernel stores its row splits' partial sums there and adds them in split order (no
+ * atomics: bit-identical run to run).  It runs as many of its planned splits as the workspace
+ * holds; less, NULL or unaligned is legal and means fewer splits, down to one. */
 int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32_t n_in,
                          uint32_t c_in, const void *w_cast, uint32_t K, uint32_t c_out,
                          const int32_t *out_nbr, const int32_t *in_nbr, uint32_t n_out,
@@ -230,7 +231,8 @@ int meb200_conv_pack_weights_batched(const meb200_pack_job *jobs_dev, uint32_t n
  *                              Wv[4 k + c][n] = W[k][c][n] (zero for padded k, c)
  *   grad_weight_v  [V, c_out]  fp32, same indexing (fully written by the call)
  *   workspace      meb200_conv_workspace_bytes(n_out, V, c_out, 1, dtype) bytes, 16-byte aligned,
- *                  for the row-split partial sums (less, NULL or unaligned is legal: fewer splits)
+ *                  for the row-split partial sums, as in meb200_conv_backward (less, NULL or
+ *                  unaligned is legal and means fewer splits, down to one)
  * bf16 / fp16 only; c_out a multiple of 16, <= 256. */
 uint32_t meb200_conv_stem_virtual_channels(uint32_t K);
 int meb200_conv_stem_supported(int dtype, uint32_t K, uint32_t c_out);
@@ -256,8 +258,8 @@ int meb200_chwise_gather(const void *x, int dtype, uint32_t n_x, uint32_t C, con
 /* dW[k, c] (fp32 [K, C], fully written) = sum over o with out_nbr[k, o] >= 0 of
  * x[out_nbr[k, o], c] * g[o, c].  x: [n_x, C], g: [n_out, C] in `dtype`.  workspace:
  * meb200_chwise_wgrad_workspace_bytes(n_out, C, K, dtype) bytes, 16-byte aligned, for the row
- * splits' partial sums, added in split order; less, NULL or unaligned is legal and means fewer
- * splits, down to one. */
+ * splits' partial sums, added in split order, as in meb200_conv_backward (less, NULL or unaligned
+ * is legal and means fewer splits, down to one). */
 uint64_t meb200_chwise_wgrad_workspace_bytes(uint32_t n_out, uint32_t C, uint32_t K, int dtype);
 int meb200_chwise_wgrad(const void *x, const void *g, int dtype, uint32_t n_x, uint32_t C,
                         const int32_t *out_nbr, uint32_t K, uint32_t n_out, float *dW,

@@ -436,12 +436,9 @@ int meb200_bn_apply_fused(const void *x, int dtype, uint32_t n, uint32_t C, cons
   if (n == 0) return MEB200_OK;
   unsigned grid;
   uint32_t rows = bn_rows_per_cta(n, C, &grid);
-  switch (dtype) {
-    case MEB200_F32: k_bn_apply<float, 0><<<grid, kBnThreads, 0, s>>>((const float *)x, nullptr, (const float *)residual, mean, invstd, weight, bias, nullptr, 1.0, nullptr, n, C, rows, relu, (float *)y, nullptr); break;
-    case MEB200_BF16: k_bn_apply<__nv_bfloat16, 0><<<grid, kBnThreads, 0, s>>>((const __nv_bfloat16 *)x, nullptr, (const __nv_bfloat16 *)residual, mean, invstd, weight, bias, nullptr, 1.0, nullptr, n, C, rows, relu, (__nv_bfloat16 *)y, nullptr); break;
-    case MEB200_F16: k_bn_apply<__half, 0><<<grid, kBnThreads, 0, s>>>((const __half *)x, nullptr, (const __half *)residual, mean, invstd, weight, bias, nullptr, 1.0, nullptr, n, C, rows, relu, (__half *)y, nullptr); break;
-    default: set_error("batch norm: unsupported dtype %d", dtype); return MEB200_ERR_UNSUPPORTED;
-  }
+  MEB_DISPATCH_DTYPE(dtype, k_bn_apply<T, 0><<<grid, kBnThreads, 0, s>>>(
+                                (const T *)x, nullptr, (const T *)residual, mean, invstd, weight,
+                                bias, nullptr, 1.0, nullptr, n, C, rows, relu, (T *)y, nullptr));
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
@@ -458,23 +455,14 @@ static int bn_launch_reduce(int mode, const void *a, const void *x, const void *
   }
   if (grid == 0) grid = 1;          // an empty rank still takes part in the exchange
   const size_t smem = bn_reduce_smem(C);
-#define MEB_BN_RED(TT)                                                                            \
-  do {                                                                                            \
-    if (mode == 0)                                                                                \
-      k_bn_reduce<TT, 0><<<grid, kBnThreads, smem, s>>>((const TT *)a, nullptr, nullptr, nullptr, \
-                                                       nullptr, n, C, rows, sums, tail);          \
-    else                                                                                          \
-      k_bn_reduce<TT, 1><<<grid, kBnThreads, smem, s>>>((const TT *)a, (const TT *)x,             \
-                                                       (const TT *)ymask, mean, invstd, n, C,     \
-                                                       rows, sums, tail);                         \
-  } while (0)
-  switch (dtype) {
-    case MEB200_F32: MEB_BN_RED(float); break;
-    case MEB200_BF16: MEB_BN_RED(__nv_bfloat16); break;
-    case MEB200_F16: MEB_BN_RED(__half); break;
-    default: set_error("batch norm: unsupported dtype %d", dtype); return MEB200_ERR_UNSUPPORTED;
-  }
-#undef MEB_BN_RED
+  MEB_DISPATCH_DTYPE(dtype,
+    if (mode == 0)
+      k_bn_reduce<T, 0><<<grid, kBnThreads, smem, s>>>((const T *)a, nullptr, nullptr, nullptr,
+                                                      nullptr, n, C, rows, sums, tail);
+    else
+      k_bn_reduce<T, 1><<<grid, kBnThreads, smem, s>>>((const T *)a, (const T *)x,
+                                                      (const T *)ymask, mean, invstd, n, C, rows,
+                                                      sums, tail));
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
@@ -608,12 +596,10 @@ int meb200_bn_backward_apply_fused(const void *dy, const void *x, const void *y_
   MEB_CHECK_ARG(count > 0 || d_count != nullptr, "count");
   unsigned grid;
   uint32_t rows = bn_rows_per_cta(n, C, &grid);
-  switch (dtype) {
-    case MEB200_F32: k_bn_apply<float, 1><<<grid, kBnThreads, 0, s>>>((const float *)dy, (const float *)x, (const float *)y_mask, mean, invstd, weight, nullptr, sums, count, d_count, n, C, rows, 0, (float *)dx, (float *)d_residual); break;
-    case MEB200_BF16: k_bn_apply<__nv_bfloat16, 1><<<grid, kBnThreads, 0, s>>>((const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)x, (const __nv_bfloat16 *)y_mask, mean, invstd, weight, nullptr, sums, count, d_count, n, C, rows, 0, (__nv_bfloat16 *)dx, (__nv_bfloat16 *)d_residual); break;
-    case MEB200_F16: k_bn_apply<__half, 1><<<grid, kBnThreads, 0, s>>>((const __half *)dy, (const __half *)x, (const __half *)y_mask, mean, invstd, weight, nullptr, sums, count, d_count, n, C, rows, 0, (__half *)dx, (__half *)d_residual); break;
-    default: set_error("batch norm: unsupported dtype %d", dtype); return MEB200_ERR_UNSUPPORTED;
-  }
+  MEB_DISPATCH_DTYPE(dtype, k_bn_apply<T, 1><<<grid, kBnThreads, 0, s>>>(
+                                (const T *)dy, (const T *)x, (const T *)y_mask, mean, invstd,
+                                weight, nullptr, sums, count, d_count, n, C, rows, 0, (T *)dx,
+                                (T *)d_residual));
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }

@@ -10,7 +10,7 @@
 // gather, a fixed row order in the wgrad) and rounded once; no atomics, bit-identical run to run.
 #include <algorithm>
 
-#include "conv_simt.cuh"
+#include "common.cuh"
 
 namespace meb200 {
 
@@ -145,8 +145,6 @@ k_chwise_wgrad(const T *__restrict__ x, const T *__restrict__ g, uint32_t C,
   for (int v = 0; v < V; ++v) dst[v] = acc[v];
 }
 
-static bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 // Vector lanes of one wgrad slab: the row's vectors, rounded up to a power of two, at most 32.
 static uint32_t wgrad_slab_lanes(uint32_t vpr) {
   uint32_t s = 1;
@@ -154,18 +152,12 @@ static uint32_t wgrad_slab_lanes(uint32_t vpr) {
   return s;
 }
 
-// Rows per split of k_chwise_wgrad (at most max_splits splits): about eight 256-thread CTAs per SM
-// over the grid, each split at least 1024 rows.
-static uint32_t chwise_wgrad_rows(uint32_t vpr, uint32_t K, uint32_t n_out, uint64_t max_splits) {
+// Row splits k_chwise_wgrad plans: about eight 256-thread CTAs per SM over the grid, each split at
+// least 1024 rows.
+static uint32_t chwise_wgrad_splits(uint32_t vpr, uint32_t K, uint32_t n_out) {
   const uint64_t slabs = cdiv(vpr, wgrad_slab_lanes(vpr));
-  uint64_t splits = std::max<uint64_t>(1, cdiv(8ull * num_sms(), (uint64_t)K * slabs));
-  splits = std::min<uint64_t>({splits, cdiv(n_out, 1024), 65535, max_splits});
-  return cdiv(n_out, splits);
-}
-
-static uint32_t vec_width(int dtype, uint32_t C) {
-  const size_t s = dtype_size(dtype);
-  return (C * s) % 16 == 0 ? (uint32_t)(16 / s) : 1;
+  const uint64_t splits = std::max<uint64_t>(1, cdiv(8ull * num_sms(), (uint64_t)K * slabs));
+  return (uint32_t)std::min<uint64_t>({splits, cdiv(n_out, 1024), 65535});
 }
 
 template <typename T, int V>
@@ -178,22 +170,14 @@ static int launch_gather(const void *x, uint32_t C, const float *W, const int32_
   return MEB200_OK;
 }
 
-template <typename T>
-static int gather_t(const void *x, uint32_t C, const float *W, const int32_t *nbr, uint32_t K,
-                    uint32_t n_rows, void *y, bool vec, cudaStream_t stream) {
-  if (vec) return launch_gather<T, 16 / sizeof(T)>(x, C, W, nbr, K, n_rows, y, stream);
-  return launch_gather<T, 1>(x, C, W, nbr, K, n_rows, y, stream);
-}
-
 template <typename T, int V>
 static int launch_wgrad(const void *x, const void *g, uint32_t C, const int32_t *out_nbr,
                         uint32_t K, uint32_t n_out, float *dW, void *workspace,
                         uint64_t workspace_bytes, cudaStream_t stream) {
   const uint32_t vpr = C / V, S = wgrad_slab_lanes(vpr);
-  // a missing or small workspace leaves fewer splits (one: the CTAs store into dW directly)
-  const uint64_t slot = (uint64_t)K * C * sizeof(float);
-  const uint64_t fit = workspace == nullptr ? 1 : std::max<uint64_t>(1, workspace_bytes / slot);
-  const uint32_t rows = chwise_wgrad_rows(vpr, K, n_out, fit);
+  const uint32_t planned = chwise_wgrad_splits(vpr, K, n_out);
+  const uint32_t rows = cdiv(n_out, workspace_splits(planned, workspace, workspace_bytes,
+                                                     (uint64_t)K * C * sizeof(float)));
   const uint32_t splits = cdiv(n_out, rows);
   float *part = splits > 1 ? reinterpret_cast<float *>(workspace) : dW;
   dim3 grid(K, splits, cdiv(vpr, S)), block(S, CW_THREADS / S);
@@ -202,16 +186,6 @@ static int launch_wgrad(const void *x, const void *g, uint32_t C, const int32_t 
   MEB_LAUNCH_OK();
   if (splits == 1) return MEB200_OK;
   return launch_split_sum(part, dW, (size_t)K * C, splits, stream);
-}
-
-template <typename T>
-static int wgrad_t(const void *x, const void *g, uint32_t C, const int32_t *out_nbr, uint32_t K,
-                   uint32_t n_out, float *dW, void *workspace, uint64_t workspace_bytes, bool vec,
-                   cudaStream_t stream) {
-  if (vec)
-    return launch_wgrad<T, 16 / sizeof(T)>(x, g, C, out_nbr, K, n_out, dW, workspace,
-                                           workspace_bytes, stream);
-  return launch_wgrad<T, 1>(x, g, C, out_nbr, K, n_out, dW, workspace, workspace_bytes, stream);
 }
 
 }  // namespace meb200
@@ -226,20 +200,15 @@ int meb200_chwise_gather(const void *x, int dtype, uint32_t n_x, uint32_t C, con
   MEB_CHECK_ARG(K >= 1, "kernel volume %u", K);
   MEB_CHECK_ARG(x != nullptr || n_x == 0, "null x with %u rows", n_x);
   MEB_CHECK_ARG(W && nbr && y, "null buffer");
-  const bool vec = vec_width(dtype, C) > 1 && aligned16(x) && aligned16(y) && aligned16(W);
   cudaStream_t s = (cudaStream_t)stream;
-  switch (dtype) {
-    case MEB200_F32: return gather_t<float>(x, C, W, nbr, K, n_rows, y, vec, s);
-    case MEB200_BF16: return gather_t<__nv_bfloat16>(x, C, W, nbr, K, n_rows, y, vec, s);
-    case MEB200_F16: return gather_t<__half>(x, C, W, nbr, K, n_rows, y, vec, s);
-  }
-  set_error("channel-wise convolution: unsupported dtype %d", dtype);
-  return MEB200_ERR_UNSUPPORTED;
+  MEB_DISPATCH_DTYPE(dtype, MEB_DISPATCH_VEC(T, C, aligned(16, x, y, W),
+                                             return launch_gather<T, V>(x, C, W, nbr, K, n_rows, y, s)));
 }
 
 uint64_t meb200_chwise_wgrad_workspace_bytes(uint32_t n_out, uint32_t C, uint32_t K, int dtype) {
   if (n_out == 0 || C == 0 || K == 0) return 0;
-  const uint32_t rows = chwise_wgrad_rows(C / vec_width(dtype, C), K, n_out, UINT64_MAX);
+  const uint32_t vpr = C / vec_elems(dtype_size(dtype), C);
+  const uint32_t rows = cdiv(n_out, chwise_wgrad_splits(vpr, K, n_out));
   const uint32_t splits = cdiv(n_out, rows);
   return splits > 1 ? (uint64_t)splits * K * C * sizeof(float) : 0;
 }
@@ -256,19 +225,9 @@ int meb200_chwise_wgrad(const void *x, const void *g, int dtype, uint32_t n_x, u
   }
   MEB_CHECK_ARG(x != nullptr || n_x == 0, "null x with %u rows", n_x);
   MEB_CHECK_ARG(g && out_nbr, "null buffer");
-  if (workspace != nullptr && !aligned16(workspace)) workspace = nullptr;   // one split
-  const bool vec = vec_width(dtype, C) > 1 && aligned16(x) && aligned16(g);
-  switch (dtype) {
-    case MEB200_F32:
-      return wgrad_t<float>(x, g, C, out_nbr, K, n_out, dW, workspace, workspace_bytes, vec, s);
-    case MEB200_BF16:
-      return wgrad_t<__nv_bfloat16>(x, g, C, out_nbr, K, n_out, dW, workspace, workspace_bytes,
-                                    vec, s);
-    case MEB200_F16:
-      return wgrad_t<__half>(x, g, C, out_nbr, K, n_out, dW, workspace, workspace_bytes, vec, s);
-  }
-  set_error("channel-wise convolution wgrad: unsupported dtype %d", dtype);
-  return MEB200_ERR_UNSUPPORTED;
+  MEB_DISPATCH_DTYPE(dtype, MEB_DISPATCH_VEC(T, C, aligned(16, x, g),
+                                             return launch_wgrad<T, V>(x, g, C, out_nbr, K, n_out, dW,
+                                                                       workspace, workspace_bytes, s)));
 }
 
 }

@@ -1,6 +1,8 @@
-// Library-level state: last error (per thread), launch counter, build facts.
+// Library-level state: last error (per thread), launch counter, build facts; the split reduction
+// shared by the weight gradients.
 #include <stdarg.h>
 
+#include <algorithm>
 #include <atomic>
 
 #include "common.cuh"
@@ -42,6 +44,42 @@ int num_sms() {
       cached = 132;   // H100 SXM
   }
   return cached;
+}
+
+uint32_t workspace_splits(uint32_t planned, const void *workspace, uint64_t workspace_bytes,
+                          uint64_t slot_bytes) {
+  if (workspace == nullptr || !aligned(16, workspace)) return 1;
+  return (uint32_t)std::min<uint64_t>(planned, std::max<uint64_t>(1, workspace_bytes / slot_bytes));
+}
+
+__device__ __forceinline__ void add(float &a, float b) { a += b; }
+__device__ __forceinline__ void add(float4 &a, float4 b) {
+  a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+}
+
+// F = float4: four consecutive elements per thread, each summed over the splits on its own
+template <typename F>
+__global__ void __launch_bounds__(256)
+k_split_sum(const F *__restrict__ part, F *__restrict__ dW, size_t n, uint32_t splits) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n;
+       i += (size_t)gridDim.x * blockDim.x) {
+    F a = part[i];
+    for (uint32_t s = 1; s < splits; ++s) add(a, part[s * n + i]);
+    dW[i] = a;
+  }
+}
+
+int launch_split_sum(const float *part, float *dW, size_t n, uint32_t splits,
+                     cudaStream_t stream) {
+  if (n % 4 == 0 && aligned(16, part, dW)) {
+    const size_t n4 = n / 4;
+    k_split_sum<float4><<<std::min(cdiv(n4, 256), 4096u), 256, 0, stream>>>(
+        reinterpret_cast<const float4 *>(part), reinterpret_cast<float4 *>(dW), n4, splits);
+  } else {
+    k_split_sum<float><<<std::min(cdiv(n, 256), 4096u), 256, 0, stream>>>(part, dW, n, splits);
+  }
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
 }
 
 }  // namespace meb200

@@ -180,6 +180,66 @@ template <> __device__ __forceinline__ __half from_f32<__half>(float v) { return
 
 inline size_t dtype_size(int dt) { return dt == MEB200_F32 ? 4 : 2; }
 
+// Every pointer is a multiple of `bytes` (a null pointer is)
+template <typename... P>
+inline bool aligned(size_t bytes, const P *...p) {
+  return ((reinterpret_cast<uintptr_t>(p) % bytes == 0) && ...);
+}
+
+// Elements of elem_bytes each per 16-byte vector when a row of C of them is a whole number of
+// such vectors, otherwise 1
+inline uint32_t vec_elems(size_t elem_bytes, uint32_t C) {
+  return C * elem_bytes % 16 == 0 ? (uint32_t)(16 / elem_bytes) : 1u;
+}
+
+// Dispatch a body templated on the feature type T over the runtime dtype.
+#define MEB_DISPATCH_DTYPE(dtype, ...)                                                   \
+  switch (dtype) {                                                                       \
+    case MEB200_F32: { using T = float; __VA_ARGS__; } break;                            \
+    case MEB200_BF16: { using T = __nv_bfloat16; __VA_ARGS__; } break;                   \
+    case MEB200_F16: { using T = __half; __VA_ARGS__; } break;                           \
+    default:                                                                             \
+      ::meb200::set_error("unsupported dtype %d", (int)(dtype));                         \
+      return MEB200_ERR_UNSUPPORTED;                                                     \
+  }
+
+// The same over (input dtype, output dtype), binding T and TO: a feature dtype to itself, or
+// bf16 / fp16 to fp32.
+#define MEB_DISPATCH_DTYPE_OUT(dtype, out_dtype, ...)                                    \
+  if ((out_dtype) == (dtype)) {                                                          \
+    MEB_DISPATCH_DTYPE(dtype, using TO = T; __VA_ARGS__);                                \
+  } else if ((out_dtype) == MEB200_F32 && (dtype) == MEB200_BF16) {                      \
+    using T = __nv_bfloat16; using TO = float; __VA_ARGS__;                              \
+  } else if ((out_dtype) == MEB200_F32 && (dtype) == MEB200_F16) {                       \
+    using T = __half; using TO = float; __VA_ARGS__;                                     \
+  } else {                                                                               \
+    ::meb200::set_error("unsupported dtypes in=%d out=%d", (int)(dtype), (int)(out_dtype)); \
+    return MEB200_ERR_UNSUPPORTED;                                                       \
+  }
+
+// Dispatch a body templated on V, the elements of T per access, over a row of C elements:
+// V = 16 / sizeof(T) when the row is a whole number of 16-byte vectors and `is_aligned` (the
+// pointers the kernel vectorises are 16-byte aligned), V = 1 otherwise.
+#define MEB_DISPATCH_VEC(T, C, is_aligned, ...)                                          \
+  if (::meb200::vec_elems(sizeof(T), C) > 1 && (is_aligned)) {                           \
+    constexpr int V = 16 / sizeof(T); __VA_ARGS__;                                       \
+  } else {                                                                               \
+    constexpr int V = 1; __VA_ARGS__;                                                    \
+  }
+
+// ---- deterministic split reduction -------------------------------------------------------
+// A weight gradient reduced over row splits stores each split's partial sums in its own slot of
+// the caller's workspace, then launch_split_sum adds the slots in split order: no atomics, so
+// results are bit-identical run to run.  With one split the kernel writes dW directly.
+
+// Splits to run of the `planned` ones, with slots of slot_bytes: as many as the workspace holds,
+// at least one; one when the workspace is null or not 16-byte aligned.
+uint32_t workspace_splits(uint32_t planned, const void *workspace, uint64_t workspace_bytes,
+                          uint64_t slot_bytes);
+
+// dW[i] = part[i] + part[n + i] + ... + part[(splits - 1) n + i], added in that order
+int launch_split_sum(const float *part, float *dW, size_t n, uint32_t splits, cudaStream_t stream);
+
 // V elements of T per access: 16 bytes when V = 16 / sizeof(T), one element when V = 1
 template <typename T, int V>
 __device__ __forceinline__ void load_f32(const T *p, float (&f)[V]) {

@@ -99,7 +99,7 @@ k_conv_gather_gemm(const TIn *__restrict__ A, uint32_t c_a, const TIn *__restric
 
 // part[split][k][ci][co] = sum over rows o in this CTA's split of in[nbr[k][o]][ci] * dOut[o][co]
 // Every element of the split's slot is stored once (zeros included); with one split the slot is
-// dW itself, otherwise k_split_sum adds the slots in split order.
+// dW itself, otherwise launch_split_sum adds the slots in split order.
 template <typename T>
 __global__ void __launch_bounds__(256)
 k_conv_wgrad(const T *__restrict__ in, const T *__restrict__ grad_out, uint32_t c_in,
@@ -167,33 +167,6 @@ k_conv_wgrad(const T *__restrict__ in, const T *__restrict__ grad_out, uint32_t 
       if (co < c_out) dWk[(size_t)ci * c_out + co] = acc[i][j];
     }
   }
-}
-
-// dW = part[0] + part[1] + ... + part[splits - 1], in that order
-__global__ void __launch_bounds__(256)
-k_split_sum(const float *__restrict__ part, float *__restrict__ dW, size_t n, uint32_t splits) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n;
-       i += (size_t)gridDim.x * blockDim.x) {
-    float a = part[i];
-    for (uint32_t s = 1; s < splits; ++s) a += part[s * n + i];
-    dW[i] = a;
-  }
-}
-
-int launch_split_sum(const float *part, float *dW, size_t n, uint32_t splits,
-                     cudaStream_t stream) {
-  const unsigned blocks = (unsigned)std::min<size_t>(cdiv(n, 256), 4096);
-  k_split_sum<<<blocks, 256, 0, stream>>>(part, dW, n, splits);
-  MEB_LAUNCH_OK();
-  return MEB200_OK;
-}
-
-// Splits that fit in `workspace_bytes`: one slot of K * c_in * c_out floats each (none: one split).
-static uint64_t workspace_slots(const void *workspace, uint64_t workspace_bytes, uint32_t c_in,
-                                uint32_t c_out, uint32_t K) {
-  if (workspace == nullptr) return 1;
-  const uint64_t fit = workspace_bytes / ((uint64_t)K * c_in * c_out * sizeof(float));
-  return fit > 1 ? fit : 1;
 }
 
 // ---- tiny input-channel count (the network stem: c_in <= 4, e.g. RGB -> 32, K = 125) -------
@@ -296,7 +269,7 @@ k_conv_small_cin_fwd(const T *__restrict__ in, uint32_t c_in, const T *__restric
 // every lane fetches its own dOut row slab (vector loads) and input row and accumulates a private
 // [CIN][32] tile in registers, so 32 row fetches are in flight per warp instead of one.  The
 // 32 private tiles are folded with butterfly shuffles once per warp and stored to the row slice's
-// slot part[slice][k][c][co] (dW itself with one slice); k_split_sum adds the slots in order.
+// slot part[slice][k][c][co] (dW itself with one slice); launch_split_sum adds the slots in order.
 constexpr int WG_SCAN = 256;             // table entries scanned per round (8 per lane)
 constexpr int WG_LIST = WG_SCAN + 32;    // + carried remainder (< 32)
 
@@ -433,26 +406,20 @@ int conv_small_cin_forward(const void *in, int in_dtype, uint32_t c_in, const vo
                            uint32_t c_out, const int32_t *nbr, uint32_t n_out, void *out,
                            int out_dtype, cudaStream_t stream) {
   if (n_out == 0) return MEB200_OK;
-  if (in_dtype == MEB200_F32 && out_dtype == MEB200_F32)
-    return launch_small_fwd<float, float>(in, c_in, W, K, c_out, nbr, n_out, out, stream);
-  if (in_dtype == MEB200_BF16 && out_dtype == MEB200_BF16)
-    return launch_small_fwd<__nv_bfloat16, __nv_bfloat16>(in, c_in, W, K, c_out, nbr, n_out, out, stream);
-  if (in_dtype == MEB200_BF16 && out_dtype == MEB200_F32)
-    return launch_small_fwd<__nv_bfloat16, float>(in, c_in, W, K, c_out, nbr, n_out, out, stream);
-  if (in_dtype == MEB200_F16 && out_dtype == MEB200_F16)
-    return launch_small_fwd<__half, __half>(in, c_in, W, K, c_out, nbr, n_out, out, stream);
-  if (in_dtype == MEB200_F16 && out_dtype == MEB200_F32)
-    return launch_small_fwd<__half, float>(in, c_in, W, K, c_out, nbr, n_out, out, stream);
-  return MEB200_ERR_UNSUPPORTED;
+  MEB_DISPATCH_DTYPE_OUT(in_dtype, out_dtype,
+                         return launch_small_fwd<T, TO>(in, c_in, W, K, c_out, nbr, n_out, out, stream));
 }
 
-// Row slices of k_conv_small_cin_wgrad (at most max_slices): one 8-warp CTA per SM (register
-// tiles), aiming at ~4 CTAs per SM over the whole grid; slices are whole scan rounds, >= 4 each.
-static uint32_t small_wgrad_rows(uint32_t c_out, uint32_t K, uint32_t n_out, uint64_t max_slices) {
+// Row slices k_conv_small_cin_wgrad plans: one 8-warp CTA per SM (register tiles), aiming at
+// ~4 CTAs per SM over the whole grid.
+static uint32_t small_wgrad_slices(uint32_t c_out, uint32_t K) {
   const uint32_t kgroups = cdiv(K, 8), slabs = cdiv(c_out, 32);
-  uint64_t want = std::max<uint64_t>(1, cdiv(4ull * num_sms(), (uint64_t)kgroups * slabs));
-  if (want > max_slices) want = max_slices;
-  uint32_t rows_per_block = cdiv(cdiv(n_out, (uint32_t)want), WG_SCAN) * WG_SCAN;
+  return std::max<uint32_t>(1, cdiv(4ull * num_sms(), (uint64_t)kgroups * slabs));
+}
+
+// Rows per slice for `slices` slices: whole scan rounds, >= 4 each.
+static uint32_t small_wgrad_rows(uint32_t n_out, uint32_t slices) {
+  const uint32_t rows_per_block = cdiv(cdiv(n_out, slices), WG_SCAN) * WG_SCAN;
   return std::max<uint32_t>(rows_per_block, 4 * WG_SCAN);
 }
 
@@ -460,8 +427,9 @@ template <typename T>
 static int launch_small_wgrad(const void *in, const void *gout, uint32_t c_in, uint32_t K,
                               uint32_t c_out, const int32_t *nbr, uint32_t n_out, float *dW,
                               void *workspace, uint64_t workspace_bytes, cudaStream_t stream) {
-  const uint32_t rows_per_block =
-      small_wgrad_rows(c_out, K, n_out, workspace_slots(workspace, workspace_bytes, c_in, c_out, K));
+  const uint32_t rows_per_block = small_wgrad_rows(
+      n_out, workspace_splits(small_wgrad_slices(c_out, K), workspace, workspace_bytes,
+                              (uint64_t)K * c_in * c_out * sizeof(float)));
   dim3 grid(cdiv(n_out, rows_per_block), cdiv(K, 8), cdiv(c_out, 32));
   float *part = grid.x > 1 ? reinterpret_cast<float *>(workspace) : dW;
   const T *x = (const T *)in, *g = (const T *)gout;
@@ -484,19 +452,9 @@ int conv_small_cin_wgrad(const void *in, const void *grad_out, int dtype, uint32
     MEB_CUDA(cudaMemsetAsync(grad_weight, 0, (size_t)K * c_in * c_out * sizeof(float), stream));
     return MEB200_OK;
   }
-  switch (dtype) {
-    case MEB200_F32:
-      return launch_small_wgrad<float>(in, grad_out, c_in, K, c_out, out_nbr, n_out, grad_weight,
-                                       workspace, workspace_bytes, stream);
-    case MEB200_BF16:
-      return launch_small_wgrad<__nv_bfloat16>(in, grad_out, c_in, K, c_out, out_nbr, n_out,
-                                               grad_weight, workspace, workspace_bytes, stream);
-    case MEB200_F16:
-      return launch_small_wgrad<__half>(in, grad_out, c_in, K, c_out, out_nbr, n_out, grad_weight,
-                                        workspace, workspace_bytes, stream);
-    default:
-      return MEB200_ERR_UNSUPPORTED;
-  }
+  MEB_DISPATCH_DTYPE(dtype, return launch_small_wgrad<T>(in, grad_out, c_in, K, c_out, out_nbr,
+                                                         n_out, grad_weight, workspace,
+                                                         workspace_bytes, stream));
 }
 
 template <typename TIn, typename TOut>
@@ -520,36 +478,29 @@ int conv_forward_simt(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in
                       cudaStream_t stream) {
   (void)n_in;
   if (n_out == 0) return MEB200_OK;
-  if (in_dtype == MEB200_F32 && out_dtype == MEB200_F32)
-    return launch_gg<float, float>(in, c_in, weight, K, c_out, trans_w, nbr, n_out, out, stream);
-  if (in_dtype == MEB200_BF16 && out_dtype == MEB200_F32)
-    return launch_gg<__nv_bfloat16, float>(in, c_in, weight, K, c_out, trans_w, nbr, n_out, out, stream);
-  if (in_dtype == MEB200_BF16 && out_dtype == MEB200_BF16)
-    return launch_gg<__nv_bfloat16, __nv_bfloat16>(in, c_in, weight, K, c_out, trans_w, nbr, n_out, out, stream);
-  if (in_dtype == MEB200_F16 && out_dtype == MEB200_F32)
-    return launch_gg<__half, float>(in, c_in, weight, K, c_out, trans_w, nbr, n_out, out, stream);
-  if (in_dtype == MEB200_F16 && out_dtype == MEB200_F16)
-    return launch_gg<__half, __half>(in, c_in, weight, K, c_out, trans_w, nbr, n_out, out, stream);
-  set_error("conv (simt): unsupported dtype combination in=%d out=%d", in_dtype, out_dtype);
-  return MEB200_ERR_UNSUPPORTED;
+  MEB_DISPATCH_DTYPE_OUT(in_dtype, out_dtype,
+                         return launch_gg<T, TO>(in, c_in, weight, K, c_out, trans_w, nbr, n_out,
+                                                 out, stream));
 }
 
-// Rows per split of k_conv_wgrad (at most max_splits splits): enough CTAs for ~4 waves, each
-// split a multiple of TK rows and at least 8 * TK.
-static uint32_t simt_wgrad_rows(uint32_t c_in, uint32_t c_out, uint32_t K, uint32_t n_out,
-                                uint64_t max_splits) {
+// Row splits k_conv_wgrad plans: enough CTAs for ~4 waves, each split at least 8 * TK rows.
+static uint32_t simt_wgrad_splits(uint32_t c_in, uint32_t c_out, uint32_t K, uint32_t n_out) {
   const uint64_t tiles = (uint64_t)cdiv(c_in, TM) * cdiv(c_out, TN);
-  uint64_t splits = std::max<uint64_t>(1, cdiv(4ull * num_sms(), (uint64_t)K * tiles));
-  splits = std::min<uint64_t>({splits, cdiv(n_out, 8 * TK), 65535, max_splits});
-  return cdiv(cdiv(n_out, (uint32_t)splits), TK) * TK;
+  const uint64_t splits = std::max<uint64_t>(1, cdiv(4ull * num_sms(), (uint64_t)K * tiles));
+  return (uint32_t)std::min<uint64_t>({splits, cdiv(n_out, 8 * TK), 65535});
+}
+
+// Rows per split for `splits` splits: a multiple of TK.
+static uint32_t simt_wgrad_rows(uint32_t n_out, uint32_t splits) {
+  return cdiv(cdiv(n_out, splits), TK) * TK;
 }
 
 uint64_t conv_wgrad_simt_workspace_bytes(uint32_t c_in, uint32_t c_out, uint32_t K,
                                          uint32_t n_out) {
   if (n_out == 0 || K == 0 || c_in == 0 || c_out == 0) return 0;
   const uint32_t rows = conv_small_cin_supported(c_in, c_out)
-                            ? small_wgrad_rows(c_out, K, n_out, UINT64_MAX)
-                            : simt_wgrad_rows(c_in, c_out, K, n_out, UINT64_MAX);
+                            ? small_wgrad_rows(n_out, small_wgrad_slices(c_out, K))
+                            : simt_wgrad_rows(n_out, simt_wgrad_splits(c_in, c_out, K, n_out));
   const uint32_t splits = cdiv(n_out, rows);
   return splits > 1 ? (uint64_t)splits * K * c_in * c_out * sizeof(float) : 0;
 }
@@ -563,26 +514,15 @@ int conv_wgrad_simt(const void *in, const void *grad_out, int dtype, uint32_t c_
   }
   const uint32_t tiles_n = cdiv(c_out, TN), tiles = cdiv(c_in, TM) * tiles_n;
   MEB_CHECK_ARG(tiles <= 65535, "too many channel tiles");
-  // a missing or small workspace leaves fewer splits (one: the CTAs store into dW directly)
   const uint32_t rows_per_split = simt_wgrad_rows(
-      c_in, c_out, K, n_out, workspace_slots(workspace, workspace_bytes, c_in, c_out, K));
+      n_out, workspace_splits(simt_wgrad_splits(c_in, c_out, K, n_out), workspace,
+                              workspace_bytes, (uint64_t)K * c_in * c_out * sizeof(float)));
   const uint32_t splits = cdiv(n_out, rows_per_split);
   float *part = splits > 1 ? reinterpret_cast<float *>(workspace) : grad_weight;
   dim3 grid(K, splits, tiles);
-  switch (dtype) {
-    case MEB200_F32:
-      k_conv_wgrad<float><<<grid, 256, 0, stream>>>((const float *)in, (const float *)grad_out, c_in, c_out, out_nbr, n_out, rows_per_split, tiles_n, part);
-      break;
-    case MEB200_BF16:
-      k_conv_wgrad<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16 *)in, (const __nv_bfloat16 *)grad_out, c_in, c_out, out_nbr, n_out, rows_per_split, tiles_n, part);
-      break;
-    case MEB200_F16:
-      k_conv_wgrad<__half><<<grid, 256, 0, stream>>>((const __half *)in, (const __half *)grad_out, c_in, c_out, out_nbr, n_out, rows_per_split, tiles_n, part);
-      break;
-    default:
-      set_error("conv wgrad (simt): unsupported dtype %d", dtype);
-      return MEB200_ERR_UNSUPPORTED;
-  }
+  MEB_DISPATCH_DTYPE(dtype, k_conv_wgrad<T><<<grid, 256, 0, stream>>>(
+                                (const T *)in, (const T *)grad_out, c_in, c_out, out_nbr, n_out,
+                                rows_per_split, tiles_n, part));
   MEB_LAUNCH_OK();
   if (splits == 1) return MEB200_OK;
   return launch_split_sum(part, grad_weight, (size_t)K * c_in * c_out, splits, stream);

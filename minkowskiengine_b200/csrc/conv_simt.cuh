@@ -10,14 +10,9 @@ int conv_forward_simt(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in
                       const int32_t *nbr, uint32_t n_out, void *out, int out_dtype,
                       cudaStream_t stream);
 
-// Weight gradients store each row split's partial sums into a slot of `workspace` and add the
-// slots in split order (no atomics: bit-identical run to run).  A missing or small workspace
-// means fewer splits, down to one.  The size below fits every split the plan wants, for the
-// kernel conv_small_cin_supported() selects.
-// dW[i] = part[i] + part[n + i] + ... + part[(splits - 1) n + i], in split order (k_split_sum):
-// the fixed-order fold of the row splits' slots of every weight gradient.
-int launch_split_sum(const float *part, float *dW, size_t n, uint32_t splits, cudaStream_t stream);
-
+// Weight gradients reduce over row splits (workspace_splits / launch_split_sum in common.cuh).
+// The size below fits every split the plan wants, for the kernel conv_small_cin_supported()
+// selects.
 uint64_t conv_wgrad_simt_workspace_bytes(uint32_t c_in, uint32_t c_out, uint32_t K,
                                          uint32_t n_out);
 int conv_wgrad_simt(const void *in, const void *grad_out, int dtype, uint32_t c_in,

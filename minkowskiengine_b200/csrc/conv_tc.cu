@@ -175,7 +175,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
 //         In[i][ci] * dOut[o][co]
 // GEMM view: D[M = ci][N = co] over the reduction axis "pair"; a stage = 64 pairs.  One CTA owns
 // (offset k, 128 input channels, a share of the pairs).  With one share per offset it stores its
-// sums into dW; otherwise share s stores into partial[s] and k_wgrad_sum adds the shares in
+// sums into dW; otherwise share s stores into partial[s] and launch_split_sum adds the shares in
 // order, so the result does not depend on the order in which CTAs finish.  The pairs come from
 //   pair mode   : the compacted lists of meb200_kernel_map_pairs (segments (row chunk, offset),
 //                 padded with -1); the CTA takes the same fraction of every chunk's segment
@@ -333,19 +333,6 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_wg(const WgParams p) {
   }
 }
 
-
-// dW = partial[0] + partial[1] + ... (fixed order), four floats per thread
-__global__ void __launch_bounds__(256)
-k_wgrad_sum(const float4 *__restrict__ partial, float4 *__restrict__ dW, size_t n4, uint32_t splits) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
-    float4 a = partial[i];
-    for (uint32_t sp = 1; sp < splits; ++sp) {
-      const float4 b = partial[sp * n4 + i];
-      a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
-    }
-    dW[i] = a;
-  }
-}
 
 // ---- weight packing ----------------------------------------------------------------------------
 // Per-optimizer-step weight packing: fp32 master W[k][ci][co] -> feature dtype in the two
@@ -508,25 +495,15 @@ static int run_wgrad(int dtype, WgParams p, uint32_t K_grid, uint32_t est_stages
                      uint64_t workspace_bytes, cudaStream_t stream) {
   const uint32_t m_tiles = cdiv(p.c_in, tc::kWgChannels);
   const size_t dw_elems = (size_t)K_grid * p.c_in * p.c_out;
-  // a workspace that is missing, too small or not 16-byte aligned leaves fewer splits (or one)
-  const bool usable = workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0;
-  const uint64_t fit = usable ? workspace_bytes / (dw_elems * sizeof(float)) : 0;
-  p.n_splits = wgrad_planned_splits(p.c_in, K_grid, est_stages);
-  if (p.n_splits > fit) p.n_splits = fit > 1 ? (uint32_t)fit : 1u;
+  p.n_splits = workspace_splits(wgrad_planned_splits(p.c_in, K_grid, est_stages), workspace,
+                                workspace_bytes, dw_elems * sizeof(float));
   p.partial = p.n_splits > 1 ? reinterpret_cast<float *>(workspace) : nullptr;
   const dim3 grid(p.n_splits, m_tiles, K_grid);
   const int rc = dtype == MEB200_BF16 ? dispatch_wgrad<__nv_bfloat16>(p, grid, stream)
                                       : dispatch_wgrad<__half>(p, grid, stream);
   if (rc != MEB200_OK || p.n_splits == 1) return rc;
-  const size_t n4 = dw_elems / 4;       // c_out is a multiple of 16
-  const unsigned blocks = (unsigned)(n4 / 256 + 1 < 4096 ? n4 / 256 + 1 : 4096);
-  k_wgrad_sum<<<blocks, 256, 0, stream>>>(reinterpret_cast<const float4 *>(p.partial),
-                                          reinterpret_cast<float4 *>(p.dW), n4, p.n_splits);
-  MEB_LAUNCH_OK();
-  return MEB200_OK;
+  return launch_split_sum(p.partial, p.dW, dw_elems, p.n_splits, stream);
 }
-
-static bool aligned16(const void *a) { return (reinterpret_cast<uintptr_t>(a) & 15) == 0; }
 
 // ---- forward / dgrad ----------------------------------------------------------------------------
 bool conv_tc_supported(int dtype, uint32_t c_reduce, uint32_t c_cols) {
@@ -540,7 +517,7 @@ int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, c
                     int out_dtype, cudaStream_t stream) {
   if (n_rows == 0) return MEB200_OK;
   MEB_CHECK_ARG(conv_tc_supported(dtype, c_reduce, c_cols), "shape not supported by tc path");
-  if (!aligned16(A) || !aligned16(B)) {
+  if (!aligned(16, A, B)) {
     set_error("conv tc: operands must be 16-byte aligned");
     return MEB200_ERR_UNSUPPORTED;
   }
@@ -574,7 +551,7 @@ int conv_stem_forward_tc(const void *A4, int dtype, uint32_t K, const void *Wv, 
                          cudaStream_t stream) {
   if (n_rows == 0) return MEB200_OK;
   MEB_CHECK_ARG(conv_stem_tc_supported(dtype, K, c_cols), "stem forward: K=%u c_out=%u", K, c_cols);
-  if ((reinterpret_cast<uintptr_t>(A4) & 7) != 0 || !aligned16(Wv)) {
+  if (!aligned(8, A4) || !aligned(16, Wv)) {
     set_error("stem forward: operands must be 8 / 16-byte aligned");
     return MEB200_ERR_UNSUPPORTED;
   }
@@ -600,7 +577,7 @@ int conv_stem_wgrad_tc(const void *in4, const void *grad_out, int dtype, uint32_
     MEB_CUDA(cudaMemsetAsync(dWv, 0, (size_t)V * c_out * sizeof(float), stream));
     return MEB200_OK;
   }
-  if ((reinterpret_cast<uintptr_t>(in4) & 7) != 0 || !aligned16(grad_out)) {
+  if (!aligned(8, in4) || !aligned(16, grad_out)) {
     set_error("stem wgrad: operands must be 8 / 16-byte aligned");
     return MEB200_ERR_UNSUPPORTED;
   }
@@ -620,7 +597,7 @@ bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out) {
 int conv_wgrad_tc(const void *in, const void *grad_out, int dtype, uint32_t c_in, uint32_t K,
                   uint32_t c_out, const int32_t *out_nbr, uint32_t n_out, float *grad_weight,
                   void *workspace, uint64_t workspace_bytes, cudaStream_t stream) {
-  if (!conv_wgrad_tc_supported(dtype, c_in, c_out) || !aligned16(in) || !aligned16(grad_out)) {
+  if (!conv_wgrad_tc_supported(dtype, c_in, c_out) || !aligned(16, in, grad_out)) {
     set_error("wgrad tc: shape or alignment outside the tensor-core path (c_in=%u c_out=%u)",
               c_in, c_out);
     return MEB200_ERR_UNSUPPORTED;
@@ -645,7 +622,7 @@ int conv_wgrad_pairs(const void *in, const void *grad_out, int dtype, uint32_t c
                      const int32_t *seg_start, uint32_t n_chunks, uint32_t n_out,
                      float *grad_weight, void *workspace, uint64_t workspace_bytes,
                      cudaStream_t stream) {
-  if (!conv_wgrad_uses_pairs(dtype, c_in, c_out, K) || !aligned16(in) || !aligned16(grad_out)) {
+  if (!conv_wgrad_uses_pairs(dtype, c_in, c_out, K) || !aligned(16, in, grad_out)) {
     set_error("wgrad pairs: shape or alignment outside the tensor-core path (c_in=%u c_out=%u K=%u)",
               c_in, c_out, K);
     return MEB200_ERR_UNSUPPORTED;

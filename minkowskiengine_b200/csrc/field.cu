@@ -239,8 +239,6 @@ k_interp_fwd(const T *__restrict__ F, uint32_t C, const int32_t *__restrict__ ro
 }
 
 // ---- host dispatch ------------------------------------------------------------------------------
-static bool aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
-
 template <typename T, int V>
 static void reduce_launch(const void *src, uint32_t C, const int32_t *perm, const int32_t *start,
                           uint32_t M, const float *weight, uint32_t src_div, int mode, void *out,
@@ -285,29 +283,6 @@ static void interp_launch(const void *F, uint32_t C, const int32_t *rows, const 
                                                                        K, (T *)out);
 }
 
-template <typename T>
-static void reduce_t(bool vec, const void *src, uint32_t C, const int32_t *perm,
-                     const int32_t *start, uint32_t M, const float *weight, uint32_t src_div,
-                     int mode, void *out, int32_t *argmax, cudaStream_t st) {
-  if (vec) reduce_launch<T, 16 / sizeof(T)>(src, C, perm, start, M, weight, src_div, mode, out, argmax, st);
-  else reduce_launch<T, 1>(src, C, perm, start, M, weight, src_div, mode, out, argmax, st);
-}
-
-template <typename T>
-static void expand_t(bool vec, const void *g, uint32_t M, uint32_t C, const int64_t *inv,
-                     uint32_t n, int mode, const int32_t *start, const int32_t *argmax,
-                     const int64_t *uidx, void *out, cudaStream_t st) {
-  if (vec) expand_launch<T, 16 / sizeof(T)>(g, M, C, inv, n, mode, start, argmax, uidx, out, st);
-  else expand_launch<T, 1>(g, M, C, inv, n, mode, start, argmax, uidx, out, st);
-}
-
-template <typename T>
-static void interp_t(bool vec, const void *F, uint32_t C, const int32_t *rows, const float *w,
-                     uint32_t n, uint32_t K, void *out, cudaStream_t st) {
-  if (vec) interp_launch<T, 16 / sizeof(T)>(F, C, rows, w, n, K, out, st);
-  else interp_launch<T, 1>(F, C, rows, w, n, K, out, st);
-}
-
 static int load_strides(const int32_t *tensor_stride, uint32_t ncols, IntVec *ts) {
   MEB_CHECK_ARG(ncols >= 2 && ncols <= MEB200_MAX_NCOLS, "ncols=%u", ncols);
   MEB_CHECK_ARG(tensor_stride != nullptr, "null tensor stride");
@@ -323,14 +298,6 @@ static int load_strides(const int32_t *tensor_stride, uint32_t ncols, IntVec *ts
 }  // namespace meb200
 
 using namespace meb200;
-
-#define MEB_DISPATCH_DTYPE(dtype, FN, ...)                                                         \
-  switch (dtype) {                                                                                 \
-    case MEB200_F32: FN<float>(__VA_ARGS__); break;                                                \
-    case MEB200_BF16: FN<__nv_bfloat16>(__VA_ARGS__); break;                                       \
-    case MEB200_F16: FN<__half>(__VA_ARGS__); break;                                               \
-    default: set_error("unsupported dtype %d", dtype); return MEB200_ERR_UNSUPPORTED;              \
-  }
 
 extern "C" {
 
@@ -421,9 +388,9 @@ int meb200_field_reduce(const void *src, int dtype, uint32_t n_src, uint32_t C, 
   MEB_CHECK_ARG(mode != MEB200_FIELD_MAX || argmax != nullptr, "MAX needs argmax");
   MEB_CHECK_ARG(weight == nullptr || mode == MEB200_FIELD_SUM, "weights are for SUM only");
   cudaStream_t s = (cudaStream_t)stream;
-  bool vec = (size_t)C * dtype_size(dtype) % 16 == 0 && aligned16(src) && aligned16(out);
-  MEB_DISPATCH_DTYPE(dtype, reduce_t, vec, src, C, perm, start, M, weight, src_div, mode, out,
-                     argmax, s);
+  MEB_DISPATCH_DTYPE(dtype, MEB_DISPATCH_VEC(T, C, aligned(16, src, out),
+                                             reduce_launch<T, V>(src, C, perm, start, M, weight,
+                                                                 src_div, mode, out, argmax, s)));
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
@@ -437,9 +404,9 @@ int meb200_field_expand(const void *g, int dtype, uint32_t M, uint32_t C, const 
                     (mode == MEB200_FIELD_SUBSAMPLE && unique_index),
                 "mode %d without its table", mode);
   cudaStream_t s = (cudaStream_t)stream;
-  bool vec = (size_t)C * dtype_size(dtype) % 16 == 0 && aligned16(g) && aligned16(out);
-  MEB_DISPATCH_DTYPE(dtype, expand_t, vec, g, M, C, inv, n, mode, start, argmax, unique_index, out,
-                     s);
+  MEB_DISPATCH_DTYPE(dtype, MEB_DISPATCH_VEC(T, C, aligned(16, g, out),
+                                             expand_launch<T, V>(g, M, C, inv, n, mode, start,
+                                                                 argmax, unique_index, out, s)));
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
@@ -467,8 +434,8 @@ int meb200_interp_forward(const void *F, int dtype, uint32_t M, uint32_t C, cons
   if (n == 0 || C == 0) return MEB200_OK;
   MEB_CHECK_ARG(rows && weights && out && (F || M == 0), "null buffer");
   cudaStream_t s = (cudaStream_t)stream;
-  bool vec = (size_t)C * dtype_size(dtype) % 16 == 0 && aligned16(F) && aligned16(out);
-  MEB_DISPATCH_DTYPE(dtype, interp_t, vec, F, C, rows, weights, n, K, out, s);
+  MEB_DISPATCH_DTYPE(dtype, MEB_DISPATCH_VEC(T, C, aligned(16, F, out),
+                                             interp_launch<T, V>(F, C, rows, weights, n, K, out, s)));
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }

@@ -329,7 +329,6 @@ k_broadcast_fma(const T *__restrict__ x, const T *__restrict__ z, const float *_
 }
 
 // ---- host dispatch ---------------------------------------------------------------------------
-static bool aligned(const void *p, size_t bytes) { return ((uintptr_t)p % bytes) == 0; }  // NULL: yes
 static uint32_t group_tiles(uint32_t n) { return (n + kGroupTile - 1) / kGroupTile; }
 
 template <typename T, int V, int MODE>
@@ -353,7 +352,7 @@ static int seg_reduce_t(const void *a, const void *b, uint32_t C, const int32_t 
                         const int32_t *seg_start, const int32_t *tile_start, uint32_t B,
                         uint32_t max_tiles, int mode, float *part, int32_t *part_row,
                         cudaStream_t st) {
-  bool v4 = C % 4 == 0 && aligned(a, 4 * sizeof(T)) && aligned(b, 4 * sizeof(T));
+  bool v4 = C % 4 == 0 && aligned(4 * sizeof(T), a, b);
 #define MEB_SEG(MODE)                                                                           \
   if (v4) seg_reduce_launch<T, 4, MODE>(a, b, C, order, seg_start, tile_start, B, max_tiles, part, \
                                         part_row, st);                                          \
@@ -369,10 +368,11 @@ static int seg_reduce_t(const void *a, const void *b, uint32_t C, const int32_t 
   return MEB200_OK;
 }
 
+// The broadcasts take 4 channels per thread in every dtype (8-byte accesses in bf16 / fp16).
 template <typename T, typename TO, int V>
-static void bcast_launch(const void *x, const float *g, const int32_t *argmax,
-                         const int32_t *row_seg, uint32_t n, uint32_t C, int op, void *out,
-                         cudaStream_t st) {
+static int bcast_launch(const void *x, const float *g, const int32_t *argmax,
+                        const int32_t *row_seg, uint32_t n, uint32_t C, int op, void *out,
+                        cudaStream_t st) {
   unsigned blocks = cdiv((uint64_t)n * (C / V), 256);
   switch (op) {
     case MEB200_BCAST_ADD:
@@ -387,14 +387,15 @@ static void bcast_launch(const void *x, const float *g, const int32_t *argmax,
     default:
       k_broadcast<T, TO, V, MEB200_BCAST_MAXGRAD><<<blocks, 256, 0, st>>>((const T *)x, g, argmax, row_seg, n, C, (TO *)out);
   }
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
 }
 
-template <typename T, typename TO>
-static int bcast_t(const void *x, const float *g, const int32_t *argmax, const int32_t *row_seg,
-                   uint32_t n, uint32_t C, int op, void *out, cudaStream_t st) {
-  if (C % 4 == 0 && aligned(x, 4 * sizeof(T)) && aligned(g, 16) && aligned(out, 4 * sizeof(TO)))
-    bcast_launch<T, TO, 4>(x, g, argmax, row_seg, n, C, op, out, st);
-  else bcast_launch<T, TO, 1>(x, g, argmax, row_seg, n, C, op, out, st);
+template <typename T, int V>
+static int fma_launch(const void *x, const void *z, const float *g, const float *h, const float *k,
+                      const int32_t *row_seg, uint32_t n, uint32_t C, void *out, cudaStream_t st) {
+  k_broadcast_fma<T, V><<<cdiv((uint64_t)n * (C / V), 256), 256, 0, st>>>(
+      (const T *)x, (const T *)z, g, h, k, row_seg, n, C, (T *)out);
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
@@ -412,26 +413,10 @@ int meb200_broadcast_fma(const void *x, const void *z, int dtype, const float *g
   MEB_CHECK_ARG(x && g && row_seg && out, "null buffer");
   MEB_CHECK_ARG((z == nullptr) == (h == nullptr), "z and h go together");
   cudaStream_t s = (cudaStream_t)stream;
-#define MEB_FMA(T)                                                                              \
-  {                                                                                             \
-    size_t vb = 4 * sizeof(T);                                                                  \
-    if (C % 4 == 0 && aligned(x, vb) && aligned(z, vb) && aligned(out, vb))                     \
-      k_broadcast_fma<T, 4><<<cdiv((uint64_t)n * (C / 4), 256), 256, 0, s>>>(                   \
-          (const T *)x, (const T *)z, g, h, k, row_seg, n, C, (T *)out);                        \
-    else                                                                                        \
-      k_broadcast_fma<T, 1><<<cdiv((uint64_t)n * C, 256), 256, 0, s>>>(                          \
-          (const T *)x, (const T *)z, g, h, k, row_seg, n, C, (T *)out);                        \
-    MEB_LAUNCH_OK();                                                                            \
-    return MEB200_OK;                                                                           \
-  }
-  switch (dtype) {
-    case MEB200_F32: MEB_FMA(float)
-    case MEB200_BF16: MEB_FMA(__nv_bfloat16)
-    case MEB200_F16: MEB_FMA(__half)
-  }
-#undef MEB_FMA
-  set_error("broadcast_fma: unsupported dtype %d", dtype);
-  return MEB200_ERR_UNSUPPORTED;
+  MEB_DISPATCH_DTYPE(dtype,
+    if (C % 4 == 0 && aligned(4 * sizeof(T), x, z, out))
+      return fma_launch<T, 4>(x, z, g, h, k, row_seg, n, C, out, s);
+    return fma_launch<T, 1>(x, z, g, h, k, row_seg, n, C, out, s));
 }
 
 uint64_t meb200_origin_group_scratch_bytes(uint32_t n, uint32_t B) {
@@ -499,14 +484,8 @@ int meb200_segment_reduce(const void *a, const void *b, int dtype, uint32_t n, u
   int32_t *part_row = (int32_t *)(part + (size_t)max_tiles * C);
   int rc = MEB200_OK;
   if (n > 0) {
-    switch (dtype) {
-      case MEB200_F32: rc = seg_reduce_t<float>(a, b, C, order, seg_start, tile_start, B, max_tiles, mode, part, part_row, s); break;
-      case MEB200_BF16: rc = seg_reduce_t<__nv_bfloat16>(a, b, C, order, seg_start, tile_start, B, max_tiles, mode, part, part_row, s); break;
-      case MEB200_F16: rc = seg_reduce_t<__half>(a, b, C, order, seg_start, tile_start, B, max_tiles, mode, part, part_row, s); break;
-      default:
-        set_error("segment reduction: unsupported dtype %d", dtype);
-        return MEB200_ERR_UNSUPPORTED;
-    }
+    MEB_DISPATCH_DTYPE(dtype, rc = seg_reduce_t<T>(a, b, C, order, seg_start, tile_start, B,
+                                                   max_tiles, mode, part, part_row, s));
     if (rc != MEB200_OK) return rc;
   }
   unsigned blocks = cdiv((uint64_t)B * C, 256);
@@ -531,18 +510,10 @@ int meb200_broadcast(const void *x, int dtype, const float *g, const int32_t *ar
   MEB_CHECK_ARG(out_dtype == dtype || out_dtype == MEB200_F32,
                 "out_dtype %d must be the feature dtype %d or F32", out_dtype, dtype);
   cudaStream_t s = (cudaStream_t)stream;
-  bool f32 = out_dtype == MEB200_F32;
-  switch (dtype) {
-    case MEB200_F32: return bcast_t<float, float>(x, g, argmax, row_seg, n, C, op, out, s);
-    case MEB200_BF16:
-      return f32 ? bcast_t<__nv_bfloat16, float>(x, g, argmax, row_seg, n, C, op, out, s)
-                 : bcast_t<__nv_bfloat16, __nv_bfloat16>(x, g, argmax, row_seg, n, C, op, out, s);
-    case MEB200_F16:
-      return f32 ? bcast_t<__half, float>(x, g, argmax, row_seg, n, C, op, out, s)
-                 : bcast_t<__half, __half>(x, g, argmax, row_seg, n, C, op, out, s);
-  }
-  set_error("broadcast: unsupported dtype %d", dtype);
-  return MEB200_ERR_UNSUPPORTED;
+  MEB_DISPATCH_DTYPE_OUT(dtype, out_dtype,
+    if (C % 4 == 0 && aligned(4 * sizeof(T), x) && aligned(16, g) && aligned(4 * sizeof(TO), out))
+      return bcast_launch<T, TO, 4>(x, g, argmax, row_seg, n, C, op, out, s);
+    return bcast_launch<T, TO, 1>(x, g, argmax, row_seg, n, C, op, out, s));
 }
 
 }

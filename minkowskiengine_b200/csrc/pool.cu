@@ -168,13 +168,7 @@ int meb200_pool_forward(const void *in, int dtype, uint32_t n_in, uint32_t C,
   MEB_CHECK_ARG((uint64_t)n_in * C < 0x7FFFFFFFull || mode != MEB200_POOL_MAX,
                 "max_index is int32: n_in*C too large");
   cudaStream_t s = (cudaStream_t)stream;
-  switch (dtype) {
-    case MEB200_F32: return pool_fwd_t<float>(in, C, out_nbr, K, n_out, mode, out, aux, s);
-    case MEB200_BF16: return pool_fwd_t<__nv_bfloat16>(in, C, out_nbr, K, n_out, mode, out, aux, s);
-    case MEB200_F16: return pool_fwd_t<__half>(in, C, out_nbr, K, n_out, mode, out, aux, s);
-  }
-  set_error("pooling: unsupported dtype %d", dtype);
-  return MEB200_ERR_UNSUPPORTED;
+  MEB_DISPATCH_DTYPE(dtype, return pool_fwd_t<T>(in, C, out_nbr, K, n_out, mode, out, aux, s));
 }
 
 int meb200_pool_backward(const void *grad_out, int dtype, uint32_t n_in, uint32_t C,
@@ -187,13 +181,8 @@ int meb200_pool_backward(const void *grad_out, int dtype, uint32_t n_in, uint32_
   MEB_CHECK_ARG((uint64_t)n_in * C < 0x7FFFFFFFull || mode != MEB200_POOL_MAX,
                 "max_index is int32: n_in*C too large");
   cudaStream_t s = (cudaStream_t)stream;
-  switch (dtype) {
-    case MEB200_F32: return pool_bwd_t<float>(grad_out, n_in, C, in_nbr, K, n_out, mode, aux, grad_in, s);
-    case MEB200_BF16: return pool_bwd_t<__nv_bfloat16>(grad_out, n_in, C, in_nbr, K, n_out, mode, aux, grad_in, s);
-    case MEB200_F16: return pool_bwd_t<__half>(grad_out, n_in, C, in_nbr, K, n_out, mode, aux, grad_in, s);
-  }
-  set_error("pooling: unsupported dtype %d", dtype);
-  return MEB200_ERR_UNSUPPORTED;
+  MEB_DISPATCH_DTYPE(dtype, return pool_bwd_t<T>(grad_out, n_in, C, in_nbr, K, n_out, mode, aux,
+                                                  grad_in, s));
 }
 
 }

@@ -130,8 +130,6 @@ k_union_fold_bwd(const T *const *__restrict__ inputs, uint32_t N, const int32_t 
 }
 
 // ---- host dispatch ---------------------------------------------------------------------------
-static bool aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
-
 template <typename T, int V>
 static void fold_launch(const void *const *inputs, uint32_t N, const int32_t *src, uint32_t M,
                         uint32_t C, int op, void *out, cudaStream_t st) {
@@ -167,29 +165,6 @@ static void fold_bwd_launch(const void *const *inputs, uint32_t N, const int32_t
 
 using namespace meb200;
 
-#define MEB_DISPATCH_DTYPE(dtype, FN, ...)                                                         \
-  switch (dtype) {                                                                                 \
-    case MEB200_F32: FN<float>(__VA_ARGS__); break;                                                \
-    case MEB200_BF16: FN<__nv_bfloat16>(__VA_ARGS__); break;                                       \
-    case MEB200_F16: FN<__half>(__VA_ARGS__); break;                                               \
-    default: set_error("unsupported dtype %d", dtype); return MEB200_ERR_UNSUPPORTED;              \
-  }
-
-template <typename T>
-static void fold_t(bool vec, const void *const *inputs, uint32_t N, const int32_t *src, uint32_t M,
-                   uint32_t C, int op, void *out, cudaStream_t st) {
-  if (vec) fold_launch<T, 16 / sizeof(T)>(inputs, N, src, M, C, op, out, st);
-  else fold_launch<T, 1>(inputs, N, src, M, C, op, out, st);
-}
-
-template <typename T>
-static void fold_bwd_t(bool vec, const void *const *inputs, uint32_t N, const int32_t *src,
-                       uint32_t M, uint32_t C, int op, const void *g, uint32_t i, const int64_t *u_i,
-                       uint32_t n_i, void *grad, cudaStream_t st) {
-  if (vec) fold_bwd_launch<T, 16 / sizeof(T)>(inputs, N, src, M, C, op, g, i, u_i, n_i, grad, st);
-  else fold_bwd_launch<T, 1>(inputs, N, src, M, C, op, g, i, u_i, n_i, grad, st);
-}
-
 extern "C" {
 
 int meb200_gather_rows(const void *src, int dtype, uint32_t n_src, uint32_t C, const int64_t *idx,
@@ -200,7 +175,7 @@ int meb200_gather_rows(const void *src, int dtype, uint32_t n_src, uint32_t C, c
   MEB_CHECK_ARG(idx && out && (src || n_src == 0), "null buffer");
   cudaStream_t s = (cudaStream_t)stream;
   size_t row = (size_t)C * dtype_size(dtype);
-  if (row % 16 == 0 && aligned16(src) && aligned16(out)) {
+  if (row % 16 == 0 && aligned(16, src, out)) {
     uint32_t CW = (uint32_t)(row / 16);
     k_gather_rows<uint4><<<cdiv((uint64_t)n_out * CW, 256), 256, 0, s>>>(
         (const uint4 *)src, n_src, CW, idx, n_out, (uint4 *)out);
@@ -222,8 +197,8 @@ int meb200_union_fold_forward(const void *const *inputs, uint32_t N, uint32_t in
   MEB_CHECK_ARG(op >= MEB200_UNION_ADD && op <= MEB200_UNION_DIV, "op %d is not a fold", op);
   MEB_CHECK_ARG(N >= 1 && inputs && src && out, "null buffer");
   cudaStream_t s = (cudaStream_t)stream;
-  bool vec = (size_t)C * dtype_size(dtype) % 16 == 0 && inputs_align % 16 == 0 && aligned16(out);
-  MEB_DISPATCH_DTYPE(dtype, fold_t, vec, inputs, N, src, M, C, op, out, s);
+  MEB_DISPATCH_DTYPE(dtype, MEB_DISPATCH_VEC(T, C, inputs_align % 16 == 0 && aligned(16, out),
+                                             fold_launch<T, V>(inputs, N, src, M, C, op, out, s)));
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
@@ -237,10 +212,10 @@ int meb200_union_fold_backward(const void *const *inputs, uint32_t N, uint32_t i
   MEB_CHECK_ARG(i < N, "input %u of %u", i, N);
   MEB_CHECK_ARG(inputs && src && grad_out && u_i && grad_i, "null buffer");
   cudaStream_t s = (cudaStream_t)stream;
-  bool vec = (size_t)C * dtype_size(dtype) % 16 == 0 && inputs_align % 16 == 0 &&
-             aligned16(grad_out) && aligned16(grad_i);
-  MEB_DISPATCH_DTYPE(dtype, fold_bwd_t, vec, inputs, N, src, M, C, op, grad_out, i, u_i, n_i,
-                     grad_i, s);
+  MEB_DISPATCH_DTYPE(dtype,
+                     MEB_DISPATCH_VEC(T, C, inputs_align % 16 == 0 && aligned(16, grad_out, grad_i),
+                                      fold_bwd_launch<T, V>(inputs, N, src, M, C, op, grad_out, i,
+                                                            u_i, n_i, grad_i, s)));
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
