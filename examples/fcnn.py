@@ -12,6 +12,10 @@ the compiled reference (`oracle/_ref`, CPU):
 A point MLP on the TensorField, `.sparse()`, four convolution + max-pool levels, the pooled maps of
 all four levels sliced back onto the points and concatenated, a second `.sparse()` of that
 concatenation, three strided convolutions, global max and average pooling and an MLP head.
+
+`splat=True` builds MinkowskiSplatFCNN of the same example: `x.splat()` in place of the first
+`.sparse()`, and the four pooled levels brought back to the points with `interpolate` in place of
+`slice`.  The parameters are the same.
 """
 import torch.nn as nn
 
@@ -19,9 +23,9 @@ CHANNELS = (32, 48, 64, 96, 128)
 
 
 def fcnn(ME, in_channel, out_channel, embedding_channel=1024, channels=CHANNELS, hidden=512,
-         dropout=0.5, D=3):
-    """MinkowskiFCNN; `hidden` is the width of the head's MLP (the reference's 512), `dropout` the
-    probability of its dropout (the reference's 0.5)."""
+         dropout=0.5, D=3, splat=False):
+    """MinkowskiFCNN (MinkowskiSplatFCNN with `splat=True`); `hidden` is the width of the head's
+    MLP (the reference's 512), `dropout` the probability of its dropout (the reference's 0.5)."""
 
     def mlp(c_in, c_out):
         return nn.Sequential(ME.MinkowskiLinear(c_in, c_out, bias=False),
@@ -64,12 +68,15 @@ def fcnn(ME, in_channel, out_channel, embedding_channel=1024, channels=CHANNELS,
 
         def forward(self, x):
             x = self.mlp1(x)
-            y = x.sparse()
+            y = x.splat() if splat else x.sparse()
             ys = []
             for layer in (self.conv1, self.conv2, self.conv3, self.conv4):
                 y = self.pool(layer(y))
                 ys.append(y)
-            x = ME.cat(*[yi.slice(x) for yi in ys])
+            if splat:
+                x = ME.cat(*[yi.interpolate(x) for yi in ys])
+            else:
+                x = ME.cat(*[yi.slice(x) for yi in ys])
             y = self.conv5(x.sparse())
             return self.final(ME.cat(self.global_max_pool(y), self.global_avg_pool(y)))
 

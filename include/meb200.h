@@ -441,6 +441,13 @@ int meb200_field_expand(const void *g, int dtype, uint32_t M, uint32_t C, const 
 int meb200_interp_map(const float *query, uint32_t n, uint32_t ncols, const int32_t *tensor_stride,
                       const int32_t *map_coords, const uint32_t *table, uint32_t capacity,
                       int32_t *rows, float *weights, void *stream);
+/* Splat corners of n field points (float32 [n, ncols]) in one launch: out (int32 [n * 2^D, ncols],
+ * point-major) row q * 2^D + k = floorf of every column of point q (the batch column included)
+ * plus 1 on axis j when bit ncols-1-j of k is set (the corner order of meb200_interp_map).
+ * *d_bad (DEVICE uint32 status word, cleared by the call) gets bit 0 when a coordinate is not
+ * finite or a corner falls outside int32, and bit 1 when a batch value is not an integer. */
+int meb200_splat_coords(const float *field, uint32_t n, uint32_t ncols, int32_t *out,
+                        uint32_t *d_bad, void *stream);
 /* out[q, :] = sum_k weights[q, k] * F[rows[q, k], :] over the present corners in ascending k
  * (fp32, one rounding).  F: [M, C], out: [n, C] in `dtype`; K = 2^D. */
 int meb200_interp_forward(const void *F, int dtype, uint32_t M, uint32_t C, const int32_t *rows,

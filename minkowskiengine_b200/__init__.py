@@ -6,10 +6,12 @@ hot path of NVIDIA/MinkowskiEngine, behind the reference's own Python API.
     y = ME.MinkowskiConvolution(64, 128, kernel_size=3, stride=2, dimension=3).cuda()(x)
 
 Scope (SURVEY.md §8): SparseTensor / CoordinateManager / kernel maps, MinkowskiConvolution,
-MinkowskiConvolutionTranspose, MinkowskiChannelwiseConvolution (depthwise), local and global pooling, broadcast, batch and instance
+MinkowskiConvolutionTranspose, MinkowskiChannelwiseConvolution (depthwise), local pooling and
+unpooling (MinkowskiPoolingTranspose), global pooling, broadcast, batch and instance
 normalisation, pruning, union and arithmetic between sparse tensors on different coordinate maps,
-TensorField (point features quantised to voxels, sliced back and interpolated), and the thin torch
-wrappers MinkUNet, the ResNet classifiers and generative networks need.
+TensorField (point features quantised to voxels or splatted onto their corners, sliced back and
+interpolated), and the thin torch wrappers (cat / sum / mean / var, the stack containers,
+MinkowskiToFeature) that MinkUNet, the ResNet classifiers and generative networks need.
 CUDA tensors only; all device work runs in csrc/libmeb200.so (include/meb200.h).
 """
 __version__ = "0.1.0"
@@ -35,15 +37,18 @@ from .channelwise_convolution import (MinkowskiChannelwiseConvolution,
                                       MinkowskiChannelwiseConvolutionFunction)
 from .pooling import (MinkowskiAvgPooling, MinkowskiGlobalAvgPooling, MinkowskiGlobalMaxPooling,
                       MinkowskiGlobalPooling, MinkowskiGlobalPoolingFunction,
-                      MinkowskiGlobalSumPooling, MinkowskiLocalPoolingFunction, MinkowskiMaxPooling,
-                      MinkowskiSumPooling)
+                      MinkowskiGlobalSumPooling, MinkowskiLocalPoolingFunction,
+                      MinkowskiLocalPoolingTransposeFunction, MinkowskiMaxPooling,
+                      MinkowskiPoolingTranspose, MinkowskiSumPooling)
 from .broadcast import (MinkowskiBroadcast, MinkowskiBroadcastAddition,
                         MinkowskiBroadcastConcatenation, MinkowskiBroadcastFunction,
                         MinkowskiBroadcastMultiplication)
 from .normalization import (MinkowskiBatchNorm, MinkowskiInstanceNorm,
                             MinkowskiInstanceNormFunction, MinkowskiSyncBatchNorm, fused_bn_relu)
 from .nonlinearity import *  # noqa: F401,F403
-from .ops import MinkowskiLinear, MinkowskiToSparseTensor, cat
+from .ops import (MinkowskiLinear, MinkowskiStackCat, MinkowskiStackMean, MinkowskiStackSum,
+                  MinkowskiStackVar, MinkowskiToFeature, MinkowskiToSparseTensor, cat, mean, var)
+from .ops import sum  # noqa: A004 -- ME.sum, the reference's name
 from .tensor_field import TensorField
 from .interpolation import MinkowskiInterpolation, MinkowskiInterpolationFunction
 from .pruning import MinkowskiPruning, MinkowskiPruningFunction

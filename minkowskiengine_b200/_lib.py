@@ -88,6 +88,7 @@ PROTOTYPES = {
     "meb200_field_expand": (_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "meb200_interp_map": (_i32, [_vp, _u32, _u32, C.POINTER(C.c_int32), _vp, _vp, _u32, _vp, _vp,
                                  _vp]),
+    "meb200_splat_coords": (_i32, [_vp, _u32, _u32, _vp, _vp, _vp]),
     "meb200_interp_forward": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _vp]),
     "meb200_bn_workspace_bytes": (_u64, []),
     "meb200_bn_forward_train": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _vp, _i32, C.c_float,

@@ -983,6 +983,26 @@ class CoordinateMapManagerGPU_c10:
             _lib.ptr(cmap.table), cmap.capacity, _lib.ptr(rows), _lib.ptr(w), _lib.current_stream()))
         return rows, w
 
+    def splat_insert_and_map(self, field_key):
+        """reference: TensorField.splat (MinkowskiTensorField.py:53-73, 381-406).  The 2^D corners
+        floor(x) + {0,1}^D of every point (meb200_splat_coords; the batch column floored, never
+        offset), inserted point-major at tensor stride 1 as insert_and_map inserts, so rows are
+        numbered by first occurrence and a corner of weight 0 is a voxel too -> map key."""
+        _, field = self._field(field_key)
+        n, ncols = field.shape
+        dev = field.device
+        corners = torch.empty((n << (ncols - 1), ncols), dtype=torch.int32, device=dev)
+        bad = torch.empty(1, dtype=torch.int32, device=dev)
+        _lib.check(_lib.load().meb200_splat_coords(_lib.ptr(field), n, ncols, _lib.ptr(corners),
+                                                   _lib.ptr(bad), _lib.current_stream()))
+        status = int(bad.item())
+        if status & 1:
+            raise ValueError("TensorField coordinates must be finite and quantise to int32 voxels")
+        if status & 2:
+            raise ValueError("splat needs integer batch indices in the first coordinate column")
+        key, _ = self.insert_and_map(corners, [1] * (ncols - 1), "")
+        return key
+
     def interpolation_map_weight(self, key, query):
         """reference: coordinate_map_manager.cpp:1080 -> [in rows int32, out rows int32, weights fp32]
         of every present corner, ordered by query row, then corner."""
@@ -1492,6 +1512,53 @@ def LocalPoolingBackwardGPU(in_feat, grad_out_feat, num_nonzero, kernel_size, ke
         _lib.ptr(grad_out_feat), _lib.dtype_code(in_feat.dtype), km.n_in, C, _lib.ptr(km.in_nbr),
         km.K, km.n_out, mode, _lib.ptr(num_nonzero) if num_nonzero.numel() else None,
         _lib.ptr(grad_in), _lib.current_stream()))
+    return grad_in
+
+
+def LocalPoolingTransposeForwardGPU(in_feat, kernel_size, kernel_stride, kernel_dilation,
+                                    region_type, offset, expand_coordinates, pooling_mode, in_key,
+                                    out_key, manager):
+    """reference: LocalPoolingTransposeForwardGPU src/local_pooling_transpose_gpu.cu (CPU twin
+    local_pooling_transpose_cpu.cpp).  Both reference backends sum, whatever `pooling_mode` says
+    (use_avg = false): out[o] = sum_k in[out_nbr[k][o]] over the transposed pooling map; the
+    second result (num_nonzero) is empty.  Mutates `out_key` when it is unset."""
+    _check_feats(in_feat, manager, in_key)
+    if not out_key.is_key_set():
+        ik = manager._k(in_key)
+        for t, s in zip(ik[0], kernel_stride):
+            _assert(t % int(s) == 0, "Invalid up stride on tensor stride:", list(ik[0]),
+                    "kernel stride:", list(kernel_stride))
+        out_ts = [t // int(s) for t, s in zip(ik[0], kernel_stride)]
+        ok, _ = manager._stride_region(in_key, region_type, kernel_size, kernel_dilation, offset,
+                                       out_ts, out_ts, True, expand_coordinates)
+        out_key.set_key(list(ok[0]), ok[1])
+    km = manager._kernel_map(in_key, out_key, kernel_size, kernel_stride, kernel_dilation,
+                             region_type, offset, True, True)
+    C = in_feat.size(1)
+    out = torch.empty((km.n_out, C), dtype=in_feat.dtype, device=in_feat.device)
+    _lib.check(_lib.load().meb200_pool_forward(
+        _lib.ptr(in_feat), _lib.dtype_code(in_feat.dtype), km.n_in, C, _lib.ptr(km.out_nbr),
+        km.K, km.n_out, _lib.POOL_SUM, _lib.ptr(out), None, _lib.current_stream()))
+    return out, torch.empty(0, dtype=in_feat.dtype, device=in_feat.device)
+
+
+def LocalPoolingTransposeBackwardGPU(in_feat, grad_out_feat, num_nonzero, kernel_size,
+                                     kernel_stride, kernel_dilation, region_type, offset,
+                                     pooling_mode, in_key, out_key, manager):
+    """reference: LocalPoolingTransposeBackwardGPU src/local_pooling_transpose_gpu.cu: the sum's
+    adjoint, grad_in[i] = sum_k grad_out[in_nbr[k][i]] (one write per element)."""
+    _check_feats(in_feat, manager, in_key)
+    _assert(manager.exists(out_key), ERROR_MAP_NOT_FOUND)
+    grad_out_feat = grad_out_feat.contiguous()
+    _assert(in_feat.dtype == grad_out_feat.dtype, "type mismatch")
+    km = manager._kernel_map(in_key, out_key, kernel_size, kernel_stride, kernel_dilation,
+                             region_type, offset, True, True)
+    _assert(grad_out_feat.size(0) == km.n_out, "Invalid grad_out size")
+    C = in_feat.size(1)
+    grad_in = torch.empty_like(in_feat)
+    _lib.check(_lib.load().meb200_pool_backward(
+        _lib.ptr(grad_out_feat), _lib.dtype_code(in_feat.dtype), km.n_in, C, _lib.ptr(km.in_nbr),
+        km.K, km.n_out, _lib.POOL_SUM, None, _lib.ptr(grad_in), _lib.current_stream()))
     return grad_in
 
 

@@ -215,6 +215,37 @@ k_interp_map(const float *__restrict__ query, uint32_t n, IntVec ts,
   weights[t] = w;
 }
 
+// Splat corners: for point q and corner k, floorf of every column (the batch column included, as
+// the reference's create_splat_coordinates floors it) plus 1 on axis j when bit NC-1-j of k is set
+// (the corner order of k_interp_map).  Status bits: 1 = a coordinate is not finite or a corner is
+// outside int32, 2 = a batch value is not an integer (k_interp_map rounds it, so its corners would
+// be missed).
+template <int NC>
+__global__ void __launch_bounds__(256)
+k_splat_coords(const float *__restrict__ field, uint32_t n, int32_t *__restrict__ out,
+               uint32_t *__restrict__ bad) {
+  constexpr uint32_t K = 1u << (NC - 1);
+  uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (uint64_t)n * K) return;
+  uint32_t q = (uint32_t)(t / K), k = (uint32_t)(t % K);
+  const float *p = field + (size_t)q * NC;
+  uint32_t status = 0;
+  int32_t c[NC];
+#pragma unroll
+  for (int j = 0; j < NC; ++j) {
+    float x = __ldg(p + j);
+    float f = floorf(x);
+    int64_t up = (j > 0 && ((k >> (NC - 1 - j)) & 1u)) ? 1 : 0;
+    bool in = f >= -2147483648.f && f < 2147483648.f;  // false for NaN and +-inf
+    int64_t v = in ? (int64_t)f + up : 0;
+    if (!in || v > 2147483647ll) status |= 1u;
+    if (j == 0 && in && f != x) status |= 2u;
+    c[j] = (int32_t)v;
+  }
+  store_coord<NC>(out, (uint32_t)t, c);
+  if (status != 0) atomicOr(bad, status);  // flags, not a sum: any order, same word
+}
+
 template <typename T, int V>
 __global__ void __launch_bounds__(256)
 k_interp_fwd(const T *__restrict__ F, uint32_t C, const int32_t *__restrict__ rows,
@@ -425,6 +456,22 @@ int meb200_interp_map(const float *query, uint32_t n, uint32_t ncols, const int3
   cudaStream_t s = (cudaStream_t)stream;
   MEB_DISPATCH_NCOLS(ncols, k_interp_map<NC><<<cdiv(total, 256), 256, 0, s>>>(
                                 query, n, ts, map_coords, table, capacity - 1, rows, weights));
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
+}
+
+int meb200_splat_coords(const float *field, uint32_t n, uint32_t ncols, int32_t *out,
+                        uint32_t *d_bad, void *stream) {
+  MEB_CHECK_ARG(ncols >= 2 && ncols <= MEB200_MAX_NCOLS, "ncols=%u", ncols);
+  MEB_CHECK_ARG(d_bad != nullptr, "null status word");
+  cudaStream_t s = (cudaStream_t)stream;
+  MEB_CUDA(cudaMemsetAsync(d_bad, 0, 4, s));
+  if (n == 0) return MEB200_OK;
+  MEB_CHECK_ARG(field && out, "null buffer");
+  uint64_t total = (uint64_t)n << (ncols - 1);
+  MEB_CHECK_ARG(total < 0xFFFFFFFFull, "n * 2^D too large");
+  MEB_DISPATCH_NCOLS(ncols, k_splat_coords<NC><<<cdiv(total, 256), 256, 0, s>>>(field, n, out,
+                                                                                d_bad));
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }

@@ -42,11 +42,18 @@ class MinkowskiInterpolationFunction(Function):
     @staticmethod
     def backward(ctx, grad_out_feat=None, grad_rows=None, grad_weights=None):
         rows, w = ctx.saved_tensors
-        K = rows.size(1)
-        group = _C.group_by_row(rows.view(-1), ctx.M)
-        grad, _ = _C.field_reduce(grad_out_feat.contiguous(), group, ctx.M, _lib.FIELD_SUM,
-                                  weight=w.view(-1), src_div=K)
-        return grad, None, None, None
+        return interp_adjoint(grad_out_feat, rows, w, ctx.M), None, None, None
+
+
+def interp_adjoint(src, rows, w, M, group=None):
+    """[M, C] out[r] = sum over the (point q, corner k) pairs with rows[q, k] = r of w[q, k] * src[q],
+    added in pair order: the transpose of `interp_forward` (the interpolation backward and the
+    splat forward).  `group` is the grouping of rows.view(-1) by row, when the caller has it."""
+    if group is None:
+        group = _C.group_by_row(rows.view(-1), M)
+    out, _ = _C.field_reduce(src.contiguous(), group, M, _lib.FIELD_SUM, weight=w.view(-1),
+                             src_div=rows.size(1))
+    return out
 
 
 def _pairs(rows, w):

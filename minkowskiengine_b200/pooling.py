@@ -108,6 +108,64 @@ class MinkowskiMaxPooling(MinkowskiPoolingBase):
                                       dimension=dimension)
 
 
+class MinkowskiLocalPoolingTransposeFunction(Function):
+    """Unpooling (reference: MinkowskiPooling.py:441-510): the sum over the transposed pooling map,
+    whatever `pooling_mode` says, as both reference backends compute it."""
+
+    @staticmethod
+    def forward(ctx, input_features: torch.Tensor, pooling_mode: PoolingMode,
+                kernel_generator: KernelGenerator, in_coordinate_map_key: CoordinateMapKey,
+                out_coordinate_map_key: CoordinateMapKey = None,
+                coordinate_manager: CoordinateManager = None):
+        if out_coordinate_map_key is None:
+            out_coordinate_map_key = CoordinateMapKey(
+                in_coordinate_map_key.get_coordinate_size())
+        input_features = input_features.contiguous()
+        ctx.input_features = input_features
+        ctx.pooling_mode = pooling_mode
+        ctx.kernel_generator = kernel_generator
+        ctx.in_coordinate_map_key = in_coordinate_map_key
+        ctx.out_coordinate_map_key = out_coordinate_map_key
+        ctx.coordinate_manager = coordinate_manager
+        kgen = kernel_generator
+        out_feat, num_nonzero = _C.LocalPoolingTransposeForwardGPU(
+            input_features, kgen.kernel_size, kgen.kernel_stride, kgen.kernel_dilation,
+            kgen.region_type, kgen.region_offsets, kgen.expand_coordinates, pooling_mode,
+            in_coordinate_map_key, out_coordinate_map_key, coordinate_manager._manager)
+        ctx.num_nonzero = num_nonzero
+        return out_feat
+
+    @staticmethod
+    def backward(ctx, grad_out_feat):
+        grad_out_feat = grad_out_feat.contiguous()
+        kgen = ctx.kernel_generator
+        grad_in_feat = _C.LocalPoolingTransposeBackwardGPU(
+            ctx.input_features, grad_out_feat, ctx.num_nonzero, kgen.kernel_size,
+            kgen.kernel_stride, kgen.kernel_dilation, kgen.region_type, kgen.region_offsets,
+            ctx.pooling_mode, ctx.in_coordinate_map_key, ctx.out_coordinate_map_key,
+            ctx.coordinate_manager._manager)
+        return grad_in_feat, None, None, None, None, None
+
+
+class MinkowskiPoolingTranspose(MinkowskiPoolingBase):
+    """Unpooling to the finer tensor stride `tensor_stride / stride` (reference:
+    MinkowskiPooling.py:513-580): out[o] = the SUM of the input rows that reach o through the
+    transposed pooling map.  (The reference's docstring says the sum is divided by the number of
+    contributors; its code does not divide, and neither does this.)  The finer map is reused when
+    it exists; `expand_coordinates=True` generates new coordinates around every input row."""
+
+    def __init__(self, kernel_size, stride, dilation=1, kernel_generator=None,
+                 expand_coordinates=False, dimension=None):
+        if kernel_generator is None:
+            kernel_generator = KernelGenerator(kernel_size=kernel_size, stride=stride,
+                                               dilation=dilation,
+                                               expand_coordinates=expand_coordinates,
+                                               dimension=dimension)
+        MinkowskiPoolingBase.__init__(self, kernel_size, stride, dilation, kernel_generator,
+                                      is_transpose=True, dimension=dimension)
+        self.pooling = MinkowskiLocalPoolingTransposeFunction
+
+
 class MinkowskiGlobalPoolingFunction(Function):
     """Per-cloud reduction to the origin map (reference: MinkowskiPooling.py:583-630)."""
 

@@ -14,6 +14,7 @@ from .backend import CoordinateMapKey
 from .common import convert_to_int_list
 from .coordinate_manager import CoordinateManager
 from .enums import CoordinateMapType
+from .interpolation import interp_adjoint
 from .sparse_tensor import (COORDINATE_KEY_DIFFERENT_ERROR, COORDINATE_MANAGER_DIFFERENT_ERROR,
                             SparseTensor, SparseTensorOperationMode, SparseTensorQuantizationMode,
                             Tensor, global_coordinate_manager, set_global_coordinate_manager,
@@ -22,8 +23,9 @@ from .sparse_tensor import (COORDINATE_KEY_DIFFERENT_ERROR, COORDINATE_MANAGER_D
 _Q = SparseTensorQuantizationMode
 _MODES = {_Q.UNWEIGHTED_SUM: _lib.FIELD_SUM, _Q.UNWEIGHTED_AVERAGE: _lib.FIELD_AVG,
           _Q.MAX_POOL: _lib.FIELD_MAX, _Q.RANDOM_SUBSAMPLE: _lib.FIELD_SUBSAMPLE}
-SPLAT_ERROR = ("SPLAT_LINEAR_INTERPOLATION (TensorField.splat) is not implemented: it is the "
-               "adjoint of interpolation and is left for a follow-up to the TensorField feature")
+SPLAT_ERROR = ("SPLAT_LINEAR_INTERPOLATION is not a quantisation mode of TensorField or .sparse(), "
+               "as in the reference: call TensorField.splat() to splat the points linearly onto "
+               "their 2^D corners")
 
 
 class MinkowskiFieldQuantizationFunction(Function):
@@ -68,6 +70,23 @@ class MinkowskiSliceFunction(Function):
         f2s = ctx.f2s
         grad, _ = _C.field_reduce(grad_out, f2s.group(), f2s.M, _lib.FIELD_SUM)
         return grad, None
+
+
+class MinkowskiSplatFunction(Function):
+    """Points -> the M rows of a splat map: out[r] = sum of w * F[q] over the (point q, corner) pairs
+    of row r in pair order (the interpolation backward's reduction), fp32 accumulation, one
+    rounding.  The backward is the interpolation forward with the same rows and weights."""
+
+    @staticmethod
+    def forward(ctx, feats, rec, M):
+        rows, w, group = rec
+        ctx.rec = rec
+        return interp_adjoint(feats, rows, w, M, group)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        rows, w, _ = ctx.rec
+        return _C.interp_forward(grad_out.contiguous(), rows, w), None, None
 
 
 def _new_manager(D, allocator_type, minkowski_algorithm):
@@ -139,6 +158,7 @@ class TensorField(Tensor):
         self.coordinate_field_map_key = coordinate_field_map_key
         self._batch_rows = None
         self._inverse_mapping = {}   # map key -> backend._FieldToSparse
+        self._splat = {}             # splat map key -> (rows, weights, grouping by row)
 
     @property
     def coordinate_key(self):
@@ -231,7 +251,19 @@ class TensorField(Tensor):
         return SparseTensor(feats, coordinate_map_key=key, coordinate_manager=mgr)
 
     def splat(self):
-        raise NotImplementedError(SPLAT_ERROR)
+        """Linear splatting, the adjoint of multilinear interpolation (reference:
+        MinkowskiTensorField.py:381-406): every point adds w * F to each of its 2^D corners
+        floor(x) + {0,1}^D, w = prod_j (1 - |x_j - c_j|), on a new map at tensor stride 1 (rows
+        in order of first occurrence; a corner of weight 0 is a row too).  Use
+        `y.interpolate(field)` to bring a network's output back to the points."""
+        mgr = self._manager._manager
+        key = mgr.splat_insert_and_map(self.coordinate_field_map_key)
+        M = mgr.size(key)
+        rows, w = mgr._interp_map(key, self.C.float().contiguous())
+        rec = (rows, w, _C.group_by_row(rows.view(-1), M))
+        self._splat[key] = rec
+        feats = MinkowskiSplatFunction.apply(self._F, rec, M)
+        return SparseTensor(feats, coordinate_map_key=key, coordinate_manager=self._manager)
 
     def __repr__(self):
         return (self.__class__.__name__ + "(\n  coordinates=" + str(self.C) + "\n  features="
