@@ -22,6 +22,7 @@ from .enums import BroadcastMode, MinkowskiAlgorithm, PoolingMode, RegionType
 from .kernel_generator import region_offsets
 
 ERROR_MAP_NOT_FOUND = "CoordinateMap not found"  # reference: src/errors.hpp:33
+ERROR_FIELD_DOMAIN = "TensorField coordinates must be finite and quantise to int32 voxels"
 
 
 def _assert(cond, *msg):
@@ -136,42 +137,233 @@ class _CoordinateMap:
 
     @staticmethod
     def build(candidates, tensor_stride, valid=None):
-        """Deduplicating insert of candidate rows -> (map, unique_index, inverse_map)."""
-        lib = _lib.load()
+        """Deduplicating insert of candidate rows (meb200_insert_and_map) -> (map, unique_index,
+        inverse_map): rows numbered by first occurrence, -1 for a row that is not `valid`.  Zero
+        candidates give a 0-row map over an empty table without a native call."""
         n, ncols = candidates.shape
         dev = candidates.device
-        cap = int(lib.meb200_hash_capacity(n))
-        table = torch.empty(cap, dtype=torch.int32, device=dev)
-        uniq = torch.empty((n, ncols), dtype=torch.int32, device=dev)
-        uidx = torch.empty(n, dtype=torch.int64, device=dev)
-        inv = torch.empty(n, dtype=torch.int64, device=dev)
-        scratch = torch.empty(int(lib.meb200_insert_scratch_bytes(n)), dtype=torch.uint8,
-                              device=dev)
+        if n == 0:
+            table = _new_table(0, dev).fill_(-1)
+            empty = torch.empty(0, dtype=torch.int64, device=dev)
+            return _CoordinateMap(candidates, table, table.numel(), tensor_stride), empty, empty
+        table, uniq, uidx, inv, scratch = _insert_buffers(n, ncols, dev)
         m = ctypes.c_uint32(0)
-        _lib.check(lib.meb200_insert_and_map(
-            _lib.ptr(candidates), _lib.ptr(valid), n, ncols, _lib.ptr(table), cap,
-            _lib.ptr(uniq), _lib.ptr(uidx), _lib.ptr(inv), _lib.ptr(scratch),
-            ctypes.byref(m), _lib.current_stream()))
+        _lib.check(_lib.load().meb200_insert_and_map(
+            _lib.ptr(candidates), _lib.ptr(valid), n, ncols, _lib.ptr(table), table.numel(),
+            _lib.ptr(uniq), _lib.ptr(uidx), _lib.ptr(inv), _lib.ptr(scratch), ctypes.byref(m),
+            _lib.current_stream()))
         m = int(m.value)
-        cmap = _CoordinateMap(uniq[:m], table, cap, tensor_stride)
-        return cmap, uidx[:m], inv
+        return _CoordinateMap(uniq[:m], table, table.numel(), tensor_stride), uidx[:m], inv
+
+
+def _c_ints(values):
+    return (ctypes.c_int32 * len(values))(*values)
+
+
+def _new_table(n, dev):
+    """Uninitialised row-index table sized for n rows (meb200_hash_capacity slots)."""
+    return torch.empty(int(_lib.load().meb200_hash_capacity(n)), dtype=torch.int32, device=dev)
+
+
+def _insert_buffers(n, ncols, dev):
+    """(table, unique rows, unique_index, inverse_map, scratch) of an insert of n candidate rows."""
+    table = _new_table(n, dev)
+    return (table, torch.empty((n, ncols), dtype=torch.int32, device=dev),
+            torch.empty(n, dtype=torch.int64, device=dev),
+            torch.empty(n, dtype=torch.int64, device=dev),
+            torch.empty(int(_lib.load().meb200_insert_scratch_bytes(n)), dtype=torch.uint8,
+                        device=dev))
+
+
+def _distinct_map(coords, tensor_stride, table=None):
+    """Map over rows known to be distinct (meb200_map_build_table), built into `table` when given
+    (a power of two of at least twice the rows), else into a table sized for the rows."""
+    if table is None:
+        table = _new_table(coords.shape[0], coords.device)
+    _lib.check(_lib.load().meb200_map_build_table(_lib.ptr(coords), coords.shape[0],
+                                                  coords.shape[1], _lib.ptr(table), table.numel(),
+                                                  _lib.current_stream()))
+    return _CoordinateMap(coords, table, table.numel(), tensor_stride)
+
+
+def _strided(coords, tensor_stride):
+    """Candidate rows: every row of `coords` floored to `tensor_stride` (meb200_stride_coords)."""
+    out = torch.empty_like(coords)
+    _lib.check(_lib.load().meb200_stride_coords(_lib.ptr(coords), coords.shape[0], coords.shape[1],
+                                                _c_ints(tensor_stride), _lib.ptr(out),
+                                                _lib.current_stream()))
+    return out
+
+
+def _find_rows(cmap, query):
+    """int64 row of every query row in map `cmap`, -1 where it has none (meb200_map_find)."""
+    res = torch.empty(query.shape[0], dtype=torch.int32, device=query.device)
+    _lib.check(_lib.load().meb200_map_find(_lib.ptr(cmap.coords), _lib.ptr(cmap.table),
+                                           cmap.capacity, cmap.ncols, _lib.ptr(query),
+                                           query.shape[0], _lib.ptr(res), _lib.current_stream()))
+    return res.long()
+
+
+_COORDINATE_DTYPE_ERROR = {torch.int32: "coordinates must be an IntTensor",
+                           torch.float32: "field coordinates must be a FloatTensor"}
+
+
+def _check_coordinates(coordinates, tensor_stride, dtype):
+    """Checks the int32 coordinates of a map or the float32 points of a field handed to the
+    manager -> the tensor stride as a list of ints."""
+    _assert(coordinates.dim() == 2, "coordinates must be 2-dimensional")
+    _assert(coordinates.dtype == dtype, _COORDINATE_DTYPE_ERROR[dtype])
+    _assert(coordinates.is_contiguous(), "coordinates must be contiguous")
+    _assert(coordinates.is_cuda,
+            "coordinates must be a CUDA tensor: minkowskiengine_b200 implements the GPU "
+            "coordinate manager only (no CPU backend, no fallback)")
+    ts = [int(v) for v in tensor_stride]
+    _assert(coordinates.size(1) - 1 == len(ts),
+            "The coordinate dimension (coordinate_size - 1):", coordinates.size(1) - 1,
+            " must match the size of tensor stride:", ts)
+    return ts
+
+
+# ---- map prediction (DESIGN.md §2) ---------------------------------------------------------------
+# A strided map is a function of the input coordinates alone, but creating it where the network
+# first asks for it costs a blocking read of its size with the whole forward pass queued in front
+# (the host's lead over the GPU is lost at every down-sampling layer, and the coarse levels —
+# 10-30 us kernels — then run launch bound).  So the pyramid the PREVIOUS manager of the same
+# coordinate width was asked for is enqueued right behind the first inserted map, on upper-bound
+# buffers with device-side row counts (meb200_insert_and_map_enqueue); its sizes reach the host
+# long before the layers that need them.  The kernel maps are functions of the coordinate maps as
+# well: the ones the previous manager was asked for are built right there, before the first layer
+# runs.  The GPU gets ~1.5 ms of table probing to chew on while the host enqueues the layers,
+# instead of meeting each map where the forward pass first needs it with nothing else queued.
+# A wrong prediction is only wasted work: a level that is never requested, or requested with
+# another stride, is dropped.
+_PREFETCH = os.environ.get("MEB200_MAP_PREFETCH", "1") not in ("", "0")
+
+
+class _Hint:
+    """What the last manager of one coordinate width was asked for: the kernel strides along the
+    stride chain below its first inserted map, its kernel maps in order (cache keys, no tensors)
+    and the cache keys of those whose pair lists (wgrad) were built."""
+
+    __slots__ = ("pyramid", "kernel_maps", "pairs")
+
+    def __init__(self):
+        self.pyramid, self.kernel_maps, self.pairs = (), (), set()
+
+
+_HINTS = {}     # coordinate width -> _Hint
+
+
+def _hint(ncols):
+    return _HINTS.setdefault(ncols, _Hint())
 
 
 class _PendingLevel:
     """One level of a stride pyramid whose kernels are enqueued but whose size has not been read
-    yet (see CoordinateMapManagerGPU_c10._prefetch_pyramid)."""
+    yet (see _Prediction.start)."""
 
     __slots__ = ("parent_key", "tensor_stride", "uniq", "inverse", "count_dev", "count_host",
                  "event")
 
 
-# kernel strides requested along the stride chain below the first inserted map of the previous
-# coordinate manager, per coordinate width: the prediction for the next manager's pyramid
-_PYRAMID_HINT = {}
-# ... and the kernel maps it was asked for, in order (keys + kernel geometry, no tensors)
-_KMAP_HINT = {}
-_PAIR_HINT = set()      # kernel-map cache keys whose pair lists (wgrad) were asked for
-_PREFETCH = os.environ.get("MEB200_MAP_PREFETCH", "1") not in ("", "0")
+class _Prediction:
+    """The map prediction of one manager: it records what the manager is asked for from its first
+    inserted map on (into _HINTS), and builds what the previous manager was asked for behind that
+    map.  The manager is passed in, not kept: a manager must die by reference counting alone."""
+
+    __slots__ = ("ncols", "chain_tip", "chain", "seen", "requests", "replaying", "pending")
+
+    def __init__(self):
+        self.ncols = None       # width of the first inserted map, once there is one
+        self.chain_tip = None   # last map of the stride chain below that map
+        self.chain = []         # kernel strides requested along that chain
+        self.seen = set()       # kernel-map cache keys the caller has asked for
+        self.requests = []      # ... in order, from the first inserted map on
+        self.replaying = False  # building predicted kernel maps, which are not requests
+        self.pending = {}       # out key -> _PendingLevel (enqueued, size not yet read)
+
+    def start(self, mgr, key, cmap):
+        """`key` is the first map inserted into `mgr`."""
+        self.ncols, self.chain_tip = cmap.ncols, key
+        hint = _HINTS.get(cmap.ncols) if _PREFETCH else None
+        if hint is not None:
+            self._enqueue_pyramid(mgr, key, cmap, hint.pyramid)
+            self._build_kernel_maps(mgr, hint)
+
+    def stride_requested(self, in_key, out_key, kernel_stride):
+        if in_key == self.chain_tip and out_key != in_key and not self.replaying:
+            self.chain_tip = out_key
+            self.chain.append(tuple(int(s) for s in kernel_stride))
+            _hint(self.ncols).pyramid = tuple(self.chain)
+
+    def kernel_map_requested(self, cache_key, region_type):
+        if self.replaying or cache_key in self.seen:
+            return
+        self.seen.add(cache_key)
+        if region_type != RegionType.CUSTOM and self.ncols is not None:
+            self.requests.append(cache_key)
+            _hint(self.ncols).kernel_maps = tuple(self.requests)
+
+    def take(self, mgr, in_key, out_key):
+        """Makes the enqueued level `out_key` a map of `mgr` if it was built from `in_key`."""
+        lv = self.pending.pop(out_key, None)
+        if lv is None or lv.parent_key != in_key:
+            return False
+        lv.event.synchronize()          # normally long past: enqueued before the first layer
+        m = int(lv.count_host.item())
+        mgr._maps[out_key] = _distinct_map(lv.uniq[:m], lv.tensor_stride)
+        mgr._parents[out_key] = (in_key, lv.inverse[:mgr._maps[in_key].size])
+        return True
+
+    def _enqueue_pyramid(self, mgr, key, cmap, strides):
+        if not strides or cmap.size == 0:
+            return
+        n, ncols, dev = cmap.size, cmap.ncols, cmap.coords.device
+        parent_key, parent_coords, parent_count = key, cmap.coords, None
+        for ks in strides:
+            if len(ks) != len(parent_key[0]):
+                return
+            out_ts = tuple(t * s for t, s in zip(parent_key[0], ks))
+            out_key = (out_ts, parent_key[1])
+            if out_key in mgr._maps or out_key in self.pending:
+                return
+            # rows past the parent's (device-side) count are whatever the buffer holds: they are
+            # strided like the others and then ignored by the insert
+            cand = _strided(parent_coords, out_ts)
+            table, uniq, uidx, inverse, scratch = _insert_buffers(n, ncols, dev)
+            lv = _PendingLevel()
+            lv.parent_key, lv.tensor_stride, lv.uniq, lv.inverse = parent_key, out_ts, uniq, inverse
+            lv.count_dev = torch.empty(1, dtype=torch.int32, device=dev)
+            _lib.check(_lib.load().meb200_insert_and_map_enqueue(
+                _lib.ptr(cand), None, _lib.ptr(parent_count), n, ncols, _lib.ptr(table),
+                table.numel(), _lib.ptr(uniq), _lib.ptr(uidx), _lib.ptr(inverse), _lib.ptr(scratch),
+                _lib.ptr(lv.count_dev), _lib.current_stream()))
+            lv.count_host = torch.empty(1, dtype=torch.int32, pin_memory=True)
+            lv.count_host.copy_(lv.count_dev, non_blocking=True)
+            lv.event = torch.cuda.Event()
+            lv.event.record()
+            self.pending[out_key] = lv
+            parent_key, parent_coords, parent_count = out_key, uniq, lv.count_dev
+
+    def _materialize(self, mgr, key):
+        if key in mgr._maps:
+            return True
+        lv = self.pending.get(key)
+        return (lv is not None and self._materialize(mgr, lv.parent_key)
+                and self.take(mgr, lv.parent_key, key))
+
+    def _build_kernel_maps(self, mgr, hint):
+        self.replaying = True
+        try:
+            for ck in hint.kernel_maps:
+                ik, ok, ksize, kstride, kdil, region, is_transpose, is_pool = ck
+                if self._materialize(mgr, ik) and self._materialize(mgr, ok):
+                    km = mgr._kernel_map(ik, ok, ksize, kstride, kdil, region, None, is_transpose,
+                                         is_pool)
+                    if ck in hint.pairs:
+                        km.pair_lists()          # the backward pass will want them
+        finally:
+            self.replaying = False
 
 
 class _KernelMap:
@@ -208,8 +400,8 @@ class _KernelMap:
         that a consumer keeps one chunk's feature rows L2-resident across the offsets.  Built on
         first use; a swapped view shares its source's lists with the two sides exchanged."""
         if self._pairs is None:
-            if self._hint_key is not None:
-                _PAIR_HINT.add(self._hint_key)
+            if self._hint_key is not None:     # (its in map's key gives the width)
+                _hint(len(self._hint_key[0][0]) + 1).pairs.add(self._hint_key)
             if self._pair_src is not None:
                 pin, pout, seg, nch = self._pair_src.pair_lists()
                 self._pairs = (pout, pin, seg, nch)
@@ -308,13 +500,7 @@ class CoordinateMapManagerGPU_c10:
         self._maps = {}         # (tuple tensor_stride, str id) -> _CoordinateMap
         self._kernel_maps = {}  # 8-tuple (types.hpp:183-192) -> _KernelMap
         self._parents = {}      # out key -> (in key, int64 row of every in row in out map)
-        self._pending = {}      # out key -> _PendingLevel (enqueued, size not yet read)
-        self._chain_tip = None  # last map of the stride chain below the first inserted map
-        self._chain = []        # kernel strides requested along that chain
-        self._km_seen = set()   # kernel-map cache keys the caller has asked for
-        self._km_requests = []  # ... in order: the prediction for the next manager
-        self._replaying = False
-        self._hint_ncols = None
+        self._prediction = _Prediction()
         self._inserted = []     # keys of the maps made by insert_and_map, in order
         self._origin_covers = 0  # ... how many of them the origin map was built from
         self._groupings = {}    # map key -> _OriginGrouping
@@ -342,6 +528,13 @@ class CoordinateMapManagerGPU_c10:
         _assert(k in self._maps, what, ERROR_MAP_NOT_FOUND)
         return self._maps[k]
 
+    def _free_key(self, tensor_stride, string_id, taken):
+        """(tensor stride, string_id), with a random suffix when `taken` holds that key."""
+        key = (tuple(tensor_stride), string_id)
+        while key in taken:
+            key = (key[0], self.get_random_string_id(key[0], string_id)[1])
+        return key
+
     def get_random_string_id(self, tensor_stride, string_id=""):
         ts = tuple(int(v) for v in tensor_stride)
         while True:
@@ -363,19 +556,8 @@ class CoordinateMapManagerGPU_c10:
     # -- map creation ----------------------------------------------------------------
     def insert_and_map(self, coordinates, tensor_stride, string_id=""):
         """reference: coordinate_map_manager.cpp:353-399"""
-        _assert(coordinates.dim() == 2, "coordinates must be 2-dimensional")
-        _assert(coordinates.dtype == torch.int32, "coordinates must be an IntTensor")
-        _assert(coordinates.is_contiguous(), "coordinates must be contiguous")
-        _assert(coordinates.is_cuda,
-                "coordinates must be a CUDA tensor: minkowskiengine_b200 implements the GPU "
-                "coordinate manager only (no CPU backend, no fallback)")
-        ts = [int(v) for v in tensor_stride]
-        _assert(coordinates.size(1) - 1 == len(ts),
-                "The coordinate dimension (coordinate_size - 1):", coordinates.size(1) - 1,
-                " must match the size of tensor stride:", ts)
-        key = (tuple(ts), string_id)
-        if key in self._maps:
-            key = self.get_random_string_id(ts, string_id)
+        ts = _check_coordinates(coordinates, tensor_stride, torch.int32)
+        key = self._free_key(ts, string_id, self._maps)
         cmap, unique_index, inverse_map = _CoordinateMap.build(coordinates, ts)
         self._add_inserted(key, cmap)
         if cmap.size == coordinates.size(0):
@@ -392,10 +574,7 @@ class CoordinateMapManagerGPU_c10:
         self._maps[key] = cmap
         self._inserted.append(key)
         if first:
-            self._chain_tip = key
-            self._hint_ncols = cmap.ncols
-            self._prefetch_pyramid(key, cmap)
-            self._prefetch_kernel_maps(cmap.ncols)
+            self._prediction.start(self, key, cmap)
 
     def _stride(self, in_key, kernel_stride, string_id=""):
         """reference: coordinate_map_manager.cpp:406-429 -> (out key tuple, created?)"""
@@ -404,120 +583,16 @@ class CoordinateMapManagerGPU_c10:
         _assert(len(kernel_stride) == len(in_key[0]), "stride size mismatch.")
         out_ts = tuple(t * int(s) for t, s in zip(in_key[0], kernel_stride))
         out_key = (out_ts, string_id if string_id else in_key[1])
-        if in_key == self._chain_tip and out_key != in_key and not self._replaying:
-            # remember the pyramid for the next manager
-            self._chain_tip = out_key
-            self._chain.append(tuple(int(s) for s in kernel_stride))
-            _PYRAMID_HINT[len(in_key[0]) + 1] = tuple(self._chain)
+        self._prediction.stride_requested(in_key, out_key, kernel_stride)
         if out_key in self._maps:
             return out_key, False
-        if self._take_pending(in_key, out_key):
+        if self._prediction.take(self, in_key, out_key):
             return out_key, True
-        in_map = self._maps[in_key]
-        lib = _lib.load()
-        cand = torch.empty_like(in_map.coords)
-        ts_arr = (ctypes.c_int32 * len(out_ts))(*out_ts)
-        _lib.check(lib.meb200_stride_coords(_lib.ptr(in_map.coords), in_map.size, in_map.ncols,
-                                            ts_arr, _lib.ptr(cand), _lib.current_stream()))
-        out_map, _, inverse = _CoordinateMap.build(cand, out_ts)
+        out_map, _, inverse = _CoordinateMap.build(_strided(self._maps[in_key].coords, out_ts),
+                                                   out_ts)
         self._maps[out_key] = out_map
         self._parents[out_key] = (in_key, inverse)
         return out_key, True
-
-    # A strided map is a function of the input coordinates alone, but creating it where the
-    # network first asks for it costs a blocking read of its size with the whole forward pass
-    # queued in front (the host's lead over the GPU is lost at every down-sampling layer, and the
-    # coarse levels — 10-30 us kernels — then run launch bound).  So the pyramid the PREVIOUS
-    # manager was asked for (_PYRAMID_HINT) is enqueued right behind the input map, on upper-bound
-    # buffers with device-side row counts (meb200_insert_and_map_enqueue); its sizes reach the
-    # host long before the layers that need them.  A wrong prediction is only wasted work: a
-    # level that is never requested, or requested with another stride, is dropped.
-    def _prefetch_pyramid(self, key, cmap):
-        hint = _PYRAMID_HINT.get(cmap.ncols) if _PREFETCH else None
-        if not hint or cmap.size == 0:
-            return
-        lib = _lib.load()
-        dev = cmap.coords.device
-        n, ncols = cmap.size, cmap.ncols
-        stream = _lib.current_stream()
-        cap = int(lib.meb200_hash_capacity(n))
-        scratch_bytes = int(lib.meb200_insert_scratch_bytes(n))
-        parent_key, parent_coords, parent_count = key, cmap.coords, None
-        for ks in hint:
-            if len(ks) != len(parent_key[0]):
-                return
-            out_ts = tuple(t * s for t, s in zip(parent_key[0], ks))
-            out_key = (out_ts, parent_key[1])
-            if out_key in self._maps or out_key in self._pending:
-                return
-            lv = _PendingLevel()
-            lv.parent_key, lv.tensor_stride = parent_key, out_ts
-            cand = torch.empty((n, ncols), dtype=torch.int32, device=dev)
-            ts_arr = (ctypes.c_int32 * len(out_ts))(*out_ts)
-            # rows past the parent's (device-side) count are whatever the buffer holds: they are
-            # strided like the others and then ignored by the insert
-            _lib.check(lib.meb200_stride_coords(_lib.ptr(parent_coords), n, ncols, ts_arr,
-                                                _lib.ptr(cand), stream))
-            table = torch.empty(cap, dtype=torch.int32, device=dev)
-            lv.uniq = torch.empty((n, ncols), dtype=torch.int32, device=dev)
-            uidx = torch.empty(n, dtype=torch.int64, device=dev)
-            lv.inverse = torch.empty(n, dtype=torch.int64, device=dev)
-            scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=dev)
-            lv.count_dev = torch.empty(1, dtype=torch.int32, device=dev)
-            _lib.check(lib.meb200_insert_and_map_enqueue(
-                _lib.ptr(cand), None, _lib.ptr(parent_count), n, ncols, _lib.ptr(table), cap,
-                _lib.ptr(lv.uniq), _lib.ptr(uidx), _lib.ptr(lv.inverse), _lib.ptr(scratch),
-                _lib.ptr(lv.count_dev), stream))
-            lv.count_host = torch.empty(1, dtype=torch.int32, pin_memory=True)
-            lv.count_host.copy_(lv.count_dev, non_blocking=True)
-            lv.event = torch.cuda.Event()
-            lv.event.record()
-            self._pending[out_key] = lv
-            parent_key, parent_coords, parent_count = out_key, lv.uniq, lv.count_dev
-
-    # The kernel maps are functions of the coordinate maps alone as well: the ones the previous
-    # manager was asked for (_KMAP_HINT) are built right here, before the first layer runs.  The
-    # GPU gets ~1.5 ms of table probing to chew on while the host enqueues the layers, instead of
-    # meeting each map where the forward pass first needs it with nothing else queued (the coarse
-    # levels of a U-Net are launch bound: 10-30 us kernels against ~50 us of host work per layer).
-    def _materialize(self, key):
-        if key in self._maps:
-            return True
-        lv = self._pending.get(key)
-        return (lv is not None and self._materialize(lv.parent_key)
-                and self._take_pending(lv.parent_key, key))
-
-    def _prefetch_kernel_maps(self, ncols):
-        hint = _KMAP_HINT.get(ncols) if _PREFETCH else None
-        if not hint:
-            return
-        self._replaying = True
-        try:
-            for ik, ok, ksize, kstride, kdil, region, is_transpose, is_pool in hint:
-                if self._materialize(ik) and self._materialize(ok):
-                    km = self._kernel_map(ik, ok, ksize, kstride, kdil, region, None,
-                                          is_transpose, is_pool)
-                    if (ik, ok, ksize, kstride, kdil, region, is_transpose, is_pool) in _PAIR_HINT:
-                        km.pair_lists()          # the backward pass will want them
-        finally:
-            self._replaying = False
-
-    def _take_pending(self, in_key, out_key):
-        """Turns the enqueued level `out_key` into a map if it was built from `in_key`."""
-        lv = self._pending.pop(out_key, None)
-        if lv is None or lv.parent_key != in_key:
-            return False
-        lib = _lib.load()
-        lv.event.synchronize()          # normally long past: enqueued before the first layer
-        m = int(lv.count_host.item())
-        cap = int(lib.meb200_hash_capacity(m))
-        table = torch.empty(cap, dtype=torch.int32, device=lv.uniq.device)
-        coords = lv.uniq[:m]
-        _lib.check(lib.meb200_map_build_table(_lib.ptr(coords), m, coords.shape[1],
-                                              _lib.ptr(table), cap, _lib.current_stream()))
-        self._maps[out_key] = _CoordinateMap(coords, table, cap, lv.tensor_stride)
-        self._parents[out_key] = (in_key, lv.inverse[:self._maps[in_key].size])
-        return True
 
     def stride(self, key, stride, string_id=""):
         out_key, _ = self._stride(key, [int(s) for s in stride], string_id)
@@ -542,14 +617,12 @@ class CoordinateMapManagerGPU_c10:
         n = in_map.size
         cand = torch.empty((n * K, in_map.ncols), dtype=torch.int32, device=in_map.coords.device)
         valid = torch.empty(n * K, dtype=torch.uint8, device=in_map.coords.device)
-        ts_arr = (ctypes.c_int32 * len(out_ts))(*out_ts)
         _lib.check(lib.meb200_region_coords(
-            _lib.ptr(in_map.coords), n, in_map.ncols, _lib.ptr(offs), K, ts_arr,
+            _lib.ptr(in_map.coords), n, in_map.ncols, _lib.ptr(offs), K, _c_ints(out_ts),
             0 if is_transpose else 1, _lib.ptr(cand), _lib.ptr(valid), _lib.current_stream()))
         out_map, _, _ = _CoordinateMap.build(cand, out_ts, valid)
         out_map.coords = out_map.coords.clone()  # drop the n*K candidate buffer
-        if exists:
-            out_key = self.get_random_string_id(out_ts, "")
+        out_key = self._free_key(out_ts, "", self._maps)
         self._maps[out_key] = out_map
         return out_key, True
 
@@ -593,11 +666,7 @@ class CoordinateMapManagerGPU_c10:
         kdil = tuple(int(v) for v in kernel_dilation)
         _assert(len(ksize) == len(kstride) == len(kdil), "kernel size mismatch")
         cache_key = (ik, ok, ksize, kstride, kdil, region_type, bool(is_transpose), bool(is_pool))
-        if not self._replaying and cache_key not in self._km_seen:
-            self._km_seen.add(cache_key)
-            if region_type != RegionType.CUSTOM and self._hint_ncols is not None:
-                self._km_requests.append(cache_key)
-                _KMAP_HINT[self._hint_ncols] = tuple(self._km_requests)
+        self._prediction.kernel_map_requested(cache_key, region_type)
         km = self._kernel_maps.get(cache_key)
         if km is not None:
             return km
@@ -660,18 +729,7 @@ class CoordinateMapManagerGPU_c10:
         if par is not None and par[0] == in_key:
             inv = par[1]
         else:
-            lib = _lib.load()
-            cand = torch.empty_like(in_map.coords)
-            ts = out_map.tensor_stride
-            ts_arr = (ctypes.c_int32 * len(ts))(*ts)
-            _lib.check(lib.meb200_stride_coords(_lib.ptr(in_map.coords), in_map.size,
-                                                in_map.ncols, ts_arr, _lib.ptr(cand),
-                                                _lib.current_stream()))
-            res = torch.empty(in_map.size, dtype=torch.int32, device=cand.device)
-            _lib.check(lib.meb200_map_find(_lib.ptr(out_map.coords), _lib.ptr(out_map.table),
-                                           out_map.capacity, out_map.ncols, _lib.ptr(cand),
-                                           in_map.size, _lib.ptr(res), _lib.current_stream()))
-            inv = res.long()
+            inv = _find_rows(out_map, _strided(in_map.coords, out_map.tensor_stride))
         rows = torch.arange(in_map.size, dtype=torch.int64, device=inv.device)
         keep = inv >= 0
         return rows[keep], inv[keep]
@@ -700,18 +758,13 @@ class CoordinateMapManagerGPU_c10:
         key = self._origin_key(ncols)
         if key in self._maps:
             return key
-        lib = _lib.load()
         batch = torch.cat([self._maps[k].coords[:, 0] for k in self._inserted])
         cand = torch.zeros((batch.numel(), ncols), dtype=torch.int32, device=batch.device)
         cand[:, 0] = batch
         cmap, _, _ = _CoordinateMap.build(cand, key[0])
         # ascending batch index: rebuild the table over the sorted rows
         coords = cmap.coords[torch.argsort(cmap.coords[:, 0])].contiguous()
-        table = torch.empty(cmap.capacity, dtype=torch.int32, device=coords.device)
-        _lib.check(lib.meb200_map_build_table(_lib.ptr(coords), coords.shape[0], ncols,
-                                              _lib.ptr(table), cmap.capacity,
-                                              _lib.current_stream()))
-        self._maps[key] = _CoordinateMap(coords, table, cmap.capacity, key[0])
+        self._maps[key] = _distinct_map(coords, key[0], cmap.table)
         self._origin_covers = len(self._inserted)
         return key
 
@@ -769,20 +822,6 @@ class CoordinateMapManagerGPU_c10:
         return batch, rows
 
     # -- pruning and union -------------------------------------------------------------
-    def _new_map(self, cand, ts, valid=None):
-        """Insert of candidate rows (meb200_insert_and_map) -> (map, unique_index, inverse_map);
-        zero candidates or zero survivors give a 0-row map whose table is empty."""
-        dev = cand.device
-        if cand.shape[0] == 0:
-            cap = int(_lib.load().meb200_hash_capacity(0))
-            table = torch.full((cap,), -1, dtype=torch.int32, device=dev)
-            empty = torch.empty(0, dtype=torch.int64, device=dev)
-            return _CoordinateMap(cand, table, cap, ts), empty, empty
-        cmap, uidx, inv = _CoordinateMap.build(cand, ts, valid)
-        if cmap.size == 0:
-            cmap.table.fill_(-1)
-        return cmap, uidx, inv
-
     def _prune(self, in_key, keep):
         """reference: CoordinateMapManager::prune (coordinate_map_manager.cpp) -> out key tuple.
         Rows of the pruned map are the kept rows in ascending input order (the insert numbers rows
@@ -791,7 +830,8 @@ class CoordinateMapManagerGPU_c10:
         _assert(ik in self._maps, ERROR_MAP_NOT_FOUND)
         in_map = self._maps[ik]
         valid = keep if keep.dtype == torch.uint8 else keep.view(torch.uint8)
-        cmap, uidx, inv = self._new_map(in_map.coords, in_map.tensor_stride, valid.contiguous())
+        cmap, uidx, inv = _CoordinateMap.build(in_map.coords, in_map.tensor_stride,
+                                              valid.contiguous())
         ok = self.get_random_string_id(in_map.tensor_stride, "")
         self._maps[ok] = cmap
         self._prunes[(ik, ok)] = (uidx, inv)
@@ -814,7 +854,7 @@ class CoordinateMapManagerGPU_c10:
                     "of", list(k[0]), k[1], "!= tensor stride", list(ts0), "of the first input")
             _assert(m.ncols == nc0, "union_map: coordinate size", m.ncols, "!=", nc0)
         cand = torch.cat([m.coords for m in maps]).contiguous()
-        cmap, _, inv = self._new_map(cand, ts0)
+        cmap, _, inv = _CoordinateMap.build(cand, ts0)
         ok = self.get_random_string_id(ts0, "")
         self._maps[ok] = cmap
         um = _UnionMap()
@@ -839,19 +879,8 @@ class CoordinateMapManagerGPU_c10:
     # -- tensor fields -------------------------------------------------------------------
     def insert_field(self, coordinates, tensor_stride, string_id=""):
         """reference: coordinate_map_manager.cpp:145-181.  The field keeps the float32 points."""
-        _assert(coordinates.dim() == 2, "coordinates must be 2-dimensional")
-        _assert(coordinates.dtype == torch.float32, "field coordinates must be a FloatTensor")
-        _assert(coordinates.is_contiguous(), "coordinates must be contiguous")
-        _assert(coordinates.is_cuda,
-                "coordinates must be a CUDA tensor: minkowskiengine_b200 implements the GPU "
-                "coordinate manager only (no CPU backend, no fallback)")
-        ts = [int(v) for v in tensor_stride]
-        _assert(coordinates.size(1) - 1 == len(ts),
-                "The coordinate dimension (coordinate_size - 1):", coordinates.size(1) - 1,
-                " must match the size of tensor stride:", ts)
-        key = (tuple(ts), string_id)
-        while key in self._fields:
-            key = (key[0], self.get_random_string_id(ts, string_id)[1])
+        ts = _check_coordinates(coordinates, tensor_stride, torch.float32)
+        key = self._free_key(ts, string_id, self._fields)
         self._fields[key] = coordinates
         return CoordinateMapKey(list(key[0]), key[1])
 
@@ -868,37 +897,26 @@ class CoordinateMapManagerGPU_c10:
         -> map key tuple.  Cached per (field, stride, string id): quantising again returns the same
         map and grouping."""
         fk, field = self._field(field_key)
-        ts = tuple(int(v) for v in tensor_stride)
-        _assert(len(ts) + 1 == field.size(1), "The coordinate dimension (coordinate_size - 1):",
-                field.size(1) - 1, " must match the size of tensor stride:", list(ts))
+        ts = tuple(_check_coordinates(field, tensor_stride, torch.float32))
         ck = (fk, ts, string_id)
         sk = self._field_quant.get(ck)
         if sk is not None:
             return sk
-        lib = _lib.load()
         n, ncols = field.shape
-        dev = field.device
-        cap = int(lib.meb200_hash_capacity(n))
-        table = torch.empty(cap, dtype=torch.int32, device=dev)
-        q = torch.empty((n, ncols), dtype=torch.int32, device=dev)
-        uniq = torch.empty((n, ncols), dtype=torch.int32, device=dev)
-        uidx = torch.empty(n, dtype=torch.int64, device=dev)
-        inv = torch.empty(n, dtype=torch.int64, device=dev)
-        scratch = torch.empty(int(lib.meb200_insert_scratch_bytes(n)), dtype=torch.uint8, device=dev)
+        q = torch.empty((n, ncols), dtype=torch.int32, device=field.device)
+        table, uniq, uidx, inv, scratch = _insert_buffers(n, ncols, field.device)
         m = ctypes.c_uint32(0)
-        rc = lib.meb200_field_insert_and_map(
-            _lib.ptr(field), n, ncols, (ctypes.c_int32 * len(ts))(*ts), _lib.ptr(q), _lib.ptr(table),
-            cap, _lib.ptr(uniq), _lib.ptr(uidx), _lib.ptr(inv), _lib.ptr(scratch), ctypes.byref(m),
+        rc = _lib.load().meb200_field_insert_and_map(
+            _lib.ptr(field), n, ncols, _c_ints(ts), _lib.ptr(q), _lib.ptr(table), table.numel(),
+            _lib.ptr(uniq), _lib.ptr(uidx), _lib.ptr(inv), _lib.ptr(scratch), ctypes.byref(m),
             _lib.current_stream())
         if rc == _lib.ERR_DOMAIN:
-            raise ValueError("TensorField coordinates must be finite and quantise to int32 voxels")
+            raise ValueError(ERROR_FIELD_DOMAIN)
         _lib.check(rc)
         self._field_valid.add(fk)
         m = int(m.value)
-        key = (ts, string_id)
-        if key in self._maps:
-            key = self.get_random_string_id(ts, string_id)
-        self._add_inserted(key, _CoordinateMap(uniq[:m], table, cap, ts))
+        key = self._free_key(ts, string_id, self._maps)
+        self._add_inserted(key, _CoordinateMap(uniq[:m], table, table.numel(), ts))
         self._field_maps[(fk, key)] = _FieldToSparse(inv, m, uidx[:m])
         self._field_quant[ck] = key
         return key
@@ -930,27 +948,20 @@ class CoordinateMapManagerGPU_c10:
         cmap = self._get(sk)
         _assert(cmap.ncols == field.size(1), "The coordinate dimension mismatch.", field.size(1),
                 "!=", cmap.ncols)
-        lib = _lib.load()
         n, ncols = field.shape
-        stream = _lib.current_stream()
         q = torch.empty((n, ncols), dtype=torch.int32, device=field.device)
         # the validity of the coordinates reaches the host with the row count of the first map made
         # from the field; only a field never quantised before pays a read here, once
         bad = None if fk in self._field_valid else \
             torch.empty(1, dtype=torch.int32, device=field.device)
-        ts = cmap.tensor_stride
-        _lib.check(lib.meb200_quantize_field(_lib.ptr(field), n, ncols,
-                                             (ctypes.c_int32 * len(ts))(*ts), _lib.ptr(q),
-                                             _lib.ptr(bad), stream))
+        _lib.check(_lib.load().meb200_quantize_field(_lib.ptr(field), n, ncols,
+                                                     _c_ints(cmap.tensor_stride), _lib.ptr(q),
+                                                     _lib.ptr(bad), _lib.current_stream()))
         if bad is not None:
             if int(bad.item()) != 0:
-                raise ValueError("TensorField coordinates must be finite and quantise to int32 "
-                                 "voxels")
+                raise ValueError(ERROR_FIELD_DOMAIN)
             self._field_valid.add(fk)
-        res = torch.empty(n, dtype=torch.int32, device=field.device)
-        _lib.check(lib.meb200_map_find(_lib.ptr(cmap.coords), _lib.ptr(cmap.table), cmap.capacity,
-                                       ncols, _lib.ptr(q), n, _lib.ptr(res), stream))
-        f2s = _FieldToSparse(res.long(), cmap.size)
+        f2s = _FieldToSparse(_find_rows(cmap, q), cmap.size)
         self._field_maps[(fk, sk)] = f2s
         return f2s
 
@@ -977,9 +988,8 @@ class CoordinateMapManagerGPU_c10:
         K = 1 << (ncols - 1)
         rows = torch.empty((n, K), dtype=torch.int32, device=query.device)
         w = torch.empty((n, K), dtype=torch.float32, device=query.device)
-        ts = cmap.tensor_stride
         _lib.check(_lib.load().meb200_interp_map(
-            _lib.ptr(query), n, ncols, (ctypes.c_int32 * len(ts))(*ts), _lib.ptr(cmap.coords),
+            _lib.ptr(query), n, ncols, _c_ints(cmap.tensor_stride), _lib.ptr(cmap.coords),
             _lib.ptr(cmap.table), cmap.capacity, _lib.ptr(rows), _lib.ptr(w), _lib.current_stream()))
         return rows, w
 
@@ -997,7 +1007,7 @@ class CoordinateMapManagerGPU_c10:
                                                    _lib.ptr(bad), _lib.current_stream()))
         status = int(bad.item())
         if status & 1:
-            raise ValueError("TensorField coordinates must be finite and quantise to int32 voxels")
+            raise ValueError(ERROR_FIELD_DOMAIN)
         if status & 2:
             raise ValueError("splat needs integer batch indices in the first coordinate column")
         key, _ = self.insert_and_map(corners, [1] * (ncols - 1), "")
@@ -1393,6 +1403,36 @@ def _conv_backward_impl(in_feat, grad_out, kernel, km, need_in=True, need_w=True
     return grad_in, grad_w
 
 
+def _set_strided_key(manager, in_key, out_key, kernel_stride, region=None):
+    """Sets an unset `out_key` to the map at the tensor stride of `in_key` times `kernel_stride`:
+    the strided map, or with region = (region_type, kernel_size, dilation, offset) the map of the
+    regions around the input rows (expand_coordinates)."""
+    if out_key.is_key_set():
+        return
+    if region is None:
+        ok, _ = manager._stride(in_key, kernel_stride)
+    else:
+        ik = manager._k(in_key)
+        out_ts = [t * int(s) for t, s in zip(ik[0], kernel_stride)]
+        ok, _ = manager._stride_region(in_key, *region, ik[0], out_ts, False, True)
+    out_key.set_key(list(ok[0]), ok[1])
+
+
+def _set_transposed_key(manager, in_key, out_key, kernel_stride, region, expand_coordinates):
+    """Sets an unset `out_key` to the map at the tensor stride of `in_key` divided by
+    `kernel_stride`, made from the regions = (region_type, kernel_size, dilation, offset) around
+    the input rows."""
+    if out_key.is_key_set():
+        return
+    ik = manager._k(in_key)
+    for t, s in zip(ik[0], kernel_stride):
+        _assert(t % int(s) == 0, "Invalid up stride on tensor stride:", list(ik[0]),
+                "kernel stride:", list(kernel_stride))
+    out_ts = [t // int(s) for t, s in zip(ik[0], kernel_stride)]
+    ok, _ = manager._stride_region(in_key, *region, out_ts, out_ts, True, expand_coordinates)
+    out_key.set_key(list(ok[0]), ok[1])
+
+
 def ConvolutionForwardGPU(in_feat, kernel, kernel_size, kernel_stride, kernel_dilation,
                           region_type, offset, expand_coordinates, convolution_mode, in_key,
                           out_key, manager):
@@ -1402,15 +1442,9 @@ def ConvolutionForwardGPU(in_feat, kernel, kernel_size, kernel_stride, kernel_di
     _assert(kernel.is_cuda, "kernel must be CUDA")
     _check_feats(in_feat, manager, in_key)
     _assert(in_feat.size(1) == kernel.size(1), "Input feature size and kernel size mismatch")
-    if not out_key.is_key_set():
-        if expand_coordinates:
-            ik = manager._k(in_key)
-            out_ts = [t * int(s) for t, s in zip(ik[0], kernel_stride)]
-            ok, _ = manager._stride_region(in_key, region_type, kernel_size, kernel_dilation,
-                                           offset, ik[0], out_ts, False, True)
-        else:
-            ok, _ = manager._stride(in_key, kernel_stride)
-        out_key.set_key(list(ok[0]), ok[1])
+    _set_strided_key(manager, in_key, out_key, kernel_stride,
+                     (region_type, kernel_size, kernel_dilation, offset) if expand_coordinates
+                     else None)
     km = manager._kernel_map(in_key, out_key, kernel_size, kernel_stride, kernel_dilation,
                              region_type, offset, False, False)
     return _conv_forward(in_feat, kernel, km)
@@ -1436,15 +1470,9 @@ def ConvolutionTransposeForwardGPU(in_feat, kernel, kernel_size, kernel_stride,
     _assert(kernel.dim() == 3, "kernel.dim():", kernel.dim())
     _check_feats(in_feat, manager, in_key)
     _assert(in_feat.size(1) == kernel.size(1), "Input feature size and kernel size mismatch")
-    if not out_key.is_key_set():
-        ik = manager._k(in_key)
-        for t, s in zip(ik[0], kernel_stride):
-            _assert(t % int(s) == 0, "Invalid up stride on tensor stride:", list(ik[0]),
-                    "kernel stride:", list(kernel_stride))
-        out_ts = [t // int(s) for t, s in zip(ik[0], kernel_stride)]
-        ok, _ = manager._stride_region(in_key, region_type, kernel_size, kernel_dilation, offset,
-                                       out_ts, out_ts, True, generate_new_coordinates)
-        out_key.set_key(list(ok[0]), ok[1])
+    _set_transposed_key(manager, in_key, out_key, kernel_stride,
+                        (region_type, kernel_size, kernel_dilation, offset),
+                        generate_new_coordinates)
     km = manager._kernel_map(in_key, out_key, kernel_size, kernel_stride, kernel_dilation,
                              region_type, offset, True, False)
     return _conv_forward(in_feat, kernel, km)
@@ -1471,9 +1499,7 @@ def LocalPoolingForwardGPU(in_feat, kernel_size, kernel_stride, kernel_dilation,
     local_pooling_cpu.cpp:43-120) -> (out_feat, num_nonzero | max_index)"""
     _check_feats(in_feat, manager, in_key)
     _assert(pooling_mode in _POOL_CODE, "Invalid pooling mode", pooling_mode)
-    if not out_key.is_key_set():
-        ok, _ = manager._stride(in_key, kernel_stride)
-        out_key.set_key(list(ok[0]), ok[1])
+    _set_strided_key(manager, in_key, out_key, kernel_stride)
     km = manager._kernel_map(in_key, out_key, kernel_size, kernel_stride, kernel_dilation,
                              region_type, offset, False, True)
     lib = _lib.load()
@@ -1523,15 +1549,8 @@ def LocalPoolingTransposeForwardGPU(in_feat, kernel_size, kernel_stride, kernel_
     (use_avg = false): out[o] = sum_k in[out_nbr[k][o]] over the transposed pooling map; the
     second result (num_nonzero) is empty.  Mutates `out_key` when it is unset."""
     _check_feats(in_feat, manager, in_key)
-    if not out_key.is_key_set():
-        ik = manager._k(in_key)
-        for t, s in zip(ik[0], kernel_stride):
-            _assert(t % int(s) == 0, "Invalid up stride on tensor stride:", list(ik[0]),
-                    "kernel stride:", list(kernel_stride))
-        out_ts = [t // int(s) for t, s in zip(ik[0], kernel_stride)]
-        ok, _ = manager._stride_region(in_key, region_type, kernel_size, kernel_dilation, offset,
-                                       out_ts, out_ts, True, expand_coordinates)
-        out_key.set_key(list(ok[0]), ok[1])
+    _set_transposed_key(manager, in_key, out_key, kernel_stride,
+                        (region_type, kernel_size, kernel_dilation, offset), expand_coordinates)
     km = manager._kernel_map(in_key, out_key, kernel_size, kernel_stride, kernel_dilation,
                              region_type, offset, True, True)
     C = in_feat.size(1)
@@ -1582,9 +1601,7 @@ def ChannelwiseConvolutionForwardGPU(in_feat, kernel, kernel_size, kernel_stride
     fp32 [K, C] whatever its dtype.  Mutates `out_key` when it is unset."""
     _check_feats(in_feat, manager, in_key)
     _assert(kernel.is_cuda, "kernel must be CUDA")
-    if not out_key.is_key_set():
-        ok, _ = manager._stride(in_key, kernel_stride)
-        out_key.set_key(list(ok[0]), ok[1])
+    _set_strided_key(manager, in_key, out_key, kernel_stride)
     km = _chwise_map(in_feat, kernel, kernel_size, kernel_stride, kernel_dilation, region_type,
                      offset, in_key, out_key, manager)
     lib = _lib.load()

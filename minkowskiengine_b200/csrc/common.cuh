@@ -66,6 +66,27 @@ struct IntVec {  // small by-value parameter block (tensor strides, etc.)
   int32_t v[MEB200_MAX_NCOLS];
 };
 
+// The ncols - 1 tensor strides of a row width the caller has checked, each positive.
+inline int load_strides(const int32_t *tensor_stride, uint32_t ncols, IntVec *ts) {
+  MEB_CHECK_ARG(tensor_stride != nullptr, "null tensor stride");
+  *ts = IntVec{};
+  for (uint32_t j = 0; j + 1 < ncols; ++j) {
+    MEB_CHECK_ARG(tensor_stride[j] > 0, "tensor stride must be positive (axis %u: %d)", j,
+                  tensor_stride[j]);
+    ts->v[j] = tensor_stride[j];
+  }
+  return MEB200_OK;
+}
+
+// A row-index table for n rows: a power of two of at least 2n slots, or the largest table.
+inline int check_table(const uint32_t *table, uint32_t capacity, uint32_t n) {
+  MEB_CHECK_ARG(table != nullptr && capacity >= 2 && (capacity & (capacity - 1)) == 0,
+                "capacity must be a power of two (got %u)", capacity);
+  MEB_CHECK_ARG((uint64_t)capacity >= 2ull * n || capacity == 0x80000000u,
+                "table too small for %u rows", n);
+  return MEB200_OK;
+}
+
 template <int NC>
 struct Coord {
   int32_t c[NC];

@@ -250,27 +250,22 @@ k_find(const int32_t *__restrict__ map_coords, const uint32_t *__restrict__ tabl
 
 uint32_t *insert_flag_word(void *scratch, uint32_t n) { return carve(scratch, n).total + 1; }
 
-int insert_and_map(const int32_t *coords, const uint8_t *valid, uint32_t n, uint32_t ncols,
-                   uint32_t *table, uint32_t capacity, int32_t *unique_coords,
-                   int64_t *unique_index, int64_t *inverse_map, void *scratch,
-                   uint32_t *h_num_unique, uint32_t h_words, cudaStream_t stream) {
-  MEB_CHECK_ARG(h_num_unique != nullptr, "h_num_unique");
-  MEB_CHECK_ARG(table != nullptr && capacity >= 2 && (capacity & (capacity - 1)) == 0,
-                "capacity must be a power of two (got %u)", capacity);
-  MEB_CHECK_ARG((uint64_t)capacity >= 2ull * n || capacity == 0x80000000u,
-                "table too small for %u rows", n);
-  MEB_CUDA(cudaMemsetAsync(table, 0xFF, (size_t)capacity * 4, stream));
-  if (n == 0) {
-    *h_num_unique = 0;
-    return MEB200_OK;
-  }
+// Enqueues the insert of n > 0 candidate rows; the unique count is left in the scratch
+// (carve(scratch, n).total).  d_n: the number of meaningful rows when it lives on the device.
+static int enqueue_insert(const int32_t *coords, const uint8_t *valid, const uint32_t *d_n,
+                          uint32_t n, uint32_t ncols, uint32_t *table, uint32_t capacity,
+                          int32_t *unique_coords, int64_t *unique_index, int64_t *inverse_map,
+                          void *scratch, cudaStream_t stream) {
+  int rc = check_table(table, capacity, n);
+  if (rc != MEB200_OK) return rc;
   MEB_CHECK_ARG(coords && unique_coords && unique_index && inverse_map && scratch, "null buffer");
+  MEB_CUDA(cudaMemsetAsync(table, 0xFF, (size_t)capacity * 4, stream));
   InsertScratch s = carve(scratch, n);
   uint32_t nb = scan_blocks(n);
   MEB_CUDA(cudaMemsetAsync(s.ticket, 0, 8, stream));
   uint32_t mask = capacity - 1;
   MEB_DISPATCH_NCOLS(ncols, k_insert<NC><<<cdiv(n, 256), 256, 0, stream>>>(
-                                coords, valid, nullptr, n, table, mask, s.slot_of));
+                                coords, valid, d_n, n, table, mask, s.slot_of));
   MEB_LAUNCH_OK();
   k_count<<<nb, kScanThreads, 0, stream>>>(table, s.slot_of, n, s.block_sums, s.ticket, s.total);
   MEB_LAUNCH_OK();
@@ -280,18 +275,42 @@ int insert_and_map(const int32_t *coords, const uint8_t *valid, uint32_t n, uint
   MEB_LAUNCH_OK();
   k_inverse<<<cdiv(n, 256), 256, 0, stream>>>(table, s.slot_of, s.rank_of, n, inverse_map);
   MEB_LAUNCH_OK();
-  MEB_CUDA(cudaMemcpyAsync(h_num_unique, s.total, 4 * h_words, cudaMemcpyDeviceToHost, stream));
+  return MEB200_OK;
+}
+
+// Table over m rows known to be distinct.
+static int build_table(const int32_t *coords, uint32_t m, uint32_t ncols, uint32_t *table,
+                       uint32_t capacity, cudaStream_t stream) {
+  int rc = check_table(table, capacity, m);
+  if (rc != MEB200_OK) return rc;
+  MEB_CUDA(cudaMemsetAsync(table, 0xFF, (size_t)capacity * 4, stream));
+  if (m == 0) return MEB200_OK;
+  MEB_CHECK_ARG(coords != nullptr, "null coordinates");
+  MEB_DISPATCH_NCOLS(ncols, k_insert_unique<NC><<<cdiv(m, 256), 256, 0, stream>>>(
+                                coords, m, table, capacity - 1));
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
+}
+
+int insert_and_map(const int32_t *coords, const uint8_t *valid, uint32_t n, uint32_t ncols,
+                   uint32_t *table, uint32_t capacity, int32_t *unique_coords,
+                   int64_t *unique_index, int64_t *inverse_map, void *scratch,
+                   uint32_t *h_num_unique, uint32_t h_words, cudaStream_t stream) {
+  MEB_CHECK_ARG(h_num_unique != nullptr, "h_num_unique");
+  if (n == 0) {
+    int rc = build_table(nullptr, 0, ncols, table, capacity, stream);
+    if (rc == MEB200_OK) *h_num_unique = 0;
+    return rc;
+  }
+  int rc = enqueue_insert(coords, valid, nullptr, n, ncols, table, capacity, unique_coords,
+                          unique_index, inverse_map, scratch, stream);
+  if (rc != MEB200_OK) return rc;
+  MEB_CUDA(cudaMemcpyAsync(h_num_unique, carve(scratch, n).total, 4 * h_words,
+                           cudaMemcpyDeviceToHost, stream));
   MEB_CUDA(cudaStreamSynchronize(stream));
   uint32_t m = *h_num_unique;
-  if (m != n) {  // duplicates or masked rows: rebuild the table over the compacted rows
-    MEB_CUDA(cudaMemsetAsync(table, 0xFF, (size_t)capacity * 4, stream));
-    if (m > 0) {
-      MEB_DISPATCH_NCOLS(ncols, k_insert_unique<NC><<<cdiv(m, 256), 256, 0, stream>>>(
-                                    unique_coords, m, table, mask));
-      MEB_LAUNCH_OK();
-    }
-  }
-  return MEB200_OK;
+  // duplicates or masked rows: rebuild the table over the compacted rows
+  return m != n ? build_table(unique_coords, m, ncols, table, capacity, stream) : MEB200_OK;
 }
 
 }  // namespace meb200
@@ -327,46 +346,17 @@ int meb200_insert_and_map_enqueue(const int32_t *coords, const uint8_t *valid,
                                   uint32_t *d_num_unique, void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   MEB_CHECK_ARG(d_num_unique != nullptr && n > 0, "enqueue: count pointer / empty input");
-  MEB_CHECK_ARG(table != nullptr && capacity >= 2 && (capacity & (capacity - 1)) == 0,
-                "capacity must be a power of two (got %u)", capacity);
-  MEB_CHECK_ARG((uint64_t)capacity >= 2ull * n || capacity == 0x80000000u,
-                "table too small for %u rows", n);
-  MEB_CHECK_ARG(coords && unique_coords && unique_index && inverse_map && scratch, "null buffer");
-  MEB_CUDA(cudaMemsetAsync(table, 0xFF, (size_t)capacity * 4, stream));
-  InsertScratch s = carve(scratch, n);
-  uint32_t nb = scan_blocks(n);
-  MEB_CUDA(cudaMemsetAsync(s.ticket, 0, 8, stream));
-  uint32_t mask = capacity - 1;
-  MEB_DISPATCH_NCOLS(ncols, k_insert<NC><<<cdiv(n, 256), 256, 0, stream>>>(
-                                coords, valid, d_n, n, table, mask, s.slot_of));
-  MEB_LAUNCH_OK();
-  k_count<<<nb, kScanThreads, 0, stream>>>(table, s.slot_of, n, s.block_sums, s.ticket, s.total);
-  MEB_LAUNCH_OK();
-  MEB_DISPATCH_NCOLS(ncols, k_fill<NC><<<nb, kScanThreads, 0, stream>>>(
-                                coords, table, s.slot_of, n, s.block_sums, s.rank_of,
-                                unique_coords, unique_index));
-  MEB_LAUNCH_OK();
-  k_inverse<<<cdiv(n, 256), 256, 0, stream>>>(table, s.slot_of, s.rank_of, n, inverse_map);
-  MEB_LAUNCH_OK();
-  MEB_CUDA(cudaMemcpyAsync(d_num_unique, s.total, 4, cudaMemcpyDeviceToDevice, stream));
+  int rc = enqueue_insert(coords, valid, d_n, n, ncols, table, capacity, unique_coords,
+                          unique_index, inverse_map, scratch, stream);
+  if (rc != MEB200_OK) return rc;
+  MEB_CUDA(cudaMemcpyAsync(d_num_unique, carve(scratch, n).total, 4, cudaMemcpyDeviceToDevice,
+                           stream));
   return MEB200_OK;
 }
 
 int meb200_map_build_table(const int32_t *unique_coords, uint32_t m, uint32_t ncols,
                            uint32_t *table, uint32_t capacity, void *stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
-  MEB_CHECK_ARG(table != nullptr && capacity >= 2 && (capacity & (capacity - 1)) == 0,
-                "capacity must be a power of two (got %u)", capacity);
-  MEB_CHECK_ARG((uint64_t)capacity >= 2ull * m || capacity == 0x80000000u,
-                "table too small for %u rows", m);
-  MEB_CUDA(cudaMemsetAsync(table, 0xFF, (size_t)capacity * 4, stream));
-  if (m == 0) return MEB200_OK;
-  MEB_CHECK_ARG(unique_coords != nullptr, "null coordinates");
-  uint32_t mask = capacity - 1;
-  MEB_DISPATCH_NCOLS(ncols, k_insert_unique<NC><<<cdiv(m, 256), 256, 0, stream>>>(
-                                unique_coords, m, table, mask));
-  MEB_LAUNCH_OK();
-  return MEB200_OK;
+  return build_table(unique_coords, m, ncols, table, capacity, (cudaStream_t)stream_);
 }
 
 int meb200_stride_coords(const int32_t *coords, uint32_t n, uint32_t ncols,
@@ -374,12 +364,10 @@ int meb200_stride_coords(const int32_t *coords, uint32_t n, uint32_t ncols,
   cudaStream_t stream = (cudaStream_t)stream_;
   MEB_CHECK_ARG(ncols >= 2 && ncols <= MEB200_MAX_NCOLS, "ncols=%u", ncols);
   if (n == 0) return MEB200_OK;
-  MEB_CHECK_ARG(coords && out && out_tensor_stride, "null buffer");
-  IntVec ts{};
-  for (uint32_t j = 0; j + 1 < ncols; ++j) {
-    MEB_CHECK_ARG(out_tensor_stride[j] > 0, "tensor stride must be positive");
-    ts.v[j] = out_tensor_stride[j];
-  }
+  MEB_CHECK_ARG(coords && out, "null buffer");
+  IntVec ts;
+  int rc = load_strides(out_tensor_stride, ncols, &ts);
+  if (rc != MEB200_OK) return rc;
   MEB_DISPATCH_NCOLS(ncols,
                      k_stride_coords<NC><<<cdiv(n, 256), 256, 0, stream>>>(coords, n, ts, out));
   MEB_LAUNCH_OK();
@@ -392,13 +380,11 @@ int meb200_region_coords(const int32_t *coords, uint32_t n, uint32_t ncols,
   cudaStream_t stream = (cudaStream_t)stream_;
   MEB_CHECK_ARG(ncols >= 2 && ncols <= MEB200_MAX_NCOLS, "ncols=%u", ncols);
   if (n == 0 || K == 0) return MEB200_OK;
-  MEB_CHECK_ARG(coords && out && valid && offsets && out_tensor_stride, "null buffer");
+  MEB_CHECK_ARG(coords && out && valid && offsets, "null buffer");
   MEB_CHECK_ARG((uint64_t)n * K < 0xFFFFFFFFull, "n*K too large");
-  IntVec ts{};
-  for (uint32_t j = 0; j + 1 < ncols; ++j) {
-    MEB_CHECK_ARG(out_tensor_stride[j] > 0, "tensor stride must be positive");
-    ts.v[j] = out_tensor_stride[j];
-  }
+  IntVec ts;
+  int rc = load_strides(out_tensor_stride, ncols, &ts);
+  if (rc != MEB200_OK) return rc;
   MEB_DISPATCH_NCOLS(ncols, k_region_coords<NC><<<cdiv((uint64_t)n * K, 256), 256, 0, stream>>>(
                                 coords, n, offsets, K, ts, aligned_only, out, valid));
   MEB_LAUNCH_OK();

@@ -314,18 +314,6 @@ static void interp_launch(const void *F, uint32_t C, const int32_t *rows, const 
                                                                        K, (T *)out);
 }
 
-static int load_strides(const int32_t *tensor_stride, uint32_t ncols, IntVec *ts) {
-  MEB_CHECK_ARG(ncols >= 2 && ncols <= MEB200_MAX_NCOLS, "ncols=%u", ncols);
-  MEB_CHECK_ARG(tensor_stride != nullptr, "null tensor stride");
-  *ts = IntVec{};
-  for (uint32_t j = 0; j + 1 < ncols; ++j) {
-    MEB_CHECK_ARG(tensor_stride[j] > 0, "tensor stride must be positive (axis %u: %d)", j,
-                  tensor_stride[j]);
-    ts->v[j] = tensor_stride[j];
-  }
-  return MEB200_OK;
-}
-
 }  // namespace meb200
 
 using namespace meb200;
@@ -335,6 +323,7 @@ extern "C" {
 int meb200_quantize_field(const float *field, uint32_t n, uint32_t ncols,
                           const int32_t *tensor_stride, int32_t *out, uint32_t *d_bad,
                           void *stream) {
+  MEB_CHECK_ARG(ncols >= 2 && ncols <= MEB200_MAX_NCOLS, "ncols=%u", ncols);
   IntVec ts;
   int rc = load_strides(tensor_stride, ncols, &ts);
   if (rc != MEB200_OK) return rc;
@@ -445,6 +434,7 @@ int meb200_field_expand(const void *g, int dtype, uint32_t M, uint32_t C, const 
 int meb200_interp_map(const float *query, uint32_t n, uint32_t ncols, const int32_t *tensor_stride,
                       const int32_t *map_coords, const uint32_t *table, uint32_t capacity,
                       int32_t *rows, float *weights, void *stream) {
+  MEB_CHECK_ARG(ncols >= 2 && ncols <= MEB200_MAX_NCOLS, "ncols=%u", ncols);
   IntVec ts;
   int rc = load_strides(tensor_stride, ncols, &ts);
   if (rc != MEB200_OK) return rc;

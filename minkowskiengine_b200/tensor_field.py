@@ -204,7 +204,7 @@ class TensorField(Tensor):
         if rec is not None:
             return rec
         if mgr.exists_field_to_sparse(fk, key):
-            rec = mgr._field_maps[(mgr._k(fk), mgr._k(key))]
+            rec = mgr._field_sparse_record(fk, key)
         else:
             # a map this field did not make: the field's stride-1 map composed with the stride map
             # from it to `key` (reference: MinkowskiTensorField.py:408-450)
