@@ -133,11 +133,25 @@ int meb200_map_find(const int32_t *map_coords, const uint32_t *table, uint32_t c
  * y_nbr[k*ny + y] = x (y_nbr must be pre-filled with -1 by the caller).
  * offsets: DEVICE int32 [K, ncols-1] already scaled by dilation * tensor stride.
  * d_num_pairs: optional DEVICE uint32 counter, incremented by the number of hits.
+ *
+ * x_order / y_order (each may be NULL; K <= 32): the TILE ORDER of x_nbr / y_nbr, which
+ * meb200_conv_forward / meb200_conv_backward read to run only the offsets a tile of 128 table rows
+ * reaches.  The mask of row r has bit k set when nbr[k][r] >= 0; rows are stably sorted by mask
+ * (ties keep row order), slot s holds row slot_row[s].  One int32 buffer of
+ * (K + 1) * n + ceil(n / 128) words per table of n rows:
+ *   [0, K n)             the table in slot order, k-major: [k][s] = nbr[k][slot_row[s]]
+ *   [K n, (K + 1) n)     slot_row
+ *   [(K + 1) n, ...)     uint32 mask of tile t = OR of the masks of slots [128 t, 128 t + 128)
+ * Both orders asked for are written whenever K > 0, also when nx = 0 (y_nbr is then all -1 and
+ * its order the identity with empty tile masks).
+ * order_scratch: 4 * (2 m + 256 * ceil(m / 2048) + 256) bytes, m = the larger n of the orders
+ * asked for (required when one is).  Deterministic: no atomics decide an order.
  */
 int meb200_kernel_map(const int32_t *x_coords, uint32_t nx, const int32_t *y_coords,
                       uint32_t ny, const uint32_t *y_table, uint32_t y_capacity,
                       uint32_t ncols, const int32_t *offsets, uint32_t K, int32_t *x_nbr,
-                      int32_t *y_nbr, uint32_t *d_num_pairs, void *stream);
+                      int32_t *y_nbr, uint32_t *d_num_pairs, int32_t *x_order, int32_t *y_order,
+                      void *order_scratch, void *stream);
 
 /* Compacted pair lists of a neighbour table — the reference's own kernel-map representation
  * (gpu_kernel_map::in_maps / out_maps per offset, src/kernel_map.cuh:48-429; what
@@ -166,11 +180,13 @@ int meb200_kernel_map_pairs(const int32_t *nbr, uint32_t K, uint32_t n_rows, uin
  *   w_t     [K, Cout, Cin]  the same, transposed per offset (BF16/F16: required; F32: not read)
  * Both come from meb200_conv_pack_weights.  The call runs the tensor cores on w_t when the shape
  * qualifies, otherwise the small-cin or SIMT kernels on w_cast.
+ * out_order (may be NULL): the tile order of out_nbr from meb200_kernel_map; the tensor-core
+ * kernel then runs only the offsets each tile of 128 output rows reaches (read when K <= 32).
  */
 int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
                         const void *w_cast, const void *w_t, uint32_t K, uint32_t c_out,
                         const int32_t *out_nbr, uint32_t n_out, void *out, int out_dtype,
-                        void *stream);
+                        const int32_t *out_order, void *stream);
 
 /* grad_in[i,:] = sum_k grad_out[in_nbr[k,i],:] @ W[k]^T   (fully written)
  * grad_weight[k] = sum_o in[out_nbr[k,o],:]^T @ grad_out[o,:]   (fully written, fp32)
@@ -182,14 +198,16 @@ int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_
  * workspace: meb200_conv_workspace_bytes(n_out, c_in, c_out, K, dtype) bytes, 16-byte aligned.
  * Every wgrad kernel stores its row splits' partial sums there and adds them in split order (no
  * atomics: bit-identical run to run).  It runs as many of its planned splits as the workspace
- * holds; less, NULL or unaligned is legal and means fewer splits, down to one. */
+ * holds; less, NULL or unaligned is legal and means fewer splits, down to one.
+ * in_order (may be NULL): the tile order of in_nbr from meb200_kernel_map, read by the tensor-core
+ * dgrad as out_order by meb200_conv_forward. */
 int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32_t n_in,
                          uint32_t c_in, const void *w_cast, uint32_t K, uint32_t c_out,
                          const int32_t *out_nbr, const int32_t *in_nbr, uint32_t n_out,
                          void *grad_in, int grad_in_dtype, float *grad_weight,
                          const int32_t *pairs_in, const int32_t *pairs_out,
                          const int32_t *seg_start, uint32_t n_chunks, void *workspace,
-                         uint64_t workspace_bytes, void *stream);
+                         uint64_t workspace_bytes, const int32_t *in_order, void *stream);
 
 /* 1 when meb200_conv_backward's wgrad reads pair lists for this layer (so a caller builds them
  * only then), else 0. */

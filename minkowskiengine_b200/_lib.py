@@ -41,11 +41,12 @@ PROTOTYPES = {
                                     _vp, _vp, _vp]),
     "meb200_map_find": (_i32, [_vp, _vp, _u32, _u32, _vp, _u32, _vp, _vp]),
     "meb200_kernel_map": (_i32, [_vp, _u32, _vp, _u32, _vp, _u32, _u32, _vp, _u32, _vp, _vp,
-                                 _vp, _vp]),
+                                 _vp, _vp, _vp, _vp, _vp]),
     "meb200_conv_forward": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _u32, _vp,
-                                   _i32, _vp]),
+                                   _i32, _vp, _vp]),
     "meb200_conv_backward": (_i32, [_vp, _vp, _i32, _u32, _u32, _vp, _u32, _u32, _vp, _vp,
-                                    _u32, _vp, _i32, _vp, _vp, _vp, _vp, _u32, _vp, _u64, _vp]),
+                                    _u32, _vp, _i32, _vp, _vp, _vp, _vp, _u32, _vp, _u64, _vp,
+                                    _vp]),
     "meb200_conv_wgrad_uses_pairs": (_i32, [_i32, _u32, _u32, _u32]),
     "meb200_conv_pack_weights": (_i32, [_vp, _u32, _u32, _u32, _i32, _vp, _vp, _vp]),
     "meb200_conv_pack_weights_batched": (_i32, [_vp, _u32, _u32, _i32, _vp]),
@@ -108,7 +109,22 @@ PROTOTYPES = {
                                               C.c_uint64, _u32, _u32, _u32, _vp, _vp, _vp, _vp]),
 }
 
+# meb200_conv_backward gained its `in_order` pointer just before the stream.  Callers written
+# against the argument list it had before (the direct-call test helper among them) still work: a
+# call one argument short gets NULL there (no order: every tile runs every offset).  Any other
+# argument count goes to ctypes unchanged and fails there.  The backend passes the full list.
+_ORDER_ADDED = ("meb200_conv_backward",)
+
 _lib = None
+
+
+def _order_optional(fn, n_args):
+    def call(*args):
+        if len(args) == n_args - 1:
+            args = args[:-1] + (None, args[-1])
+        return fn(*args)
+    call.argtypes, call.restype = fn.argtypes, fn.restype
+    return call
 
 
 class BackendError(RuntimeError):
@@ -130,6 +146,8 @@ def load():
         fn = getattr(lib, name)  # AttributeError -> loud failure on a stale library
         fn.restype = res
         fn.argtypes = args
+    for name in _ORDER_ADDED:
+        setattr(lib, name, _order_optional(getattr(lib, name), len(PROTOTYPES[name][1])))
     _lib = lib
     return lib
 

@@ -375,13 +375,13 @@ class _KernelMap:
     `swapped()` is the reference's swap_in_out (kernel_map.cuh:191-241)."""
 
     __slots__ = ("out_nbr", "_in_nbr", "_in_thunk", "_n_in", "stride_pairs", "_n_pairs", "_pairs",
-                 "_pair_src", "_hint_key")
+                 "_pair_src", "_hint_key", "out_order", "in_order")
     PAIR_STAGE = 64   # pairs per pipeline stage of the wgrad kernel (k_wgrad_wg)
     # table rows per chunk of the pair lists (multiple of 2048): one chunk's rows of both feature
     # matrices stay L2-resident while the wgrad walks its K offsets
     PAIR_CHUNK_ROWS = 262144
 
-    def __init__(self, out_nbr, in_nbr, stride_pairs=None, n_in=None, in_thunk=None):
+    def __init__(self, out_nbr, in_nbr, stride_pairs=None, n_in=None, in_thunk=None, orders=None):
         # in_nbr may be None with (n_in, in_thunk): the reverse table of a large kernel (the
         # K = 125 stem: 400 MB at 800k rows) is only built if somebody asks for it — dgrad or a
         # transposed layer; the stem of a network needs neither
@@ -392,6 +392,9 @@ class _KernelMap:
         self._pairs = None      # (pairs_in, pairs_out, seg_start) once built
         self._pair_src = None   # the map this one is the swapped view of
         self._hint_key = None   # the manager's cache key (prediction of the next manager's needs)
+        # tile orders of out_nbr / in_nbr (meb200_kernel_map, include/meb200.h) or None: the
+        # forward reads the first, the dgrad the second
+        self.out_order, self.in_order = orders if orders is not None else (None, None)
 
     def pair_lists(self):
         """(pairs_in, pairs_out, seg_start, n_chunks): compacted (input row, output row) lists in
@@ -452,7 +455,7 @@ class _KernelMap:
 
     def swapped(self):
         sp = None if self.stride_pairs is None else (self.stride_pairs[1], self.stride_pairs[0])
-        km = _KernelMap(self.in_nbr, self.out_nbr, sp)
+        km = _KernelMap(self.in_nbr, self.out_nbr, sp, orders=(self.in_order, self.out_order))
         km._n_pairs = self._n_pairs
         km._pair_src = self
         return km
@@ -471,6 +474,19 @@ class _KernelMap:
                 o = torch.nonzero(hit[k]).flatten()
                 out[k] = torch.stack([self.out_nbr[k, o], o.int()])
         return out
+
+
+MAX_ORDER_K = 32     # tile orders are built for convolution tables of 2..32 offsets
+
+
+def tile_order_words(K, n):
+    """int32 words of the tile order of a [K, n] table (include/meb200.h, meb200_kernel_map)."""
+    return (K + 1) * n + (n + 127) // 128
+
+
+def tile_order_scratch_bytes(n):
+    """Scratch bytes meb200_kernel_map needs to build the tile orders of tables of up to n rows."""
+    return 4 * (2 * n + 256 * ((n + 2047) // 2048) + 256)
 
 
 _OFFSET_CACHE = {}
@@ -630,21 +646,30 @@ class CoordinateMapManagerGPU_c10:
     LAZY_REVERSE_K = 64      # kernels this large get their reverse table on demand
 
     @staticmethod
-    def _probe(x_map, y_map, offsets, need_y=True):
-        """x-stationary probe: returns (x_nbr [K,nx], y_nbr [K,ny] or None).  (Static: the deferred
-        reverse-table build below must not keep the manager alive through a reference cycle —
-        a manager owns ~1.5 GB of tables on the bench clouds and should die with its tensors.)"""
+    def _probe(x_map, y_map, offsets, need_y=True, orders=False):
+        """x-stationary probe: returns (x_nbr [K,nx], y_nbr [K,ny] or None), and with `orders` (and
+        y) also the tile orders of both tables, (x_order, y_order) or (None, None) where K is
+        outside 2..MAX_ORDER_K.  (Static: the deferred reverse-table build below must not keep the
+        manager alive through a reference cycle — a manager owns ~1.5 GB of tables on the bench
+        clouds and should die with its tensors.)"""
         lib = _lib.load()
         K = offsets.shape[0]
         dev = x_map.coords.device
         x_nbr = torch.empty((K, x_map.size), dtype=torch.int32, device=dev)
         y_nbr = torch.full((K, y_map.size), -1, dtype=torch.int32, device=dev) if need_y else None
+        x_order = y_order = scratch = None
+        if orders and need_y and 2 <= K <= MAX_ORDER_K:
+            x_order = torch.empty(tile_order_words(K, x_map.size), dtype=torch.int32, device=dev)
+            y_order = torch.empty(tile_order_words(K, y_map.size), dtype=torch.int32, device=dev)
+            scratch = torch.empty(tile_order_scratch_bytes(max(x_map.size, y_map.size)),
+                                  dtype=torch.uint8, device=dev)
 
         def launch():
             _lib.check(lib.meb200_kernel_map(
                 _lib.ptr(x_map.coords), x_map.size, _lib.ptr(y_map.coords), y_map.size,
                 _lib.ptr(y_map.table), y_map.capacity, x_map.ncols, _lib.ptr(offsets), K,
-                _lib.ptr(x_nbr), _lib.ptr(y_nbr), None, _lib.current_stream()))
+                _lib.ptr(x_nbr), _lib.ptr(y_nbr), None, _lib.ptr(x_order), _lib.ptr(y_order),
+                _lib.ptr(scratch), _lib.current_stream()))
         if _PROFILE is not None:
             # algorithmic bytes (SURVEY.md 8d): coordinate rows read once, one 4-byte table slot
             # + one coordinate row compared per probe, both neighbour tables written
@@ -655,6 +680,8 @@ class CoordinateMapManagerGPU_c10:
             _record("kernel_map", launch, probes, nbytes, always=True)
         else:
             launch()
+        if orders:
+            return x_nbr, y_nbr, x_order, y_order
         return x_nbr, y_nbr
 
     def _kernel_map(self, in_key, out_key, kernel_size, kernel_stride, kernel_dilation,
@@ -692,8 +719,8 @@ class CoordinateMapManagerGPU_c10:
                     km = _KernelMap(out_nbr, None, n_in=in_map.size,
                                     in_thunk=lambda: probe(out_map, in_map, offs)[1])
                 else:
-                    out_nbr, in_nbr = self._probe(out_map, in_map, offs)
-                    km = _KernelMap(out_nbr, in_nbr)
+                    out_nbr, in_nbr, *orders = self._probe(out_map, in_map, offs, orders=not is_pool)
+                    km = _KernelMap(out_nbr, in_nbr, orders=orders or None)
         else:
             swapped_key = (ok, ik, ksize, kstride, kdil, region_type, False, bool(is_pool))
             fwd = self._kernel_maps.get(swapped_key)
@@ -708,8 +735,8 @@ class CoordinateMapManagerGPU_c10:
                 else:
                     offs = _device_offsets(region_type, ksize, kdil, out_map.tensor_stride,
                                            custom, dev)
-                    a, b = self._probe(in_map, out_map, offs)
-                    fwd = _KernelMap(a, b)
+                    a, b, *orders = self._probe(in_map, out_map, offs, orders=not is_pool)
+                    fwd = _KernelMap(a, b, orders=orders or None)
                 fwd._hint_key = swapped_key
                 self._kernel_maps[swapped_key] = fwd
             km = fwd.swapped()
@@ -1336,7 +1363,7 @@ def _conv_forward_impl(in_feat, kernel, km, out_dtype=None):
     _lib.check(lib.meb200_conv_forward(
         _lib.ptr(in_feat), code, km.n_in, c_in, _lib.ptr(w_cast), _lib.ptr(w_t), K, c_out,
         _lib.ptr(km.out_nbr), km.n_out, _lib.ptr(out), _lib.dtype_code(out.dtype),
-        _lib.current_stream()))
+        _lib.ptr(km.out_order), _lib.current_stream()))
     return out
 
 
@@ -1397,7 +1424,7 @@ def _conv_backward_impl(in_feat, grad_out, kernel, km, need_in=True, need_w=True
         _lib.ptr(in_feat), _lib.ptr(grad_out), code, n_in, c_in, _lib.ptr(w_cast), K, c_out,
         _lib.ptr(km.out_nbr), _lib.ptr(km.in_nbr) if need_in else None, n_out, _lib.ptr(grad_in),
         code, _lib.ptr(grad_w), _lib.ptr(pin), _lib.ptr(pout), _lib.ptr(seg), nch, _lib.ptr(ws),
-        ws_bytes, _lib.current_stream()))
+        ws_bytes, _lib.ptr(km.in_order) if need_in else None, _lib.current_stream()))
     if grad_w is not None and grad_w.dtype != kernel.dtype:
         grad_w = grad_w.to(kernel.dtype)
     return grad_in, grad_w

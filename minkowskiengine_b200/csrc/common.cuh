@@ -52,6 +52,12 @@ inline unsigned cdiv(uint64_t a, uint64_t b) { return (unsigned)((a + b - 1) / b
 
 int num_sms();
 
+// ---- tile order of a neighbour table [K, n] (built by meb200_kernel_map, read by the forward /
+// dgrad kernel; layout in kernel_map.cu and include/meb200.h): one int32 buffer holding the table
+// in slot order [K][n], slot -> row [n] and one mask per 128-row tile [ceil(n / 128)].
+constexpr uint32_t kOrderTileRows = 128;
+constexpr uint32_t kMaxOrderK = 32;
+
 // The deduplicating insert behind meb200_insert_and_map (coords.cu).  Its one blocking read copies
 // h_words words to the host: the unique count, and with h_words = 2 the word beside it in the
 // scratch (insert_flag_word), which kernels enqueued before the insert may set.

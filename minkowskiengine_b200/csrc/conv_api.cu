@@ -26,7 +26,7 @@ int meb200_conv_wgrad_uses_pairs(int dtype, uint32_t c_in, uint32_t c_out, uint3
 int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
                         const void *w_cast, const void *w_t, uint32_t K, uint32_t c_out,
                         const int32_t *out_nbr, uint32_t n_out, void *out, int out_dtype,
-                        void *stream_) {
+                        const int32_t *out_order, void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (n_out == 0) return MEB200_OK;
   MEB_CHECK_ARG(in_dtype >= 0 && in_dtype <= 2 && out_dtype >= 0 && out_dtype <= 2, "dtype");
@@ -36,8 +36,8 @@ int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_
                 "null buffer");
   MEB_CHECK_ARG(c_in > 0 && c_out > 0 && K > 0, "empty channel/kernel dims");
   if (conv_tc_supported(in_dtype, c_in, c_out)) {
-    int rc = conv_forward_tc(in, in_dtype, n_in, c_in, w_t, K, c_out, out_nbr, n_out, out,
-                             out_dtype, stream);
+    int rc = conv_forward_tc(in, in_dtype, n_in, c_in, w_t, K, c_out, out_nbr, out_order, n_out,
+                             out, out_dtype, stream);
     if (rc != MEB200_ERR_UNSUPPORTED) return rc;
   }
   if (conv_small_cin_supported(c_in, c_out)) {
@@ -106,7 +106,7 @@ int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32
                          void *grad_in, int grad_in_dtype, float *grad_weight,
                          const int32_t *pairs_in, const int32_t *pairs_out,
                          const int32_t *seg_start, uint32_t n_chunks, void *workspace,
-                         uint64_t workspace_bytes, void *stream_) {
+                         uint64_t workspace_bytes, const int32_t *in_order, void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   MEB_CHECK_ARG(dtype >= 0 && dtype <= 2, "dtype");
   MEB_CHECK_ARG(grad_in_dtype == MEB200_F32 || grad_in_dtype == dtype,
@@ -118,8 +118,8 @@ int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32
     // rows = input rows, reduction over c_out, produces c_in columns.
     int rc = MEB200_ERR_UNSUPPORTED;
     if (conv_tc_supported(dtype, c_out, c_in))
-      rc = conv_forward_tc(grad_out, dtype, n_out, c_out, w_cast, K, c_in, in_nbr, n_in, grad_in,
-                           grad_in_dtype, stream);
+      rc = conv_forward_tc(grad_out, dtype, n_out, c_out, w_cast, K, c_in, in_nbr, in_order, n_in,
+                           grad_in, grad_in_dtype, stream);
     if (rc == MEB200_ERR_UNSUPPORTED)
       rc = conv_forward_simt(grad_out, dtype, n_out, c_out, w_cast, K, c_in, /*trans_w=*/true,
                              in_nbr, n_in, grad_in, grad_in_dtype, stream);

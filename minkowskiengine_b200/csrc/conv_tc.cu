@@ -72,6 +72,10 @@ struct FwdParams {
   uint32_t n_a;           // rows of A (gather indices >= n_a read as zero rows)
   uint32_t out_ld, bk, out_f32;
   uint32_t stem_K;        // > 0: network stem, virtual channel 4 k + c = A[nbr[k][r]][c], k < stem_K
+  // tile order (meb200_kernel_map, K <= 32), or both NULL: nbr is then the table in slot order,
+  // tile t runs the offsets of tile_mask[t] and writes slot s to row slot_row[s]
+  const int32_t *slot_row;
+  const uint32_t *tile_mask;
 };
 
 // NT wgmma instructions of N = NI columns each cover the c_cols = NI * NT columns of the slice.
@@ -83,14 +87,22 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
   const uint32_t row0 = blockIdx.x * tc::kFwdRows;
   const uint32_t bk = p.bk, ch = bk / 8, lch = bk == 64 ? 3 : (bk == 32 ? 2 : 1);
   const uint32_t a_bytes = tc::kFwdRows * bk * 2, stage_bytes = a_bytes + p.c_cols * bk * 2;
-  const uint32_t nch = p.c_red / bk, n_st = p.K * nch;
+  const bool ordered = p.tile_mask != nullptr;
+  const uint32_t tmask = ordered ? __ldg(p.tile_mask + blockIdx.x) : 0u;
+  const uint32_t nch = p.c_red / bk, n_st = (ordered ? __popc(tmask) : p.K) * nch;
   const T *A = reinterpret_cast<const T *>(p.A);
   const T *B = reinterpret_cast<const T *>(p.B);
   const uint32_t ar = tid >> 1, arow = row0 + ar;     // two threads per tile row of A
   const bool row_ok = arow < p.n_rows;
 
+  // producer cursor: offset ld_k (the set bits of tmask in ascending order when ordered), chunk ld_c
+  uint32_t ld_rem = tmask, ld_k = ordered ? __ffs(tmask) - 1 : 0, ld_c = 0;
   auto load = [&](uint32_t s) {
-    const uint32_t k = s / nch, c0 = (s - k * nch) * bk;
+    const uint32_t k = ld_k, c0 = ld_c * bk;
+    if (++ld_c == nch) {
+      ld_c = 0;
+      if (ordered) { ld_rem &= ld_rem - 1; ld_k = __ffs(ld_rem) - 1; } else ++ld_k;
+    }
     const uint32_t base = s0 + (s % kStages) * stage_bytes;
     if (p.stem_K == 0) {
       const int32_t src = row_ok ? __ldg(p.nbr + (size_t)k * p.n_rows + arow) : -1;
@@ -154,6 +166,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
   for (int h = 0; h < 2; ++h) {
     const uint32_t r = rbase + 8 * h;
     if (r >= p.n_rows) continue;
+    const uint32_t orow = p.slot_row != nullptr ? (uint32_t)__ldg(p.slot_row + r) : r;
 #pragma unroll
     for (int i = 0; i < NT; ++i)
 #pragma unroll
@@ -161,10 +174,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
         const uint32_t col = i * NI + 8 * j + 2 * t;
         const float v0 = acc[i][4 * j + 2 * h], v1 = acc[i][4 * j + 2 * h + 1];
         if (p.out_f32)
-          *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + (size_t)r * p.out_ld + col) =
+          *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + (size_t)orow * p.out_ld + col) =
               make_float2(v0, v1);
         else
-          *reinterpret_cast<uint32_t *>(reinterpret_cast<T *>(p.out) + (size_t)r * p.out_ld + col) =
+          *reinterpret_cast<uint32_t *>(reinterpret_cast<T *>(p.out) + (size_t)orow * p.out_ld + col) =
               pack2<T>(v0, v1);
       }
   }
@@ -512,9 +525,11 @@ bool conv_tc_supported(int dtype, uint32_t c_reduce, uint32_t c_cols) {
   return c_cols % 16 == 0 && c_cols >= 16 && c_cols <= 1024;
 }
 
+static_assert(tc::kFwdRows == kOrderTileRows, "a tile order's tiles are the kernel's row tiles");
+
 int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *B,
-                    uint32_t K, uint32_t c_cols, const int32_t *nbr, uint32_t n_rows, void *out,
-                    int out_dtype, cudaStream_t stream) {
+                    uint32_t K, uint32_t c_cols, const int32_t *nbr, const int32_t *order,
+                    uint32_t n_rows, void *out, int out_dtype, cudaStream_t stream) {
   if (n_rows == 0) return MEB200_OK;
   MEB_CHECK_ARG(conv_tc_supported(dtype, c_reduce, c_cols), "shape not supported by tc path");
   if (!aligned(16, A, B)) {
@@ -522,11 +537,16 @@ int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, c
     return MEB200_ERR_UNSUPPORTED;
   }
   const uint8_t *Wb = reinterpret_cast<const uint8_t *>(B);
+  const bool ordered = order != nullptr && K <= kMaxOrderK;
   // one launch per slice of <= 256 output columns
   const size_t out_esz = out_dtype == MEB200_F32 ? 4 : 2;
   for (uint32_t n0 = 0; n0 < c_cols; n0 += tc::kMaxCols) {
     FwdParams p{};
-    p.A = A; p.B = Wb + (size_t)n0 * c_reduce * 2; p.nbr = nbr;
+    p.A = A; p.B = Wb + (size_t)n0 * c_reduce * 2; p.nbr = ordered ? order : nbr;
+    if (ordered) {
+      p.slot_row = order + (size_t)K * n_rows;
+      p.tile_mask = reinterpret_cast<const uint32_t *>(order + (size_t)(K + 1) * n_rows);
+    }
     p.out = reinterpret_cast<uint8_t *>(out) + (size_t)n0 * out_esz;
     p.b_k_stride = (uint64_t)c_cols * c_reduce;
     p.c_red = c_reduce; p.c_cols = c_cols - n0 < tc::kMaxCols ? c_cols - n0 : tc::kMaxCols;

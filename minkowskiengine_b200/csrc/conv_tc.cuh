@@ -10,9 +10,11 @@ bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out);
 
 // out[r,:] = sum_k A[nbr[k][r],:] @ B[k]^T with B [K, c_cols, c_reduce] (reduction contiguous):
 // the forward passes w_t [K, c_out, c_in], the dgrad the layer's w_cast [K, c_in, c_out].
+// order (may be NULL; read when K <= 32): the tile order of nbr from meb200_kernel_map, so that
+// each 128-row tile runs only the offsets its rows reach.
 int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *B,
-                    uint32_t K, uint32_t c_cols, const int32_t *nbr, uint32_t n_rows, void *out,
-                    int out_dtype, cudaStream_t stream);
+                    uint32_t K, uint32_t c_cols, const int32_t *nbr, const int32_t *order,
+                    uint32_t n_rows, void *out, int out_dtype, cudaStream_t stream);
 
 // fp32 W[K,c_in,c_out] -> w_cast [K,c_in,c_out] and w_t [K,c_out,c_in] in bf16/fp16.
 int conv_pack_weights(const float *W, uint32_t K, uint32_t c_in, uint32_t c_out, int dtype,

@@ -41,6 +41,7 @@ def main():
     for _ in range(3):
         step()
     torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(3):
@@ -48,6 +49,7 @@ def main():
     e1.record()
     torch.cuda.synchronize()
     print(f"step time (no profiler): {e0.elapsed_time(e1) / 3:.2f} ms")
+    print(f"peak memory allocated in a step: {torch.cuda.max_memory_allocated() / 2**20:.0f} MiB")
     with profile(activities=[ProfilerActivity.CUDA, ProfilerActivity.CPU]) as prof:
         step()
         torch.cuda.synchronize()
