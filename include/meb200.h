@@ -40,6 +40,18 @@ extern "C" {
 #define MEB200_F32 0
 #define MEB200_BF16 1
 #define MEB200_F16 2
+/* fp32 storage, TF32 tensor-core math: the operand code of an fp32 convolution whose caller allows
+ * TF32 (torch.backends.cuda.matmul.fp32_precision == "tf32").  Accepted by meb200_conv_forward,
+ * meb200_conv_backward, the weight packing calls, meb200_conv_workspace_bytes and
+ * meb200_conv_wgrad_uses_pairs; features, outputs and grad_in are fp32 (outputs and grad_in
+ * MEB200_F32).  Rounding: the packed weights are rounded to tf32 (10 explicit mantissa bits) to
+ * nearest, ties away from zero; features and gradients are read as stored and the tensor cores
+ * truncate them to tf32 (observed on the H100); products are accumulated in fp32.  Grid: forward and dgrad run on the
+ * tensor cores when the reduction width (c_in forward, c_out dgrad) is a multiple of 8 and the
+ * output width a multiple of 16 and <= 1024; the weight gradient when c_in is a multiple of 8
+ * (>= 16) and c_out a multiple of 16 in [16, 256].  Any other shape runs the fp32 CUDA-core
+ * kernels (on the packed, tf32-rounded weights in forward and dgrad). */
+#define MEB200_TF32 3
 
 #define MEB200_MAX_NCOLS 8 /* D+1 <= 8, i.e. up to 7 spatial/temporal axes */
 
@@ -176,8 +188,9 @@ int meb200_kernel_map_pairs(const int32_t *nbr, uint32_t K, uint32_t n_rows, uin
  * out[o,:] = sum_k in[out_nbr[k,o],:] @ W[k]          (rows with out_nbr = -1 skipped)
  * Output is fully written (no pre-zeroing needed, no atomics, deterministic).
  * in_dtype: dtype of `in`, `w_cast` and `w_t`; out_dtype: dtype of `out` (F32 always allowed).
+ * TF32: fp32 `in`, `w_cast` and `w_t` from meb200_conv_pack_weights(..., MEB200_TF32, ...), F32 out.
  *   w_cast  [K, Cin, Cout]  the weights in the feature dtype
- *   w_t     [K, Cout, Cin]  the same, transposed per offset (BF16/F16: required; F32: not read)
+ *   w_t     [K, Cout, Cin]  the same, transposed per offset (BF16/F16/TF32: required; F32: not read)
  * Both come from meb200_conv_pack_weights.  The call runs the tensor cores on w_t when the shape
  * qualifies, otherwise the small-cin or SIMT kernels on w_cast.
  * out_order (may be NULL): the tile order of out_nbr from meb200_kernel_map; the tensor-core
@@ -219,8 +232,8 @@ uint64_t meb200_conv_workspace_bytes(uint32_t n_out, uint32_t c_in, uint32_t c_o
                                      int dtype);
 
 /* Weight packing, once per optimizer step instead of once per call: fp32 master weight
- * [K, Cin, Cout] -> `dtype` (BF16/F16) operand copies w_cast [K, Cin, Cout] and
- * w_t [K, Cout, Cin].  The reference keeps weights in the feature dtype and needs no such step
+ * [K, Cin, Cout] -> `dtype` (BF16/F16, or TF32: fp32 words rounded to tf32) operand copies
+ * w_cast [K, Cin, Cout] and w_t [K, Cout, Cin].  The reference keeps weights in the feature dtype and needs no such step
  * (MinkowskiConvolution.py:264-279); this is the bf16/fp16 operand cache of this backend. */
 int meb200_conv_pack_weights(const float *weight, uint32_t K, uint32_t c_in, uint32_t c_out,
                              int dtype, void *w_cast, void *w_t, void *stream);

@@ -13,6 +13,7 @@ LIB_PATH = os.path.join(_HERE, "csrc", os.environ.get("MEB200_LIB", "libmeb200.s
 
 OK = 0
 F32, BF16, F16 = 0, 1, 2
+TF32 = 3           # fp32 storage, TF32 tensor-core math (convolutions only)
 POOL_SUM, POOL_AVG, POOL_MAX = 0, 1, 2
 SEG_SUM, SEG_AVG, SEG_MAX = 0, 1, 2
 BCAST_ADD, BCAST_MUL, BCAST_COPY, BCAST_MAXGRAD = 0, 1, 2, 3
@@ -159,9 +160,10 @@ def check(rc):
 
 
 def dtype_code(torch_dtype):
+    """Code of a feature dtype, or of the convolution operand type "tf32" (backend._operand)."""
     import torch
     try:
-        return {torch.float32: F32, torch.bfloat16: BF16, torch.float16: F16}[torch_dtype]
+        return {torch.float32: F32, torch.bfloat16: BF16, torch.float16: F16, "tf32": TF32}[torch_dtype]
     except KeyError:
         raise BackendError(
             f"unsupported feature dtype {torch_dtype}: this backend computes in "

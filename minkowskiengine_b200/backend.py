@@ -1179,7 +1179,10 @@ def _conv_forward(in_feat, kernel, km, out_dtype=None):
 
 
 # ---- packed weights: one cast + transpose per optimizer step, not per call -------------------
-_PACKED = {}   # id(kernel tensor) -> (weakref, version, data_ptr, dtype, (w_cast, w_t))
+# An "operand" is what the convolution kernels multiply: a feature dtype, or TF32 (fp32 features,
+# tf32 tensor-core math, fp32 packed weights rounded to tf32).
+TF32 = "tf32"
+_PACKED = {}   # id(kernel tensor) -> (weakref, version, data_ptr, operand, (w_cast, w_t))
 _ERR_UNSUPPORTED = -3
 
 
@@ -1189,8 +1192,23 @@ class _PackJob(ctypes.Structure):      # == meb200_pack_job (include/meb200.h)
                 ("tile_begin", ctypes.c_uint32)]
 
 
+def _operand(feat_dtype):
+    """The operand of a convolution over `feat_dtype` features: TF32 for fp32 features while torch
+    lets fp32 matmuls use TF32, else the dtype itself.  Read at every call, as torch reads its own
+    flag at every matmul.  Only `fp32_precision` is read: it is right after every setter style,
+    while `allow_tf32` and `get_float32_matmul_precision()` raise once the newer API was used."""
+    if feat_dtype == torch.float32 and torch.backends.cuda.matmul.fp32_precision == "tf32":
+        return TF32
+    return feat_dtype
+
+
+def _operand_storage(op):
+    """torch dtype of an operand's packed weights."""
+    return torch.float32 if op == TF32 else op
+
+
 class _PackTable:
-    """Every fp32 convolution kernel of one (device, operand dtype) seen so far, with its packed
+    """Every fp32 convolution kernel of one (device, operand) seen so far, with its packed
     buffers and a DEVICE job table: when the optimizer has stepped, the first layer that notices
     re-packs ALL of them with one launch (meb200_conv_pack_weights_batched) instead of every
     layer paying an allocation, a ctypes call and a launch on the forward pass (55 of them per
@@ -1248,7 +1266,7 @@ class _PackTable:
             _PACKED[key] = (ref, k._version, ptr, self.dtype, packed)
 
 
-_PACK_TABLES = {}      # (device index, dtype) -> _PackTable
+_PACK_TABLES = {}      # (device index, operand) -> _PackTable
 
 
 def _is_master(kernel):
@@ -1266,10 +1284,11 @@ def _cached(key, kernel, dtype):
 
 
 def _packed_weights(kernel, dtype):
-    """(w_cast [K,Cin,Cout], w_t [K,Cout,Cin]) of a floating kernel in `dtype` (the operand-B
-    layouts of dgrad and forward), rebuilt only when the tensor was modified in place (its autograd
-    version counter moved) or replaced.  A kernel that is not an fp32 master is packed alone from
-    an fp32 copy: bf16 / fp16 values pass through fp32 exactly, so the bytes are kernel.to(dtype)."""
+    """(w_cast [K,Cin,Cout], w_t [K,Cout,Cin]) of a floating kernel for operand `dtype` (bf16,
+    fp16 or TF32: the operand-B layouts of dgrad and forward), rebuilt only when the tensor was
+    modified in place (its autograd version counter moved) or replaced.  A kernel that is not an
+    fp32 master is packed alone from an fp32 copy: bf16 / fp16 values pass through fp32 exactly, so
+    the bytes are kernel.to(dtype).  TF32 weights are fp32 words rounded to tf32."""
     key = id(kernel)
     packed = _cached(key, kernel, dtype)
     if packed is not None:
@@ -1287,7 +1306,7 @@ def _packed_weights(kernel, dtype):
     lib = _lib.load()
     K, c_in, c_out = kernel.shape
     src = kernel.detach().float().contiguous()
-    buf = torch.empty((2, K * c_in * c_out), dtype=dtype, device=kernel.device)
+    buf = torch.empty((2, K * c_in * c_out), dtype=_operand_storage(dtype), device=kernel.device)
     w_cast, w_t = buf[0].view(K, c_in, c_out), buf[1].view(K, c_out, c_in)
     _lib.check(lib.meb200_conv_pack_weights(
         _lib.ptr(src), K, c_in, c_out, _lib.dtype_code(dtype), _lib.ptr(w_cast), _lib.ptr(w_t),
@@ -1303,7 +1322,7 @@ def _packed_weights(kernel, dtype):
 
 
 def _feature_weights(kernel, dtype):
-    """(w_cast, w_t) for features of `dtype`; fp32 features read the kernel itself (no w_t)."""
+    """(w_cast, w_t) for operand `dtype`; exact fp32 reads the kernel itself (no w_t)."""
     if dtype == torch.float32:
         return kernel.float().contiguous(), None
     return _packed_weights(kernel, dtype)
@@ -1345,7 +1364,8 @@ def _pad4(feat):
 
 def _conv_forward_impl(in_feat, kernel, km, out_dtype=None):
     lib = _lib.load()
-    code = _lib.dtype_code(in_feat.dtype)
+    op = _operand(in_feat.dtype)
+    code = _lib.dtype_code(op)
     K, c_in, c_out = kernel.shape
     _assert(K == km.K, "kernel volume", K, "does not match the kernel map", km.K)
     out = torch.empty((km.n_out, c_out), dtype=out_dtype or in_feat.dtype, device=in_feat.device)
@@ -1359,7 +1379,7 @@ def _conv_forward_impl(in_feat, kernel, km, out_dtype=None):
         if rc != _ERR_UNSUPPORTED:
             _lib.check(rc)
             return out
-    w_cast, w_t = _feature_weights(kernel, in_feat.dtype)
+    w_cast, w_t = _feature_weights(kernel, op)
     _lib.check(lib.meb200_conv_forward(
         _lib.ptr(in_feat), code, km.n_in, c_in, _lib.ptr(w_cast), _lib.ptr(w_t), K, c_out,
         _lib.ptr(km.out_nbr), km.n_out, _lib.ptr(out), _lib.dtype_code(out.dtype),
@@ -1388,7 +1408,8 @@ def _conv_backward(in_feat, grad_out, kernel, km, need_in=True, need_w=True):
 
 def _conv_backward_impl(in_feat, grad_out, kernel, km, need_in=True, need_w=True):
     lib = _lib.load()
-    code = _lib.dtype_code(in_feat.dtype)
+    op = _operand(in_feat.dtype)
+    code = _lib.dtype_code(op)
     if grad_out.dtype != in_feat.dtype:
         grad_out = grad_out.to(in_feat.dtype)
     grad_out = grad_out.contiguous()
@@ -1410,7 +1431,7 @@ def _conv_backward_impl(in_feat, grad_out, kernel, km, need_in=True, need_w=True
         if rc != _ERR_UNSUPPORTED:
             _lib.check(rc)
             return None, gwv[:K, :c_in].contiguous()
-    w_cast, _ = _feature_weights(kernel, in_feat.dtype)
+    w_cast, _ = _feature_weights(kernel, op)
     pin = pout = seg = None
     nch = 0
     ws, ws_bytes = None, 0
@@ -1423,8 +1444,9 @@ def _conv_backward_impl(in_feat, grad_out, kernel, km, need_in=True, need_w=True
     _lib.check(lib.meb200_conv_backward(
         _lib.ptr(in_feat), _lib.ptr(grad_out), code, n_in, c_in, _lib.ptr(w_cast), K, c_out,
         _lib.ptr(km.out_nbr), _lib.ptr(km.in_nbr) if need_in else None, n_out, _lib.ptr(grad_in),
-        code, _lib.ptr(grad_w), _lib.ptr(pin), _lib.ptr(pout), _lib.ptr(seg), nch, _lib.ptr(ws),
-        ws_bytes, _lib.ptr(km.in_order) if need_in else None, _lib.current_stream()))
+        _lib.dtype_code(in_feat.dtype), _lib.ptr(grad_w), _lib.ptr(pin), _lib.ptr(pout),
+        _lib.ptr(seg), nch, _lib.ptr(ws), ws_bytes, _lib.ptr(km.in_order) if need_in else None,
+        _lib.current_stream()))
     if grad_w is not None and grad_w.dtype != kernel.dtype:
         grad_w = grad_w.to(kernel.dtype)
     return grad_in, grad_w

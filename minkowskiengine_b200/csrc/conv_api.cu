@@ -8,11 +8,14 @@
 
 using namespace meb200;
 
+// dtype of the feature storage: TF32 convolutions keep fp32 features
+static int storage_dtype(int dtype) { return dtype == MEB200_TF32 ? MEB200_F32 : dtype; }
+
 extern "C" {
 
 uint64_t meb200_conv_workspace_bytes(uint32_t n_out, uint32_t c_in, uint32_t c_out, uint32_t K,
                                      int dtype) {
-  // the row-split partial sums of a SIMT wgrad (any dtype); for bf16/fp16 also those of the
+  // the row-split partial sums of a SIMT wgrad (any dtype); for bf16/fp16/TF32 also those of the
   // tensor-core wgrad (no call needs both at once)
   const uint64_t ws = conv_wgrad_simt_workspace_bytes(c_in, c_out, K, n_out);
   if (dtype == MEB200_F32) return ws;
@@ -29,7 +32,7 @@ int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_
                         const int32_t *out_order, void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (n_out == 0) return MEB200_OK;
-  MEB_CHECK_ARG(in_dtype >= 0 && in_dtype <= 2 && out_dtype >= 0 && out_dtype <= 2, "dtype");
+  MEB_CHECK_ARG(in_dtype >= 0 && in_dtype <= 3 && out_dtype >= 0 && out_dtype <= 2, "dtype");
   MEB_CHECK_ARG(out_dtype == MEB200_F32 || out_dtype == in_dtype,
                 "output dtype must be fp32 or the input dtype");
   MEB_CHECK_ARG(out && w_cast && (w_t || in_dtype == MEB200_F32) && out_nbr && (in || n_in == 0),
@@ -40,18 +43,23 @@ int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_
                              out, out_dtype, stream);
     if (rc != MEB200_ERR_UNSUPPORTED) return rc;
   }
+  const int fdt = storage_dtype(in_dtype);      // the CUDA-core kernels: exact fp32 for TF32
   if (conv_small_cin_supported(c_in, c_out)) {
-    int rc = conv_small_cin_forward(in, in_dtype, c_in, w_cast, K, c_out, out_nbr, n_out, out,
+    int rc = conv_small_cin_forward(in, fdt, c_in, w_cast, K, c_out, out_nbr, n_out, out,
                                     out_dtype, stream);
     if (rc != MEB200_ERR_UNSUPPORTED) return rc;
   }
-  return conv_forward_simt(in, in_dtype, n_in, c_in, w_cast, K, c_out, /*trans_w=*/false,
+  return conv_forward_simt(in, fdt, n_in, c_in, w_cast, K, c_out, /*trans_w=*/false,
                            out_nbr, n_out, out, out_dtype, stream);
+}
+
+static bool packed_dtype(int dtype) {
+  return dtype == MEB200_BF16 || dtype == MEB200_F16 || dtype == MEB200_TF32;
 }
 
 int meb200_conv_pack_weights(const float *weight, uint32_t K, uint32_t c_in, uint32_t c_out,
                              int dtype, void *w_cast, void *w_t, void *stream_) {
-  MEB_CHECK_ARG(dtype == MEB200_BF16 || dtype == MEB200_F16, "packed weights are bf16 or fp16");
+  MEB_CHECK_ARG(packed_dtype(dtype), "packed weights are bf16, fp16 or tf32");
   MEB_CHECK_ARG(weight && w_cast && w_t, "null buffer");
   MEB_CHECK_ARG(c_in > 0 && c_out > 0 && K > 0 && K <= 65535, "empty channel/kernel dims");
   return conv_pack_weights(weight, K, c_in, c_out, dtype, w_cast, w_t, (cudaStream_t)stream_);
@@ -61,7 +69,7 @@ static_assert(sizeof(meb200_pack_job) == sizeof(PackJob), "meb200_pack_job layou
 
 int meb200_conv_pack_weights_batched(const meb200_pack_job *jobs_dev, uint32_t n_jobs,
                                      uint32_t total_tiles, int dtype, void *stream_) {
-  MEB_CHECK_ARG(dtype == MEB200_BF16 || dtype == MEB200_F16, "packed weights are bf16 or fp16");
+  MEB_CHECK_ARG(packed_dtype(dtype), "packed weights are bf16, fp16 or tf32");
   MEB_CHECK_ARG(jobs_dev != nullptr || n_jobs == 0, "null job table");
   return conv_pack_weights_batched(reinterpret_cast<const PackJob *>(jobs_dev), n_jobs, total_tiles,
                                    dtype, (cudaStream_t)stream_);
@@ -108,9 +116,11 @@ int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32
                          const int32_t *seg_start, uint32_t n_chunks, void *workspace,
                          uint64_t workspace_bytes, const int32_t *in_order, void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  MEB_CHECK_ARG(dtype >= 0 && dtype <= 2, "dtype");
+  MEB_CHECK_ARG(dtype >= 0 && dtype <= 3, "dtype");
   MEB_CHECK_ARG(grad_in_dtype == MEB200_F32 || grad_in_dtype == dtype,
                 "grad_in dtype must be fp32 or the feature dtype");
+  MEB_CHECK_ARG(grad_in_dtype != MEB200_TF32, "grad_in of a TF32 convolution is fp32");
+  const int fdt = storage_dtype(dtype);         // the CUDA-core kernels: exact fp32 for TF32
   MEB_CHECK_ARG(c_in > 0 && c_out > 0 && K > 0, "empty channel/kernel dims");
   if (grad_in != nullptr && n_in > 0) {
     MEB_CHECK_ARG(in_nbr && w_cast && (grad_out || n_out == 0), "null buffer");
@@ -121,7 +131,7 @@ int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32
       rc = conv_forward_tc(grad_out, dtype, n_out, c_out, w_cast, K, c_in, in_nbr, in_order, n_in,
                            grad_in, grad_in_dtype, stream);
     if (rc == MEB200_ERR_UNSUPPORTED)
-      rc = conv_forward_simt(grad_out, dtype, n_out, c_out, w_cast, K, c_in, /*trans_w=*/true,
+      rc = conv_forward_simt(grad_out, fdt, n_out, c_out, w_cast, K, c_in, /*trans_w=*/true,
                              in_nbr, n_in, grad_in, grad_in_dtype, stream);
     if (rc != MEB200_OK) return rc;
   }
@@ -140,9 +150,9 @@ int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32
       if (rc != MEB200_ERR_UNSUPPORTED) return rc;
     }
     if (conv_small_cin_supported(c_in, c_out))
-      return conv_small_cin_wgrad(in, grad_out, dtype, c_in, K, c_out, out_nbr, n_out,
+      return conv_small_cin_wgrad(in, grad_out, fdt, c_in, K, c_out, out_nbr, n_out,
                                   grad_weight, workspace, workspace_bytes, stream);
-    return conv_wgrad_simt(in, grad_out, dtype, c_in, K, c_out, out_nbr, n_out, grad_weight,
+    return conv_wgrad_simt(in, grad_out, fdt, c_in, K, c_out, out_nbr, n_out, grad_weight,
                            workspace, workspace_bytes, stream);
   }
   return MEB200_OK;

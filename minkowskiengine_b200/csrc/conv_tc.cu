@@ -4,6 +4,10 @@
 //   forward / dgrad : out[r, :] = sum_k A[nbr[k][r], :] @ B_k              (k_conv_wg)
 //   wgrad           : dW[k]     += In[rows_in, :]^T @ dOut[rows_out, :]     (k_wgrad_wg)
 //
+// Operands are bf16 / fp16, or fp32 words multiplied in TF32 (MEB200_TF32: k_conv_wg<float, ..>
+// for forward / dgrad, k_wgrad_tf32 for the weight gradient, whose MN-major operands tf32 wgmma
+// cannot read).
+//
 // Replaces the reference's per-offset SIMT tile-matmul with per-element atomicAdd
 // (src/convolution_kernel.cu:114-180,320-496): forward and dgrad write every output row exactly
 // once (no atomics, no zero fill, deterministic) and the fp32 accumulator stays in registers
@@ -41,6 +45,8 @@ __device__ __forceinline__ uint32_t cm_off(uint32_t r, uint32_t j, uint32_t chun
 
 template <typename T>
 constexpr bool kIsBf16 = std::is_same<T, __nv_bfloat16>::value;
+template <typename T>
+constexpr bool kIsTf32 = std::is_same<T, float>::value;   // fp32 storage, tf32 MMAs
 
 template <typename T>
 __device__ __forceinline__ uint32_t pack2(float a, float b);
@@ -85,8 +91,11 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
   const uint32_t s0 = smem_u32(align1k(smem_raw));
   const uint32_t tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
   const uint32_t row0 = blockIdx.x * tc::kFwdRows;
-  const uint32_t bk = p.bk, ch = bk / 8, lch = bk == 64 ? 3 : (bk == 32 ? 2 : 1);
-  const uint32_t a_bytes = tc::kFwdRows * bk * 2, stage_bytes = a_bytes + p.c_cols * bk * 2;
+  // a stage holds `width` bytes of every row: ch 16-byte chunks of kEpc elements, bk channels
+  constexpr uint32_t kEpc = 16 / sizeof(T);
+  const uint32_t bk = p.bk, width = bk * sizeof(T), ch = width / 16;
+  const uint32_t lch = width == 128 ? 3 : (width == 64 ? 2 : 1);
+  const uint32_t a_bytes = tc::kFwdRows * width, stage_bytes = a_bytes + p.c_cols * width;
   const bool ordered = p.tile_mask != nullptr;
   const uint32_t tmask = ordered ? __ldg(p.tile_mask + blockIdx.x) : 0u;
   const uint32_t nch = p.c_red / bk, n_st = (ordered ? __popc(tmask) : p.K) * nch;
@@ -104,12 +113,12 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
       if (ordered) { ld_rem &= ld_rem - 1; ld_k = __ffs(ld_rem) - 1; } else ++ld_k;
     }
     const uint32_t base = s0 + (s % kStages) * stage_bytes;
-    if (p.stem_K == 0) {
+    if (kIsTf32<T> || p.stem_K == 0) {
       const int32_t src = row_ok ? __ldg(p.nbr + (size_t)k * p.n_rows + arow) : -1;
       const bool ok = src >= 0 && (uint32_t)src < p.n_a;
       const T *rp = A + (size_t)(ok ? src : 0) * p.c_red + c0;
       for (uint32_t j = tid & 1u; j < ch; j += 2)
-        cp_async16(base + cm_off(ar, j, ch), rp + 8 * j, ok ? 16u : 0u);
+        cp_async16(base + cm_off(ar, j, ch), rp + kEpc * j, ok ? 16u : 0u);
     } else {
       // chunk j = virtual channels c0 + 8j..: offsets (c0 + 8j) / 4 + {0, 1}, 8 bytes each
       for (uint32_t j = tid & 1u; j < ch; j += 2)
@@ -125,7 +134,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
     const uint32_t nb = p.c_cols * ch;
     for (uint32_t i = tid; i < nb; i += kThreads) {
       const uint32_t n = i >> lch, j = i & (ch - 1);
-      cp_async16(base + a_bytes + cm_off(n, j, ch), Bk + (size_t)n * p.c_red + 8 * j, 16u);
+      cp_async16(base + a_bytes + cm_off(n, j, ch), Bk + (size_t)n * p.c_red + kEpc * j, 16u);
     }
   };
 
@@ -146,14 +155,17 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
     __syncthreads();                    // ... everybody's; the MMAs of stage s - 2 have retired
     if (s + kStages - 2 < n_st) load(s + kStages - 2);   // into the slot of stage s - 2
     cp_async_commit();
-    const uint32_t a0 = s0 + (s % kStages) * stage_bytes + wg * 64 * bk * 2;
+    const uint32_t a0 = s0 + (s % kStages) * stage_bytes + wg * 64 * width;
     const uint32_t b0 = s0 + (s % kStages) * stage_bytes + a_bytes;
     wgmma_fence();
-    for (uint32_t kk = 0; kk < bk / 16; ++kk) {
+    for (uint32_t kk = 0; kk < width / 32; ++kk) {     // one k-step = 32 bytes = 2 core matrices
       const uint64_t da = wgmma_desc(a0 + kk * 256, 128, sbo);
 #pragma unroll
-      for (int i = 0; i < NT; ++i)
-        wgmma<NI, kIsBf16<T>, 0, 0>(acc[i], da, wgmma_desc(b0 + i * NI * bk * 2 + kk * 256, 128, sbo));
+      for (int i = 0; i < NT; ++i) {
+        const uint64_t db = wgmma_desc(b0 + i * NI * width + kk * 256, 128, sbo);
+        if constexpr (kIsTf32<T>) wgmma_tf32<NI, 0, 0>(acc[i], da, db);
+        else wgmma<NI, kIsBf16<T>, 0, 0>(acc[i], da, db);
+      }
     }
     wgmma_commit();
     wgmma_wait<1>();
@@ -173,10 +185,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
       for (int j = 0; j < NI / 8; ++j) {
         const uint32_t col = i * NI + 8 * j + 2 * t;
         const float v0 = acc[i][4 * j + 2 * h], v1 = acc[i][4 * j + 2 * h + 1];
-        if (p.out_f32)
+        if (kIsTf32<T> || p.out_f32)
           *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + (size_t)orow * p.out_ld + col) =
               make_float2(v0, v1);
-        else
+        else if constexpr (!kIsTf32<T>)
           *reinterpret_cast<uint32_t *>(reinterpret_cast<T *>(p.out) + (size_t)orow * p.out_ld + col) =
               pack2<T>(v0, v1);
       }
@@ -346,12 +358,138 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_wg(const WgParams p) {
   }
 }
 
+// TF32 wgrad.  wgmma reads tf32 operands K-major only, and both wgrad operands are gathered
+// MN-major (a pair's channels are contiguous), so this kernel multiplies with the warp-level
+// mma.sync.m16n8k8 instead, whose fragments are plain 32-bit shared-memory loads of any layout.
+// Same CTAs (offset, 128 input channels, share), shares (wg_range) and stores as k_wgrad_wg; a
+// share is walked in stages of kWgRowsTf32 pairs.  Stage = In [32 pairs][128 + pad channels] and
+// dOut [32 pairs][c_out + pad], row-major.  Warp w owns channels 32 (w & 3).. (two 16-row M tiles)
+// and output columns (w >> 2) * c_out / 2.. (NB 8-column N tiles): NB = c_out / 16.
+template <int NB>
+__global__ void __launch_bounds__(kThreads, 1) k_wgrad_tf32(const WgParams p) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  float *sm = reinterpret_cast<float *>(align1k(smem_raw));
+  constexpr uint32_t R = tc::kWgRowsTf32, SA = tc::kWgChannels + tc::kWgPadTf32;
+  const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t k = blockIdx.z, ci0 = blockIdx.y * tc::kWgChannels;
+  const uint32_t SB = p.c_out + tc::kWgPadTf32, chB = p.c_out / 4;
+  const uint32_t stage_floats = R * (SA + SB);
+  const uint32_t n_chunks = p.pin != nullptr ? p.n_chunks : 1u;
+  const float *In = reinterpret_cast<const float *>(p.in);
+  const float *G = reinterpret_cast<const float *>(p.gout);
+
+  uint32_t n_st = 0;
+  for (uint32_t c = 0; c < n_chunks; ++c) {
+    uint32_t lo, hi;
+    wg_range(p, k, c, lo, hi);
+    n_st += (hi - lo + R - 1) / R;
+  }
+  uint32_t wc = 0, pos = 0, end = 0;
+  auto open = [&]() {
+    for (; wc < n_chunks; ++wc) {
+      wg_range(p, k, wc, pos, end);
+      if (pos < end) return;
+    }
+  };
+  open();
+
+  const uint32_t ar = tid >> 3;         // eight threads per In row, 4 chunks of 4 channels each
+  auto load = [&](uint32_t s) {
+    const uint32_t base = smem_u32(sm + (s % kStages) * stage_floats);
+    const uint32_t e = pos;
+    int32_t src = -1;
+    if (e + ar < end)
+      src = p.pin != nullptr ? __ldg(p.pin + e + ar) : __ldg(p.nbr + (size_t)k * p.n_out + e + ar);
+    const bool ok = src >= 0 && (uint32_t)src < p.n_in;
+    const float *rp = In + (size_t)(ok ? src : 0) * p.c_in + ci0;
+#pragma unroll
+    for (uint32_t m = 0; m < 4; ++m) {
+      const uint32_t j = (tid & 7u) + 8 * m;
+      const bool okj = ok && ci0 + 4 * j < p.c_in;
+      cp_async16(base + (ar * SA + 4 * j) * 4, okj ? rp + 4 * j : In, okj ? 16u : 0u);
+    }
+    const uint32_t nb = R * chB;
+    for (uint32_t i = tid; i < nb; i += kThreads) {
+      const uint32_t r = i / chB, j = i - r * chB;
+      int32_t o = -1;
+      if (e + r < end) o = p.pin != nullptr ? __ldg(p.pout + e + r) : (int32_t)(e + r);
+      const bool okr = o >= 0 && (uint32_t)o < p.n_out;
+      cp_async16(base + (R * SA + r * SB + 4 * j) * 4, G + (size_t)(okr ? o : 0) * p.c_out + 4 * j,
+                 okr ? 16u : 0u);
+    }
+    pos += R;
+    if (pos >= end) { ++wc; open(); }
+  };
+
+  float acc[2][NB][4];
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < NB; ++ni)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[mi][ni][q] = 0.f;
+
+  for (uint32_t s = 0; s < kStages - 2; ++s) {
+    if (s < n_st) load(s);
+    cp_async_commit();
+  }
+  const uint32_t g = lane >> 2, t = lane & 3;
+  const uint32_t m0 = (warp & 3) * 32, n0 = (warp >> 2) * NB * 8;
+  for (uint32_t s = 0; s < n_st; ++s) {
+    cp_async_wait<kStages - 3>();
+    __syncthreads();                    // stage s landed everywhere; stage s - 2 is no longer read
+    if (s + kStages - 2 < n_st) load(s + kStages - 2);
+    cp_async_commit();
+    const uint32_t *sA = reinterpret_cast<const uint32_t *>(sm + (s % kStages) * stage_floats);
+    const uint32_t *sB = sA + R * SA;
+    // (the widest tiles keep 128 accumulators: unrolled k-steps would spill them)
+#pragma unroll(NB > 12 ? 1 : 4)
+    for (uint32_t kk = 0; kk < R; kk += 8) {
+      // A[m = channel][k = pair] = In stage [pair][channel]; B[k = pair][n = column] = dOut stage
+      uint32_t a[2][4];
+#pragma unroll
+      for (int mi = 0; mi < 2; ++mi) {
+        const uint32_t *pa = sA + (kk + t) * SA + m0 + 16 * mi + g;
+        a[mi][0] = pa[0]; a[mi][1] = pa[8]; a[mi][2] = pa[4 * SA]; a[mi][3] = pa[4 * SA + 8];
+      }
+#pragma unroll
+      for (int ni = 0; ni < NB; ++ni) {   // B fragments one N tile at a time (register budget)
+        const uint32_t *pb = sB + (kk + t) * SB + n0 + 8 * ni + g;
+        const uint32_t b[2] = {pb[0], pb[4 * SB]};
+        mma_tf32_16x8x8(acc[0][ni], a[0], b);
+        mma_tf32_16x8x8(acc[1][ni], a[1], b);
+      }
+    }
+  }
+
+  const size_t dw_elems = (size_t)p.K * p.c_in * p.c_out;   // every element written by one CTA
+  float *dWk = (p.n_splits > 1 ? p.partial + blockIdx.x * dw_elems : p.dW) + (size_t)k * p.c_in * p.c_out;
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t ci = ci0 + m0 + 16 * mi + g + 8 * h;
+      if (ci >= p.c_in) continue;
+#pragma unroll
+      for (int ni = 0; ni < NB; ++ni)
+        *reinterpret_cast<float2 *>(dWk + (size_t)ci * p.c_out + n0 + 8 * ni + 2 * t) =
+            make_float2(acc[mi][ni][2 * h], acc[mi][ni][2 * h + 1]);
+    }
+}
+
 
 // ---- weight packing ----------------------------------------------------------------------------
-// Per-optimizer-step weight packing: fp32 master W[k][ci][co] -> feature dtype in the two
+// Per-optimizer-step weight packing: fp32 master W[k][ci][co] -> the operand type in the two
 // operand-B layouts of the wgmma kernels, in one pass:
 //   Wc [k][ci][co]  dgrad operand B            Wt [k][co][ci]  forward operand B
-// One CTA packs the 32 x 32 tile (k, ci0.., co0..).
+// bf16 / fp16: rounded to nearest even; TF32 (T = float): rounded to the nearest tf32 value, ties
+// away from zero (cvt.rna), and kept in fp32 words, so that the forward and the dgrad multiply the
+// same matrix.  One CTA packs the 32 x 32 tile (k, ci0.., co0..).
+template <typename T>
+__device__ __forceinline__ T to_operand(float v) {
+  if constexpr (kIsTf32<T>) return tf32_rna(v); else return from_f32<T>(v);
+}
+
 template <typename T>
 __device__ __forceinline__ void pack_tile(const float *__restrict__ W, T *__restrict__ Wc,
                                           T *__restrict__ Wt, uint32_t c_in, uint32_t c_out,
@@ -363,12 +501,12 @@ __device__ __forceinline__ void pack_tile(const float *__restrict__ W, T *__rest
     if (ci0 + i < c_in && co0 + tx < c_out) {
       const float v = W[base + (size_t)(ci0 + i) * c_out + co0 + tx];
       tile[i][tx] = v;
-      Wc[base + (size_t)(ci0 + i) * c_out + co0 + tx] = from_f32<T>(v);
+      Wc[base + (size_t)(ci0 + i) * c_out + co0 + tx] = to_operand<T>(v);
     }
   __syncthreads();
   for (uint32_t i = ty; i < 32; i += 8)
     if (co0 + i < c_out && ci0 + tx < c_in)
-      Wt[base + (size_t)(co0 + i) * c_in + ci0 + tx] = from_f32<T>(tile[tx][i]);
+      Wt[base + (size_t)(co0 + i) * c_in + ci0 + tx] = to_operand<T>(tile[tx][i]);
 }
 
 template <typename T>
@@ -404,6 +542,8 @@ int conv_pack_weights_batched(const PackJob *jobs_dev, uint32_t n_jobs, uint32_t
   if (n_jobs == 0 || total_tiles == 0) return MEB200_OK;
   if (dtype == MEB200_BF16)
     k_pack_w_batched<__nv_bfloat16><<<total_tiles, 256, 0, stream>>>(jobs_dev, n_jobs);
+  else if (dtype == MEB200_TF32)
+    k_pack_w_batched<float><<<total_tiles, 256, 0, stream>>>(jobs_dev, n_jobs);
   else
     k_pack_w_batched<__half><<<total_tiles, 256, 0, stream>>>(jobs_dev, n_jobs);
   MEB_LAUNCH_OK();
@@ -416,6 +556,8 @@ int conv_pack_weights(const float *W, uint32_t K, uint32_t c_in, uint32_t c_out,
   if (dtype == MEB200_BF16)
     k_pack_w<__nv_bfloat16><<<grid, 256, 0, stream>>>(W, (__nv_bfloat16 *)w_cast,
                                                       (__nv_bfloat16 *)w_t, c_in, c_out);
+  else if (dtype == MEB200_TF32)
+    k_pack_w<float><<<grid, 256, 0, stream>>>(W, (float *)w_cast, (float *)w_t, c_in, c_out);
   else
     k_pack_w<__half><<<grid, 256, 0, stream>>>(W, (__half *)w_cast, (__half *)w_t, c_in, c_out);
   MEB_LAUNCH_OK();
@@ -458,7 +600,8 @@ template <typename T, int NI, int NT>
 static int launch_fwd(const FwdParams &p, cudaStream_t stream) {
   auto kern = k_conv_wg<T, NI, NT>;
   MEB_BIG_SMEM(kern);
-  kern<<<cdiv(p.n_rows, tc::kFwdRows), kThreads, tc::fwd_smem_bytes(p.bk, p.c_cols), stream>>>(p);
+  kern<<<cdiv(p.n_rows, tc::kFwdRows), kThreads, tc::fwd_ring_bytes(p.bk * sizeof(T), p.c_cols),
+         stream>>>(p);
   count_tc_launch();
   MEB_LAUNCH_OK();
   return MEB200_OK;
@@ -472,6 +615,7 @@ static int dispatch_fwd(const FwdParams &p, cudaStream_t stream) {
   return MEB200_ERR_UNSUPPORTED;
 }
 static int run_fwd(int dtype, const FwdParams &p, cudaStream_t stream) {
+  if (dtype == MEB200_TF32) return dispatch_fwd<float>(p, stream);
   return dtype == MEB200_BF16 ? dispatch_fwd<__nv_bfloat16>(p, stream)
                               : dispatch_fwd<__half>(p, stream);
 }
@@ -490,6 +634,26 @@ static int dispatch_wgrad(const WgParams &p, dim3 grid, cudaStream_t stream) {
 #define MEB_L(NI, NT) launch_wgrad<T, NI, NT>(p, grid, stream)
   MEB_COLS_DISPATCH(p.c_out, MEB_L)
 #undef MEB_L
+  set_error("wgrad tc: %u output channels", p.c_out);
+  return MEB200_ERR_UNSUPPORTED;
+}
+template <int NB>
+static int launch_wgrad_tf32(const WgParams &p, dim3 grid, cudaStream_t stream) {
+  auto kern = k_wgrad_tf32<NB>;
+  MEB_BIG_SMEM(kern);
+  kern<<<grid, kThreads, tc::wgrad_tf32_smem_bytes(p.c_out), stream>>>(p);
+  count_tc_launch();
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
+}
+static int dispatch_wgrad_tf32(const WgParams &p, dim3 grid, cudaStream_t stream) {
+  switch (p.c_out / 16) {
+#define MEB_L(NB) case NB: return launch_wgrad_tf32<NB>(p, grid, stream);
+    MEB_L(1) MEB_L(2) MEB_L(3) MEB_L(4) MEB_L(5) MEB_L(6) MEB_L(7) MEB_L(8)
+    MEB_L(9) MEB_L(10) MEB_L(11) MEB_L(12) MEB_L(13) MEB_L(14) MEB_L(15) MEB_L(16)
+#undef MEB_L
+    default: break;
+  }
   set_error("wgrad tc: %u output channels", p.c_out);
   return MEB200_ERR_UNSUPPORTED;
 }
@@ -512,16 +676,19 @@ static int run_wgrad(int dtype, WgParams p, uint32_t K_grid, uint32_t est_stages
                                 workspace_bytes, dw_elems * sizeof(float));
   p.partial = p.n_splits > 1 ? reinterpret_cast<float *>(workspace) : nullptr;
   const dim3 grid(p.n_splits, m_tiles, K_grid);
-  const int rc = dtype == MEB200_BF16 ? dispatch_wgrad<__nv_bfloat16>(p, grid, stream)
-                                      : dispatch_wgrad<__half>(p, grid, stream);
+  const int rc = dtype == MEB200_TF32   ? dispatch_wgrad_tf32(p, grid, stream)
+                 : dtype == MEB200_BF16 ? dispatch_wgrad<__nv_bfloat16>(p, grid, stream)
+                                        : dispatch_wgrad<__half>(p, grid, stream);
   if (rc != MEB200_OK || p.n_splits == 1) return rc;
   return launch_split_sum(p.partial, p.dW, dw_elems, p.n_splits, stream);
 }
 
 // ---- forward / dgrad ----------------------------------------------------------------------------
+static uint32_t operand_bytes(int dtype) { return dtype == MEB200_TF32 ? 4 : 2; }
+
 bool conv_tc_supported(int dtype, uint32_t c_reduce, uint32_t c_cols) {
-  if (dtype != MEB200_BF16 && dtype != MEB200_F16) return false;
-  if (tc::fwd_bk(c_reduce) == 0) return false;
+  if (dtype != MEB200_BF16 && dtype != MEB200_F16 && dtype != MEB200_TF32) return false;
+  if (tc::fwd_stage_bytes(c_reduce, operand_bytes(dtype)) == 0) return false;
   return c_cols % 16 == 0 && c_cols >= 16 && c_cols <= 1024;
 }
 
@@ -539,10 +706,10 @@ int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, c
   const uint8_t *Wb = reinterpret_cast<const uint8_t *>(B);
   const bool ordered = order != nullptr && K <= kMaxOrderK;
   // one launch per slice of <= 256 output columns
-  const size_t out_esz = out_dtype == MEB200_F32 ? 4 : 2;
+  const size_t out_esz = out_dtype == MEB200_F32 ? 4 : 2, esz = operand_bytes(dtype);
   for (uint32_t n0 = 0; n0 < c_cols; n0 += tc::kMaxCols) {
     FwdParams p{};
-    p.A = A; p.B = Wb + (size_t)n0 * c_reduce * 2; p.nbr = ordered ? order : nbr;
+    p.A = A; p.B = Wb + (size_t)n0 * c_reduce * esz; p.nbr = ordered ? order : nbr;
     if (ordered) {
       p.slot_row = order + (size_t)K * n_rows;
       p.tile_mask = reinterpret_cast<const uint32_t *>(order + (size_t)(K + 1) * n_rows);
@@ -551,7 +718,7 @@ int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, c
     p.b_k_stride = (uint64_t)c_cols * c_reduce;
     p.c_red = c_reduce; p.c_cols = c_cols - n0 < tc::kMaxCols ? c_cols - n0 : tc::kMaxCols;
     p.K = K; p.n_rows = n_rows; p.n_a = n_a; p.out_ld = c_cols;
-    p.bk = tc::fwd_bk(c_reduce); p.out_f32 = out_dtype == MEB200_F32;
+    p.bk = tc::fwd_stage_bytes(c_reduce, esz) / esz; p.out_f32 = out_dtype == MEB200_F32;
     const int rc = run_fwd(dtype, p, stream);
     if (rc != MEB200_OK) return rc;
   }
@@ -610,7 +777,7 @@ int conv_stem_wgrad_tc(const void *in4, const void *grad_out, int dtype, uint32_
 
 // ---- wgrad ---------------------------------------------------------------------------------------
 bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out) {
-  if (dtype != MEB200_BF16 && dtype != MEB200_F16) return false;
+  if (dtype != MEB200_BF16 && dtype != MEB200_F16 && dtype != MEB200_TF32) return false;
   return c_in % 8 == 0 && c_in >= 16 && c_out % 16 == 0 && c_out >= 16 && c_out <= tc::kMaxCols;
 }
 

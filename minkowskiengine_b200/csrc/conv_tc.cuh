@@ -1,10 +1,11 @@
-// wgmma (Hopper warpgroup MMA) sparse convolution kernels, bf16/fp16 operands, fp32 accumulation.
+// Tensor-core sparse convolution kernels: bf16/fp16 operands, or fp32 ones multiplied in TF32
+// (MEB200_TF32), fp32 accumulation.
 #pragma once
 #include "common.cuh"
 
 namespace meb200 {
 
-// bf16/fp16 features with channel counts the wgmma tiles cover.
+// bf16/fp16/TF32 operands with channel counts the tiles cover.
 bool conv_tc_supported(int dtype, uint32_t c_reduce, uint32_t c_cols);
 bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out);
 
@@ -16,7 +17,8 @@ int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, c
                     uint32_t K, uint32_t c_cols, const int32_t *nbr, const int32_t *order,
                     uint32_t n_rows, void *out, int out_dtype, cudaStream_t stream);
 
-// fp32 W[K,c_in,c_out] -> w_cast [K,c_in,c_out] and w_t [K,c_out,c_in] in bf16/fp16.
+// fp32 W[K,c_in,c_out] -> w_cast [K,c_in,c_out] and w_t [K,c_out,c_in] in bf16/fp16, or in fp32
+// words rounded to tf32 (MEB200_TF32).
 int conv_pack_weights(const float *W, uint32_t K, uint32_t c_in, uint32_t c_out, int dtype,
                       void *w_cast, void *w_t, cudaStream_t stream);
 

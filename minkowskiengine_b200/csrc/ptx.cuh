@@ -1,5 +1,6 @@
 // Thin inline-PTX wrappers for the Hopper (sm_90a) primitives the tensor-core kernels use:
-// cp.async, the async-proxy fence, and warpgroup MMA (wgmma) with shared-memory descriptors.
+// cp.async, the async-proxy fence, warpgroup MMA (wgmma) with shared-memory descriptors, and the
+// warp-level tf32 MMA of the TF32 weight gradient.
 #pragma once
 #include <stdint.h>
 
@@ -101,7 +102,54 @@ __device__ __forceinline__ void wgmma_64_f16(float (&d)[32], uint64_t da, uint64
                "%32, %33, p, 1, 1, %35, %36;\n\t}"
                : MEB_F8(d, 0), MEB_F8(d, 8), MEB_F8(d, 16), MEB_F8(d, 24) : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
 }
+// tf32: D[64 x N] += A[64 x 8] * B[8 x N] over fp32 words (the same 32 bytes of a row per k-step
+// as the 16-bit forms).  The instruction has no transpose immediates: both operands K-major.
+__device__ __forceinline__ void wgmma_16_tf32(float (&d)[8], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, "
+               "%8, %9, p, 1, 1;\n\t}"
+               : MEB_F8(d, 0) : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_32_tf32(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+               "%16, %17, p, 1, 1;\n\t}"
+               : MEB_F8(d, 0), MEB_F8(d, 8) : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_64_tf32(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+               "%32, %33, p, 1, 1;\n\t}"
+               : MEB_F8(d, 0), MEB_F8(d, 8), MEB_F8(d, 16), MEB_F8(d, 24) : "l"(da), "l"(db), "r"(1));
+}
 #undef MEB_F8
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t da, uint64_t db) {
+  static_assert(N == 16 || N == 32 || N == 64, "wgmma: N is 16, 32 or 64");
+  static_assert(TA == 0 && TB == 0, "tf32 wgmma reads K-major operands only");
+  if constexpr (N == 16) wgmma_16_tf32(d, da, db);
+  else if constexpr (N == 32) wgmma_32_tf32(d, da, db);
+  else wgmma_64_tf32(d, da, db);
+}
+
+// fp32 -> the nearest tf32 value (ties away from zero), kept in an fp32 word
+__device__ __forceinline__ float tf32_rna(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return __uint_as_float(r);
+}
+
+// Warp-level D[16 x 8] += A[16 x 8] * B[8 x 8] in tf32 (fp32 words as stored), lane = 4g + t:
+//   a = A[g][t], A[g + 8][t], A[g][t + 4], A[g + 8][t + 4];  b = B[t][g], B[t + 4][g]
+//   d = D[g][2t], D[g][2t + 1], D[g + 8][2t], D[g + 8][2t + 1]
+__device__ __forceinline__ void mma_tf32_16x8x8(float (&d)[4], const uint32_t (&a)[4],
+                                                const uint32_t (&b)[2]) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, "
+               "{%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+
 template <int N, bool BF16, int TA, int TB>
 __device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t da, uint64_t db) {
   static_assert(N == 16 || N == 32 || N == 64, "wgmma: N is 16, 32 or 64");

@@ -16,17 +16,33 @@ constexpr uint32_t kWgChannels = 128;       // wgrad: input channels per CTA (2 
 
 inline uint32_t cdiv_u(uint64_t a, uint64_t b) { return (uint32_t)((a + b - 1) / b); }
 
-// forward / dgrad: reduction channels per stage (64, 32 or 16), 0 = unsupported
-inline uint32_t fwd_bk(uint32_t c_red) {
-  return c_red % 64 == 0 ? 64 : (c_red % 32 == 0 ? 32 : (c_red % 16 == 0 ? 16 : 0));
+// forward / dgrad: bytes of every operand row one stage holds (128, 64 or 32: one wgmma k-step
+// reads 32 bytes of a row whatever the element size), for `c_red` reduction channels of `esz`
+// bytes each; 0 = unsupported (the row is not a whole number of 32-byte k-steps)
+inline uint32_t fwd_stage_bytes(uint32_t c_red, uint32_t esz) {
+  const uint32_t b = c_red * esz;
+  return b % 128 == 0 ? 128 : (b % 64 == 0 ? 64 : (b % 32 == 0 ? 32 : 0));
 }
-// one stage = A [128 rows x bk] + B [c_cols x bk], 16-bit elements; +1 KB for alignment
-inline uint32_t fwd_smem_bytes(uint32_t bk, uint32_t c_cols) {
-  return 1024 + kStages * (kFwdRows + c_cols) * bk * 2;
+// one stage = A [128 rows x width] + B [c_cols x width], width in bytes; +1 KB for alignment
+inline uint32_t fwd_ring_bytes(uint32_t width, uint32_t c_cols) {
+  return 1024 + kStages * (kFwdRows + c_cols) * width;
 }
-// one stage = A [64 rows x 128 channels] + B [64 rows x c_out]
+// 16-bit elements: reduction channels per stage (64, 32 or 16), 0 = unsupported
+inline uint32_t fwd_bk(uint32_t c_red) { return fwd_stage_bytes(c_red, 2) / 2; }
+inline uint32_t fwd_smem_bytes(uint32_t bk, uint32_t c_cols) { return fwd_ring_bytes(bk * 2, c_cols); }
+
+// one stage = A [64 rows x 128 channels] + B [64 rows x c_out], 16-bit elements
 inline uint32_t wgrad_smem_bytes(uint32_t c_out) {
   return 1024 + kStages * kWgRows * (kWgChannels + c_out) * 2;
+}
+
+// TF32 wgrad (warp-level mma.sync, fp32 operands read as stored): stages of kWgRowsTf32 pairs, each
+// row padded by kWgPadTf32 floats, so that a row stride is 8 or 24 words modulo the 32 banks and the
+// fragment loads of a warp (lanes = 4 rows x 8 columns) hit 32 different banks.
+constexpr uint32_t kWgRowsTf32 = 32;
+constexpr uint32_t kWgPadTf32 = 8;
+inline uint32_t wgrad_tf32_smem_bytes(uint32_t c_out) {
+  return 1024 + kStages * kWgRowsTf32 * (kWgChannels + kWgPadTf32 + c_out + kWgPadTf32) * 4;
 }
 
 // wgrad row splits: enough CTAs for two waves over (k, channel tile) pairs, but at least
