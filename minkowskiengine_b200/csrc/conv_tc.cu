@@ -198,10 +198,12 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
 // =====================================================================================
 // wgrad:  dW[k][ci][co] += sum over (input row i, output row o) pairs of offset k of
 //         In[i][ci] * dOut[o][co]
-// GEMM view: D[M = ci][N = co] over the reduction axis "pair"; a stage = 64 pairs.  One CTA owns
-// (offset k, 128 input channels, a share of the pairs).  With one share per offset it stores its
-// sums into dW; otherwise share s stores into partial[s] and launch_split_sum adds the shares in
-// order, so the result does not depend on the order in which CTAs finish.  The pairs come from
+// GEMM view: D[M = ci][N = co] over the reduction axis "pair"; a stage = 64 pairs.  One unit =
+// (offset k, 128 input channels, a share of the pairs), run by one CTA, or in pair mode by one CTA
+// per column slice when k has over twice the mean pairs (k_wgrad_wg).  With one share per
+// offset it stores its sums into dW; otherwise share s stores into partial[s] and
+// launch_split_sum adds the shares in order, so the result does not depend on the order in which
+// CTAs finish, nor on the column slicing.  The pairs come from
 //   pair mode   : the compacted lists of meb200_kernel_map_pairs (segments (row chunk, offset),
 //                 padded with -1); the CTA takes the same fraction of every chunk's segment
 //   dense mode  : all output rows o of the table, i = nbr[k][o]
@@ -216,6 +218,7 @@ struct WgParams {
   float *partial;          // [n_splits][K, c_in, c_out] when n_splits > 1
   uint32_t c_in, c_out, K, n_in, n_out, n_chunks, n_splits;
   uint32_t stem_K;         // > 0: stem mode
+  uint32_t col_slices;     // pair mode, k_wgrad_wg: NT = heavy offsets in column slices (below)
 };
 
 // This CTA's share [lo, hi) of chunk c's pairs of offset k, in whole 64-pair stages.
@@ -233,15 +236,19 @@ __device__ __forceinline__ void wg_range(const WgParams &p, uint32_t k, uint32_t
   if (lo > hi) lo = hi;
 }
 
+// One (offset k, channel tile, share) unit of k_wgrad_wg over the NI * NT output columns col0..:
+// NT wgmma instructions of N = NI columns each.  An output element's sum is the same sequence of
+// m64nNIk16 instructions on the same operands whichever columns the CTA covers, so a unit cut into
+// column slices gives the same bits as the whole unit.
 template <typename T, int NI, int NT>
-__global__ void __launch_bounds__(kThreads, 1) k_wgrad_wg(const WgParams p) {
+__device__ __forceinline__ void wgrad_unit(const WgParams &p, uint32_t k, uint32_t col0) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t s0 = smem_u32(align1k(smem_raw));
   const uint32_t tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
-  const uint32_t k = blockIdx.z, ci0 = blockIdx.y * tc::kWgChannels;
+  const uint32_t ci0 = blockIdx.y * tc::kWgChannels;
   constexpr uint32_t kChA = tc::kWgChannels / 8;                    // 16 chunks per A row
   constexpr uint32_t a_bytes = tc::kWgRows * tc::kWgChannels * 2;
-  const uint32_t chB = p.c_out / 8, stage_bytes = a_bytes + tc::kWgRows * p.c_out * 2;
+  constexpr uint32_t chB = NI * NT / 8, stage_bytes = a_bytes + tc::kWgRows * NI * NT * 2;
   const uint32_t n_chunks = p.pin != nullptr ? p.n_chunks : 1u;
   const T *In = reinterpret_cast<const T *>(p.in);
   const T *G = reinterpret_cast<const T *>(p.gout);
@@ -298,8 +305,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_wg(const WgParams p) {
       int32_t o = -1;
       if (e + r < end) o = p.pin != nullptr ? __ldg(p.pout + e + r) : (int32_t)(e + r);
       const bool ok = o >= 0 && (uint32_t)o < p.n_out;
-      cp_async16(base + a_bytes + cm_off(r, j, chB), G + (size_t)(ok ? o : 0) * p.c_out + 8 * j,
-                 ok ? 16u : 0u);
+      cp_async16(base + a_bytes + cm_off(r, j, chB),
+                 G + (size_t)(ok ? o : 0) * p.c_out + col0 + 8 * j, ok ? 16u : 0u);
     }
     pos += tc::kWgRows;
     if (pos >= end) { ++wc; open(); }
@@ -352,10 +359,49 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_wg(const WgParams p) {
     for (int i = 0; i < NT; ++i)
 #pragma unroll
       for (int j = 0; j < NI / 8; ++j) {
-        *reinterpret_cast<float2 *>(dWk + (size_t)ci * p.c_out + i * NI + 8 * j + 2 * t) =
+        *reinterpret_cast<float2 *>(dWk + (size_t)ci * p.c_out + col0 + i * NI + 8 * j + 2 * t) =
             make_float2(acc[i][4 * j + 2 * h], acc[i][4 * j + 2 * h + 1]);
       }
   }
+}
+
+// 64-pair stages of offset k, over all row chunks of the pair lists
+__device__ __forceinline__ uint32_t wg_offset_stages(const WgParams &p, uint32_t k) {
+  uint32_t s = 0;
+  for (uint32_t c = 0; c < p.n_chunks; ++c)
+    s += ((uint32_t)(__ldg(p.seg + (size_t)c * p.K + k + 1) - __ldg(p.seg + (size_t)c * p.K + k)) +
+          tc::kWgRows - 1) / tc::kWgRows;
+  return s;
+}
+
+// Pair mode with col_slices = NT: blockIdx.z = k * NT + j.  An offset with more than twice the
+// mean stages per offset (the centre offset of a stride-1 map has 3.2x) runs each of its units as
+// NT CTAs of NI columns (slice j); the others as one CTA of all columns (j = 0, the rest exit).
+// The sums are those of the unsliced grid, bit for bit; only the longest CTAs get shorter.  (A
+// slice gathers the whole input tile for a part of the columns, and the extra CTAs can spill into
+// a second wave: below twice the mean that costs more than it saves.)
+// (tiles of up to 128 columns fit two CTAs per SM in shared memory: keep the registers for two)
+template <typename T, int NI, int NT>
+__global__ void __launch_bounds__(kThreads, NI * NT <= 128 ? 2 : 1) k_wgrad_wg(const WgParams p) {
+  if constexpr (NT > 1) {
+    if (p.col_slices == NT) {
+      const uint32_t k = blockIdx.z / NT, j = blockIdx.z % NT;
+      // total stages: every warp adds the segments lane-strided, the same sum in every warp
+      const uint32_t lane = threadIdx.x & 31, n_seg = p.n_chunks * p.K;
+      uint32_t t = 0;
+      for (uint32_t i = lane; i < n_seg; i += 32)
+        t += ((uint32_t)(__ldg(p.seg + i + 1) - __ldg(p.seg + i)) + tc::kWgRows - 1) / tc::kWgRows;
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) t += __shfl_xor_sync(0xffffffffu, t, d);
+      if ((uint64_t)wg_offset_stages(p, k) * p.K > 2ull * t) {
+        wgrad_unit<T, NI, 1>(p, k, j * NI);
+      } else if (j == 0) {
+        wgrad_unit<T, NI, NT>(p, k, 0);
+      }
+      return;
+    }
+  }
+  wgrad_unit<T, NI, NT>(p, blockIdx.z, 0);
 }
 
 // TF32 wgrad.  wgmma reads tf32 operands K-major only, and both wgrad operands are gathered
@@ -657,6 +703,13 @@ static int dispatch_wgrad_tf32(const WgParams &p, dim3 grid, cudaStream_t stream
   set_error("wgrad tc: %u output channels", p.c_out);
   return MEB200_ERR_UNSUPPORTED;
 }
+// wgmma instructions (NT of MEB_COLS_DISPATCH) per row of a k_wgrad_wg tile of c_out columns
+static uint32_t wgrad_col_instructions(uint32_t c_out) {
+#define MEB_NT(NI, NT) NT
+  MEB_COLS_DISPATCH(c_out, MEB_NT)
+#undef MEB_NT
+  return 1;
+}
 static uint32_t wgrad_planned_splits(uint32_t c_in, uint32_t K, uint32_t est_stages) {
   return tc::wgrad_splits(est_stages, K, cdiv(c_in, tc::kWgChannels), (uint32_t)num_sms());
 }
@@ -666,8 +719,9 @@ uint64_t conv_wgrad_workspace_bytes(uint32_t c_in, uint32_t c_out, uint32_t K, u
   return splits > 1 ? (uint64_t)splits * K * c_in * c_out * sizeof(float) : 0;
 }
 
-// grid = (row splits, 128-channel tiles of c_in, offsets).  The splits are what the workspace
-// holds of the planned ones (one split: no workspace, the CTAs store into dW directly).
+// grid = (row splits, 128-channel tiles of c_in, offsets x column slices).  The splits are what
+// the workspace holds of the planned ones (one split: no workspace, the CTAs store into dW
+// directly); column slices only change which CTA computes which columns (k_wgrad_wg).
 static int run_wgrad(int dtype, WgParams p, uint32_t K_grid, uint32_t est_stages, void *workspace,
                      uint64_t workspace_bytes, cudaStream_t stream) {
   const uint32_t m_tiles = cdiv(p.c_in, tc::kWgChannels);
@@ -675,7 +729,9 @@ static int run_wgrad(int dtype, WgParams p, uint32_t K_grid, uint32_t est_stages
   p.n_splits = workspace_splits(wgrad_planned_splits(p.c_in, K_grid, est_stages), workspace,
                                 workspace_bytes, dw_elems * sizeof(float));
   p.partial = p.n_splits > 1 ? reinterpret_cast<float *>(workspace) : nullptr;
-  const dim3 grid(p.n_splits, m_tiles, K_grid);
+  // pair mode on the 16-bit kernel: room for the column slices of the heavy offsets
+  p.col_slices = p.pin != nullptr && dtype != MEB200_TF32 ? wgrad_col_instructions(p.c_out) : 1;
+  const dim3 grid(p.n_splits, m_tiles, K_grid * p.col_slices);
   const int rc = dtype == MEB200_TF32   ? dispatch_wgrad_tf32(p, grid, stream)
                  : dtype == MEB200_BF16 ? dispatch_wgrad<__nv_bfloat16>(p, grid, stream)
                                         : dispatch_wgrad<__half>(p, grid, stream);

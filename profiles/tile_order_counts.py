@@ -7,6 +7,13 @@ Per stride level of MinkUNet34C, for the k3 table of the level and for the k2s2 
 the level and the next: `dense` = every offset for every tile (no order), `natural` = only the
 offsets a tile reaches in the map's own row order, `sorted` = the same after the stable sort by
 neighbour mask, `bound` = pairs / 128 (every tile full of pairs).
+
+A second table counts the pair-mode weight gradient's 64-pair stages on the same tables (pair-list
+chunks of 262144 rows, one 128-channel tile, CTA time proportional to its stages, CTAs placed in
+launch order on the first free of `--resident` slots): `per offset` = the makespan of the same
+number of CTAs for every offset (tc_config.h wgrad_splits, each 1/splits of its offset), `bound` =
+total / resident.  An offset above twice the mean sets the makespan: k_wgrad_wg runs its CTAs in
+column slices.
 """
 import argparse
 import os
@@ -61,11 +68,50 @@ def _row(name, masks, K):
     return dense, srt, pairs / TILE
 
 
+WG_STAGE, WG_CHUNK, SMS = 64, 262144, 132
+
+
+def _wgrad_stages(masks, K):
+    """[K] 64-pair stages of every offset's pair list, summed over its row chunks."""
+    n = len(masks)
+    st = np.zeros(K, dtype=np.int64)
+    for c0 in range(0, n, WG_CHUNK):
+        m = masks[c0:c0 + WG_CHUNK]
+        for k in range(K):
+            st[k] += (int(((m >> k) & 1).sum()) + WG_STAGE - 1) // WG_STAGE
+    return st
+
+
+def _makespan(works, slots):
+    """CTAs of the given works placed in order on the first free of `slots` slots."""
+    free = np.zeros(slots, dtype=np.int64)
+    for w in works:
+        i = int(np.argmin(free))
+        free[i] += w
+    return int(free.max())
+
+
+def _wgrad_row(name, masks, K, resident):
+    st = _wgrad_stages(masks, K)
+    n = len(masks)
+    # wgrad_splits(n / 192 + 1, K, 1, 132) CTAs per offset, share x of offset k taking about
+    # 1/splits of its stages; launch order: the shares of an offset, then the next offset
+    want = -(-2 * SMS // K)
+    splits = max(1, min(want, (n // (3 * WG_STAGE) + 1) // 4))
+    works = [int(s) * (x + 1) // splits - int(s) * x // splits for s in st for x in range(splits)]
+    today = _makespan(works, resident)
+    bound = -(-int(st.sum()) // resident)
+    print(f"| {name} | {n:,} | {st.max() / st.mean():.2f} | {splits * K} | {today:,} | "
+          f"{bound:,} | {today / max(bound, 1):.2f} |")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--clouds", type=int, default=8)
     ap.add_argument("--voxels", type=int, default=100_000)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--resident", type=int, default=264,
+                    help="wgrad CTAs the GPU runs at once (2 per SM at c_out <= 96 on 132 SMs)")
     a = ap.parse_args()
     import torch
     from examples.synthetic import surface_cloud
@@ -78,14 +124,26 @@ def main():
     levels = [coords]
     for ts in (2, 4, 8, 16):
         levels.append(_strided(levels[-1], ts))
+    tables = []
     for i, c in enumerate(levels):
         ts = 2 ** i
-        _row(f"k3, stride {ts}", _masks(c, c, np.array(k3) * ts), 27)
+        tables.append((f"k3, stride {ts}", _masks(c, c, np.array(k3) * ts), 27))
+        _row(*tables[-1])
         if i + 1 < len(levels):
             coarse = levels[i + 1]
             # strided k2s2: coarse rows gather fine rows; transposed: fine rows gather one coarse row
-            _row(f"k2s2 {ts} → {2 * ts}", _masks(coarse, c, np.array(k2) * ts), 8)
-            _row(f"k2s2 transposed {2 * ts} → {ts}", _masks(c, coarse, -np.array(k2) * ts), 8)
+            tables.append((f"k2s2 {ts} → {2 * ts}", _masks(coarse, c, np.array(k2) * ts), 8))
+            _row(*tables[-1])
+            tables.append((f"k2s2 transposed {2 * ts} → {ts}",
+                           _masks(c, coarse, -np.array(k2) * ts), 8))
+            _row(*tables[-1])
+    print()
+    print(f"wgrad stages (makespan of the slowest of {a.resident} CTA slots):")
+    print()
+    print("| table | rows | max / mean stages per offset | CTAs | per offset | bound | ratio |")
+    print("|---|---|---|---|---|---|---|")
+    for name, masks, K in tables:
+        _wgrad_row(name, masks, K, a.resident)
 
 
 if __name__ == "__main__":
