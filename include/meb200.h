@@ -405,6 +405,54 @@ int meb200_union_fold_backward(const void *const *inputs, uint32_t N, uint32_t i
                                const void *grad_out, uint32_t i, const int64_t *u_i, uint32_t n_i,
                                void *grad_i, void *stream);
 
+/* ---- dense tensors: feature rows <-> a dense volume (reference: SparseTensor.dense
+ *      MinkowskiSparseTensor.py:460-557, to_sparse MinkowskiOps.py:279-317).  Data movement only:
+ *      bit-exact in every dtype.  Every output element is written exactly once: no memset, no
+ *      atomics.  16-byte accesses where C * sizeof(dtype) % 16 == 0 and the pointers and strides
+ *      allow.
+ *   A dense tensor [B, C, X1..XD] in any axis order, or any strided view of one, is described by
+ *   its ELEMENT strides; offsets are 64-bit.  Columns follow coordinate rows: column 0 the batch
+ *   index, columns 1..D the axes.  Cell (i_0..i_D) holds the coordinate origin[j] + i_j * step[j]
+ *   (column 0: origin 0, step 1). ---------------------------------------------------------------- */
+typedef struct {
+  uint32_t ncols;                    /* D + 1                                          */
+  uint32_t channels;                 /* C                                              */
+  uint32_t shape[MEB200_MAX_NCOLS];  /* B, X1..XD                                      */
+  int64_t stride[MEB200_MAX_NCOLS];  /* element stride of the batch axis and each axis */
+  int64_t channel_stride;
+  int32_t origin[MEB200_MAX_NCOLS];  /* 0, min_coordinate                              */
+  int32_t step[MEB200_MAX_NCOLS];    /* 1, then the tensor stride (contracted) or 1    */
+} meb200_dense_desc;
+
+/* dense[cell, :] = feats[r, :] where row r of the map lies on the cell's coordinate, else 0, for
+ * every cell: the map's table is probed once per cell as meb200_map_find probes it, so rows
+ * outside the volume are never reached (cropped), and with step 1 on a strided map the cells off
+ * its lattice are zero.  feats: [n, C] in `dtype`; desc: HOST.  SparseTensor.dense forward and
+ * the backward of to_sparse (reference: the index assignment of MinkowskiSparseTensor.py:546-554). */
+int meb200_dense_from_rows(const void *feats, int dtype, uint32_t n, const int32_t *map_coords,
+                           const uint32_t *table, uint32_t capacity,
+                           const meb200_dense_desc *desc, void *dense, void *stream);
+
+/* out[r, :] = dense[cell of coords[r], :] for r < n, 0 where the row lies outside the volume or
+ * off the step lattice.  coords: int32 [n, ncols]; out: [n, C] in `dtype`; desc: HOST.  The
+ * features of to_sparse (reference: MinkowskiOps.py:311-316) and the backward of dense. */
+int meb200_dense_to_rows(const void *dense, int dtype, const meb200_dense_desc *desc,
+                         const int32_t *coords, uint32_t n, void *out, void *stream);
+
+/* Non-zero cells of a dense volume (reference: abs(x).sum(channel) != 0, where, stack —
+ * MinkowskiOps.py:308-310): a cell counts when any channel is not +0 / -0 (NaN counts).  _count
+ * flags the cells in one pass over the volume, scans the flags and writes the number of non-zero
+ * cells to *h_count (HOST) after a stream synchronise: the one blocking point, the caller needs it
+ * to size `coords`.  _coords then writes their indices (origin and step are not applied), int32
+ * [*h_count, ncols], in row-major (batch, X1..XD) order.  scratch:
+ * meb200_dense_nonzero_scratch_bytes(cells) bytes, cells = the product of desc->shape, at most
+ * 2^32 - 2049; the same scratch, untouched, goes to _coords. */
+uint64_t meb200_dense_nonzero_scratch_bytes(uint64_t cells);
+int meb200_dense_nonzero_count(const void *dense, int dtype, const meb200_dense_desc *desc,
+                               void *scratch, uint32_t *h_count, void *stream);
+int meb200_dense_nonzero_coords(const meb200_dense_desc *desc, void *scratch, int32_t *coords,
+                                void *stream);
+
 /* ---- tensor fields: points with float coordinates, quantised to voxels (reference:
  *      MinkowskiTensorField.py, CoordinateFieldMapCPU::quantize_coordinates
  *      coordinate_map_cpu.hpp:994-1037, interpolation_map_weight_kernel :139-240,

@@ -10,7 +10,8 @@ MinkowskiConvolutionTranspose, MinkowskiChannelwiseConvolution (depthwise), loca
 unpooling (MinkowskiPoolingTranspose), global pooling, broadcast, batch and instance
 normalisation, pruning, union and arithmetic between sparse tensors on different coordinate maps,
 TensorField (point features quantised to voxels or splatted onto their corners, sliced back and
-interpolated), and the thin torch wrappers (cat / sum / mean / var, the stack containers,
+interpolated), dense-tensor interop (SparseTensor.dense, MinkowskiToDenseTensor, to_sparse,
+to_sparse_all, dense_coordinates), and the thin torch wrappers (cat / sum / mean / var, the stack containers,
 MinkowskiToFeature) that MinkUNet, the ResNet classifiers and generative networks need.
 CUDA tensors only; all device work runs in csrc/libmeb200.so (include/meb200.h).
 """
@@ -53,4 +54,6 @@ from .tensor_field import TensorField
 from .interpolation import MinkowskiInterpolation, MinkowskiInterpolationFunction
 from .pruning import MinkowskiPruning, MinkowskiPruningFunction
 from .union import MinkowskiUnion, MinkowskiUnionFunction
+from .dense import (MinkowskiDenseToRowsFunction, MinkowskiToDenseFunction, MinkowskiToDenseTensor,
+                    dense_coordinates, to_sparse, to_sparse_all)
 from . import modules, utils  # noqa: F401

@@ -80,6 +80,11 @@ PROTOTYPES = {
     "meb200_union_fold_forward": (_i32, [_vp, _u32, _u32, _vp, _u32, _u32, _i32, _i32, _vp, _vp]),
     "meb200_union_fold_backward": (_i32, [_vp, _u32, _u32, _vp, _u32, _u32, _i32, _i32, _vp, _u32,
                                           _vp, _u32, _vp, _vp]),
+    "meb200_dense_from_rows": (_i32, [_vp, _i32, _u32, _vp, _vp, _u32, _vp, _vp, _vp]),
+    "meb200_dense_to_rows": (_i32, [_vp, _i32, _vp, _vp, _u32, _vp, _vp]),
+    "meb200_dense_nonzero_scratch_bytes": (_u64, [_u64]),
+    "meb200_dense_nonzero_count": (_i32, [_vp, _i32, _vp, _vp, C.POINTER(_u32), _vp]),
+    "meb200_dense_nonzero_coords": (_i32, [_vp, _vp, _vp, _vp]),
     "meb200_quantize_field": (_i32, [_vp, _u32, _u32, C.POINTER(C.c_int32), _vp, _vp, _vp]),
     "meb200_field_insert_and_map": (_i32, [_vp, _u32, _u32, C.POINTER(C.c_int32), _vp, _vp, _u32,
                                            _vp, _vp, _vp, _vp, C.POINTER(_u32), _vp]),

@@ -4,6 +4,7 @@
 import torch
 from torch.nn import Module
 
+from .dense import to_sparse, to_sparse_all
 from .sparse_tensor import (COORDINATE_KEY_DIFFERENT_ERROR, COORDINATE_MANAGER_DIFFERENT_ERROR,
                             SparseTensor)
 from .tensor_field import TensorField
@@ -128,13 +129,26 @@ class MinkowskiStackVar(torch.nn.Sequential):
 
 
 class MinkowskiToSparseTensor(Module):
-    """TensorField -> SparseTensor through `TensorField.sparse()` (a SparseTensor passes through)
-    (reference: MinkowskiOps.py:276-352)."""
+    """TensorField -> SparseTensor through `TensorField.sparse()` (a SparseTensor passes through);
+    a dense [B, C, X1..XD] torch.Tensor -> `to_sparse_all(input, coordinates)` when `coordinates`
+    are given (cache them with `dense_coordinates` for a fixed shape), else `to_sparse(input)`
+    when `remove_zeros`, else `to_sparse_all(input)` (reference: MinkowskiOps.py:351-411, as its
+    docstring has it)."""
+
+    def __init__(self, remove_zeros=True, coordinates=None):
+        super().__init__()
+        self.remove_zeros = remove_zeros
+        self.coordinates = coordinates
 
     def forward(self, input):
         if isinstance(input, TensorField):
             return input.sparse()
-        assert isinstance(input, SparseTensor), "Input must be a TensorField or a SparseTensor"
+        if isinstance(input, torch.Tensor):
+            if self.coordinates is not None:
+                return to_sparse_all(input, self.coordinates)
+            return to_sparse(input) if self.remove_zeros else to_sparse_all(input)
+        assert isinstance(input, SparseTensor), \
+            "Input must be a TensorField, a SparseTensor or a torch.Tensor"
         return input
 
     def __repr__(self):

@@ -387,26 +387,19 @@ class SparseTensor(Tensor):
                                                     self.coordinate_map_key, self._manager)[0]
 
     def dense(self, shape=None, min_coordinate=None, contract_stride=True):
-        """Dense [B, C, X1..XD] tensor (reference: MinkowskiSparseTensor.py:347-448)."""
-        ts = torch.tensor(self.tensor_stride, device=self.device, dtype=torch.int64)
-        coords = self.C.long()
-        b = coords[:, 0]
-        xyz = coords[:, 1:]
-        if min_coordinate is None:
-            min_coordinate = xyz.min(0).values if len(xyz) else torch.zeros_like(ts)
-        else:
-            min_coordinate = torch.as_tensor(min_coordinate, device=self.device).long().flatten()
-        xyz = xyz - min_coordinate
-        if contract_stride:
-            xyz = xyz // ts
-        nb = int(b.max().item()) + 1 if len(b) else 0
-        spatial = (xyz.max(0).values + 1).tolist() if len(xyz) else [0] * self._D
-        if shape is not None:
-            nb, spatial = shape[0], list(shape[2:])
-        dense = torch.zeros([nb, self._F.size(1)] + spatial, dtype=self.dtype, device=self.device)
-        idx = (b,) + tuple(xyz[:, i] for i in range(self._D))
-        dense.permute(0, *range(2, 2 + self._D), 1)[idx] = self._F
-        return dense, min_coordinate.int(), torch.tensor(self.tensor_stride, dtype=torch.int32)
+        """Dense [B, C, X1..XD] tensor, differentiable in the features (reference:
+        MinkowskiSparseTensor.py:460-557) -> (tensor, min_coordinate int32 [D], tensor stride int32
+        [D]).  Cell i of an axis holds coordinate min_coordinate + i * tensor_stride (+ i with
+        contract_stride=False, the cells between the voxels then zero).
+
+        shape: [B, C, X1..XD] of the result (its C is replaced by the feature width); the extent
+        of the coordinates when None.  Voxels outside the volume are cropped.
+        min_coordinate: D ints divisible by the tensor stride; the smallest coordinate of every
+        axis when None (negative coordinates are accepted, where the reference asks for a
+        min_coordinate).  With both given nothing is read back from the device; otherwise the
+        extent of the coordinates is, once."""
+        from .dense import sparse_to_dense
+        return sparse_to_dense(self, shape, min_coordinate, contract_stride)
 
 
 def _get_coordinate_map_key(input: SparseTensor, coordinates=None, tensor_stride=1,
