@@ -136,7 +136,9 @@ int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32
     if (rc != MEB200_OK) return rc;
   }
   if (grad_weight != nullptr) {
-    MEB_CHECK_ARG(out_nbr && (in || n_in == 0) && (grad_out || n_out == 0), "null buffer");
+    // an empty output map's table [K, 0] may be a null pointer: its weight gradient is zero
+    MEB_CHECK_ARG((out_nbr || n_out == 0) && (in || n_in == 0) && (grad_out || n_out == 0),
+                  "null buffer");
     if (pairs_in && pairs_out && seg_start && n_chunks > 0 &&
         conv_wgrad_uses_pairs(dtype, c_in, c_out, K)) {
       int rc = conv_wgrad_pairs(in, grad_out, dtype, c_in, K, c_out, pairs_in, pairs_out,

@@ -98,6 +98,15 @@ def assert_one_rounding(y, ref, A, what="", acc=1.0):
             f"|err| {err.flatten()[j].item():.3e} > bound {bound.flatten()[j].item():.3e}")
 
 
+def one_rounding_ratio(y, ref, A, acc=1.0):
+    """max |y - ref| / one_rounding_bound(ref, A, y.dtype, acc) over the elements with a nonzero
+    bound: how close the error comes to the bound (at most 1 passes)."""
+    err = (y.double() - ref.double()).abs()
+    bound = one_rounding_bound(ref, A, y.dtype, acc)
+    m = bound > 0
+    return float((err[m] / bound[m]).max()) if bool(m.any()) else 0.0
+
+
 # ---- convolution layers on random neighbour tables, and their float64 restatement --------------
 def _table(K, n_rows, n_other, density, seed, device):
     """Random k-major neighbour table [K, n_rows] with fully empty rows and an all-empty offset."""
@@ -173,11 +182,12 @@ class _Route:
 
 
 def lib_conv_backward(feats, gout, w, km, grad_in_dtype=None, need_w=False, pairs=False,
-                      workspace=None):
+                      workspace=None, grad_w=None):
     """One `meb200_conv_backward` call with the caller's choices, which `backend` makes itself:
     the dtype of grad_in (None: no dgrad; fp32 gives the accumulator before any rounding), the
     pair-list or the dense-table wgrad, and the workspace, given as a uint8 tensor (its size, or
-    None for no workspace).  Returns (grad_in, grad_w)."""
+    None for no workspace).  `grad_w`: the fp32 tensor the wgrad writes (default: a new one).
+    Returns (grad_in, grad_w)."""
     from minkowskiengine_b200 import _lib, backend
     lib = _lib.load()
     dt = feats.dtype
@@ -186,7 +196,10 @@ def lib_conv_backward(feats, gout, w, km, grad_in_dtype=None, need_w=False, pair
     w_cast, _ = backend._feature_weights(w, dt)
     gi = None if grad_in_dtype is None else \
         torch.empty((km.n_in, c_in), dtype=grad_in_dtype, device=feats.device)
-    gw = torch.empty((K, c_in, c_out), dtype=torch.float32, device=feats.device) if need_w else None
+    gw = None
+    if need_w:
+        gw = grad_w if grad_w is not None else \
+            torch.empty((K, c_in, c_out), dtype=torch.float32, device=feats.device)
     pin = pout = seg = None
     nch = 0
     if pairs:

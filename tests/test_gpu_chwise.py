@@ -1,5 +1,5 @@
 """Channel-wise (depthwise) convolution on the GPU: the native kernels (csrc/chwise.cu) against the
-float64 restatement (tests/chwise_oracle.py) element by element in bf16 / fp16, the public layer
+float64 restatement (tests/chwise_oracle.py) element by element in fp32, bf16 and fp16, the public layer
 against the compiled reference's fixtures (tests/golden/ref_chwise_*, written by
 tests/golden/make_chwise_fixtures.py), and one training step of examples/convnext.py against the
 reference's."""
@@ -8,7 +8,7 @@ import pytest
 import torch
 
 import chwise_oracle as CO
-from helpers import assert_one_rounding, golden, one_rounding_bound, rel_err, state_digest
+from helpers import assert_one_rounding, golden, one_rounding_ratio as _ratio, rel_err, state_digest
 from oracle import oracle_np as O
 
 pytestmark = pytest.mark.gpu
@@ -93,15 +93,6 @@ def _wgrad(x, g, nbr, workspace="plan"):
     return dW
 
 
-def _ratio(y, ref, A):
-    """max |y - ref| / bound over all elements, with the bound of assert_one_rounding (acc = 1):
-    how close the measured error comes to it (at most 1 passes)."""
-    err = (y.double() - ref.double()).abs()
-    bound = one_rounding_bound(ref, A, y.dtype)
-    m = bound > 0
-    return float((err[m] / bound[m]).max()) if bool(m.any()) else 0.0
-
-
 def _table(K, n_rows, n_other, density, seed, device):
     """Random k-major table [K, n_rows] with rows that have no neighbour and, for K > 2, an offset
     without any pair."""
@@ -143,9 +134,12 @@ def _check_all(x, go, W, out_nbr, in_nbr, what):
 
 
 # ---- the kernels, element by element -------------------------------------------------------------
+# fp32 reads 4-channel vectors when C % 4 == 0 (C = 4, 12, 20 among them), bf16 / fp16 8-channel
+# ones when C % 8 == 0; every other C reads single channels
 @pytest.mark.parametrize("K", [1, 27, 125, 343])
-@pytest.mark.parametrize("C", [1, 3, 8, 24, 64, 96, 200, 256, 512])
-@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16], ids=["bf16", "fp16"])
+@pytest.mark.parametrize("C", [1, 3, 4, 8, 12, 20, 24, 64, 96, 200, 256, 512])
+@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16, torch.float16],
+                         ids=["fp32", "bf16", "fp16"])
 def test_kernels_one_rounding(cuda, dtype, C, K):
     ops = _operands(C, K, 700, 500, dtype, cuda, 1000 + C + K)
     r = _check_all(*ops, f"{dtype} C={C} K={K}")
@@ -153,9 +147,10 @@ def test_kernels_one_rounding(cuda, dtype, C, K):
 
 
 @pytest.mark.parametrize("n_rows", [1, 255, 256, 257, 1023, 1024, 1025, 2049, 40_000])
-def test_row_counts_at_tile_and_split_edges(cuda, n_rows):
-    ops = _operands(64, 27, n_rows, 3000, torch.bfloat16, cuda, 7 + n_rows)
-    _check_all(*ops, f"n_rows={n_rows}")
+@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16], ids=["fp32", "bf16"])
+def test_row_counts_at_tile_and_split_edges(cuda, dtype, n_rows):
+    ops = _operands(64, 27, n_rows, 3000, dtype, cuda, 7 + n_rows)
+    _check_all(*ops, f"{dtype} n_rows={n_rows}")
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16], ids=["fp32", "bf16"])
@@ -173,22 +168,26 @@ def test_zero_rows_launch_nothing(cuda, dtype):
 
 
 def test_wgrad_workspace_full_small_and_none(cuda):
+    """fp32 (4-channel vectors) and bf16 (8-channel vectors)."""
     from minkowskiengine_b200 import _lib
-    x, go, W, out_nbr, _ = _operands(64, 27, 50_000, 20_000, torch.bfloat16, cuda, 5)
-    nbytes = int(_lib.load().meb200_chwise_wgrad_workspace_bytes(50_000, 64, 27, _lib.BF16))
-    slot = 27 * 64 * 4
-    assert nbytes >= 3 * slot, "the plan should split this layer's rows"
-    ref, A = CO.wgrad(x, go, out_nbr)
-    full = _wgrad(x, go, out_nbr)
-    small = _wgrad(x, go, out_nbr, torch.empty(2 * slot, dtype=torch.uint8, device=cuda))
-    none = _wgrad(x, go, out_nbr, None)
-    unaligned = _wgrad(x, go, out_nbr, torch.empty(nbytes + 16, dtype=torch.uint8,
-                                                   device=cuda)[8:8 + nbytes])
-    for what, dW in (("full", full), ("small", small), ("none", none), ("unaligned", unaligned)):
-        assert_one_rounding(dW, ref, A, f"workspace {what}")
-    assert torch.equal(none, unaligned)          # an unaligned workspace means one split
-    print(f"chwise wgrad ratio one split over 50k rows: {_ratio(none, ref, A):.3f}, "
-          f"planned splits: {_ratio(full, ref, A):.3f}")
+    for dtype in (torch.float32, torch.bfloat16):
+        x, go, W, out_nbr, _ = _operands(64, 27, 50_000, 20_000, dtype, cuda, 5)
+        nbytes = int(_lib.load().meb200_chwise_wgrad_workspace_bytes(50_000, 64, 27,
+                                                                     _lib.dtype_code(dtype)))
+        slot = 27 * 64 * 4
+        assert nbytes >= 3 * slot, f"{dtype}: the plan should split this layer's rows"
+        ref, A = CO.wgrad(x, go, out_nbr)
+        full = _wgrad(x, go, out_nbr)
+        small = _wgrad(x, go, out_nbr, torch.empty(2 * slot, dtype=torch.uint8, device=cuda))
+        none = _wgrad(x, go, out_nbr, None)
+        unaligned = _wgrad(x, go, out_nbr, torch.empty(nbytes + 16, dtype=torch.uint8,
+                                                       device=cuda)[8:8 + nbytes])
+        for what, dW in (("full", full), ("small", small), ("none", none),
+                         ("unaligned", unaligned)):
+            assert_one_rounding(dW, ref, A, f"{dtype} workspace {what}")
+        assert torch.equal(none, unaligned), dtype    # an unaligned workspace means one split
+        print(f"chwise wgrad ratio {dtype} one split over 50k rows: {_ratio(none, ref, A):.3f}, "
+              f"planned splits: {_ratio(full, ref, A):.3f}")
 
 
 # ---- the public layer ----------------------------------------------------------------------------

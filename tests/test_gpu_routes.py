@@ -1,5 +1,5 @@
-"""The convolution routes off the wgmma grid, in bf16 / fp16, against a float64 restatement on the
-device, element by element.
+"""The convolution routes off the wgmma grid, in fp32, bf16 and fp16, against a float64
+restatement on the device, element by element.
 
 `meb200_conv_{forward,backward}` send a layer to one of several kernels by dtype and channel
 counts: `k_conv_wg` / `k_wgrad_wg` (tensor cores) when every side is on the 16-channel grid,
@@ -7,7 +7,8 @@ counts: `k_conv_wg` / `k_wgrad_wg` (tensor cores) when every side is on the 16-c
 c_in <= 4, and mixtures (forward in 256-column tensor-core slices with a SIMT wgrad for c_out >
 256; SIMT dgrad with the dense-table `k_wgrad_wg` when only the wgrad qualifies).  Every case
 states which route it covers through the tensor-core launch counter, so that a change of dispatch
-cannot move a case to another route unnoticed.
+cannot move a case to another route unnoticed.  Under torch's default matmul switch, which this
+file pins, fp32 launches no tensor-core kernel in any case.
 
 Bound (tests/helpers.py): |y - ref| <= delta = 2^-20 * A in fp32 and one rounding on top of that in
 bf16 / fp16, A the same reduction over absolute values.  The weight gradients are fp32 and must be
@@ -15,14 +16,26 @@ bit-identical run to run: every split's partial sums are added in a fixed order.
 import pytest
 import torch
 
-from helpers import _Route, _inputs, _pairs, _table, assert_one_rounding, ref_conv, ref_wgrad
+from helpers import (_Route, _inputs, _pairs, _table, assert_one_rounding, one_rounding_ratio,
+                     ref_conv, ref_wgrad)
 from oracle import oracle_np as O
 
 pytestmark = pytest.mark.gpu
 
 
-# (cin, cout, n_in, n_out, K, forward on tensor cores, dgrad on tensor cores)
-# The wgrad of every case runs on CUDA cores: k_conv_small_cin_wgrad for cin <= 4, else k_conv_wgrad.
+@pytest.fixture(autouse=True)
+def exact_fp32():
+    """fp32 convolutions on the CUDA cores: torch's default matmul switch, restored afterwards."""
+    saved = torch.backends.cuda.matmul.fp32_precision
+    torch.backends.cuda.matmul.fp32_precision = "ieee"
+    yield
+    torch.backends.cuda.matmul.fp32_precision = saved
+
+
+# (cin, cout, n_in, n_out, K, forward on tensor cores, dgrad on tensor cores) in bf16 / fp16
+# The wgrad of every case runs on CUDA cores: k_conv_small_cin_wgrad for cin <= 4 and cout <= 64,
+# else k_conv_wgrad.  The last two have cout off the 16-channel grid, so that the bf16 / fp16 stem
+# kernels do not take them either.
 ROUTES = {
     "head_96to20_k1": (96, 20, 200_000, 200_000, 1, False, False),    # MinkUNet head
     "cout1": (16, 1, 20_000, 20_000, 27, False, False),              # completion classifiers
@@ -31,14 +44,20 @@ ROUTES = {
     "cout272_slices": (128, 272, 8_000, 8_000, 27, True, True),        # two column slices
     "cout512_slices": (64, 512, 8_000, 8_000, 8, True, True),
     "stem_3to20_k125": (3, 20, 50_000, 50_000, 125, False, False),   # k_conv_small_cin_*
+    # the small-cin forward's fallback to k_conv_gather_gemm: K * c_in * 64 fp32 weights > 200 KB
+    "stem_4to56_k343": (4, 56, 20_000, 20_000, 343, False, False),
+    "cin3_cout72": (3, 72, 20_000, 20_000, 27, False, False),        # c_out > 64: no small-cin
 }
 
 
-@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16], ids=["bf16", "fp16"])
+@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16, torch.float16],
+                         ids=["fp32", "bf16", "fp16"])
 @pytest.mark.parametrize("case", list(ROUTES))
 def test_route_forward_dgrad_wgrad(ME, cuda, case, dtype):
     from minkowskiengine_b200 import backend
     cin, cout, n_in, n_out, K, fwd_tc, dgrad_tc = ROUTES[case]
+    if dtype == torch.float32:
+        fwd_tc = dgrad_tc = False
     feats, gout, w = _inputs(cin, cout, n_in, n_out, K, dtype, cuda, seed=cin * 131 + cout)
     wl = w.to(dtype)
     out_nbr = _table(K, n_out, n_in, 0.35, seed=K + n_out, device=cuda)
@@ -47,7 +66,9 @@ def test_route_forward_dgrad_wgrad(ME, cuda, case, dtype):
     y_ref, y_A = ref_conv(feats, wl, _pairs(out_nbr), n_out)
     with _Route(fwd_tc, f"{case} forward"):
         y = backend._conv_forward(feats, w, km)
+        y2 = backend._conv_forward(feats, w, km)
         y32 = backend._conv_forward(feats, w, km, out_dtype=torch.float32)
+    assert torch.equal(y, y2), f"{case} forward differs run to run"
     assert y.dtype == dtype and y32.dtype == torch.float32
     assert_one_rounding(y, y_ref, y_A, f"{case} forward")
     assert_one_rounding(y32, y_ref, y_A, f"{case} forward, fp32 output")
@@ -55,8 +76,10 @@ def test_route_forward_dgrad_wgrad(ME, cuda, case, dtype):
     gi_ref, gi_A = ref_conv(gout, wl.transpose(1, 2), _pairs(in_nbr), n_in)
     with _Route(dgrad_tc, f"{case} dgrad"):
         gi, _ = backend._conv_backward(feats, gout, w, km, need_in=True, need_w=False)
+        gi2, _ = backend._conv_backward(feats, gout, w, km, need_in=True, need_w=False)
     assert gi.dtype == dtype
     assert_one_rounding(gi, gi_ref, gi_A, f"{case} dgrad")
+    assert torch.equal(gi, gi2), f"{case} dgrad differs run to run"
 
     gw_ref, gw_A = ref_wgrad(feats, gout, _pairs(out_nbr))
     with _Route(False, f"{case} wgrad"):
@@ -66,6 +89,9 @@ def test_route_forward_dgrad_wgrad(ME, cuda, case, dtype):
     assert gw.dtype == torch.float32
     assert_one_rounding(gw, gw_ref, gw_A, f"{case} wgrad")
     assert torch.equal(gw, gw2), f"{case} wgrad differs run to run"
+    print(f"route ratio {dtype} {case}: fwd {one_rounding_ratio(y32, y_ref, y_A):.3f} "
+          f"dgrad {one_rounding_ratio(gi, gi_ref, gi_A):.3f} "
+          f"wgrad {one_rounding_ratio(gw, gw_ref, gw_A):.3f}")
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16], ids=["bf16", "fp16"])

@@ -217,11 +217,31 @@ def _fwd_bwd(conv, x):
     return y
 
 
+def _tf32_rna(t):
+    """t rounded to the nearest tf32 value, ties away from zero, as cvt.rna rounds the packed
+    weights: add half of the lowest kept mantissa bit to the magnitude, then clear the 13 dropped
+    bits."""
+    return ((t.contiguous().view(torch.int32) + 0x1000) & ~0x1FFF).view(torch.float32)
+
+
+# Which directions of a layer run on the tensor cores under "tf32": (forward, dgrad, wgrad).
+# 24 -> 48 is split: its dgrad writes 24 columns, off the 16-column grid.
+_TF32_DIRECTIONS = {(32, 64): (True, True, True), (64, 32): (True, True, True),
+                    (3, 32): (False, False, False), (32, 20): (False, False, False),
+                    (24, 48): (True, False, True)}
+
+
 @pytest.mark.parametrize("cin,cout,tc", [(32, 64, True), (64, 32, True), (3, 32, False),
-                                         (32, 20, False)])
+                                         (32, 20, False), (24, 48, True)])
 def test_route_follows_the_switch(ME, cuda, cin, cout, tc):
     """Default switch: an fp32 convolution launches no tensor-core kernel, forward or backward.
-    "tf32": on-grid shapes launch some; the stem (c_in = 3) and c_out = 20 launch none."""
+    "tf32": on-grid shapes launch some; the stem (c_in = 3) and c_out = 20 launch none.
+
+    Per direction on the layer's kernel map, under "tf32": a forward or dgrad off the grid runs
+    the exact CUDA-core kernels on the packed weights, which are rounded to tf32, so it equals bit
+    for bit the default switch on the rounded weights; an off-grid wgrad reads no weights and
+    equals the default switch's."""
+    from minkowskiengine_b200 import backend
     saved = torch.backends.cuda.matmul.fp32_precision
     try:
         torch.backends.cuda.matmul.fp32_precision = "none"
@@ -232,6 +252,36 @@ def test_route_follows_the_switch(ME, cuda, cin, cout, tc):
         x.F.grad = None
         with _Route(tc, f"fp32 {cin}->{cout} tf32"):
             _fwd_bwd(conv, x)
+
+        key = x.coordinate_map_key
+        km = x.coordinate_manager._manager._kernel_map(
+            key, key, [3] * 3, [1] * 3, [1] * 3, ME.RegionType.HYPER_CUBE, torch.IntTensor(),
+            False, False)
+        feats = x.F.detach()
+        g = torch.Generator().manual_seed(cin + cout)
+        gout = (torch.rand(km.n_out, cout, generator=g) - 0.5).to(cuda)
+        fwd_tc, dgrad_tc, wgrad_tc = _TF32_DIRECTIONS[(cin, cout)]
+        with _Route(fwd_tc, f"tf32 {cin}->{cout} forward"):
+            y = backend._conv_forward(feats, conv.kernel, km)
+        with _Route(dgrad_tc, f"tf32 {cin}->{cout} dgrad"):
+            gi, _ = backend._conv_backward(feats, gout, conv.kernel, km, need_in=True, need_w=False)
+        with _Route(wgrad_tc, f"tf32 {cin}->{cout} wgrad"):
+            _, gw = backend._conv_backward(feats, gout, conv.kernel, km, need_in=False, need_w=True)
+
+        torch.backends.cuda.matmul.fp32_precision = "none"
+        w_rna = _tf32_rna(conv.kernel.detach())
+        assert not torch.equal(w_rna, conv.kernel.detach())     # the rounding changes something
+        with _Route(False, f"fp32 {cin}->{cout} default, per direction"):
+            y_rna = backend._conv_forward(feats, w_rna, km)
+            gi_rna, _ = backend._conv_backward(feats, gout, w_rna, km, need_in=True, need_w=False)
+            _, gw_exact = backend._conv_backward(feats, gout, conv.kernel, km, need_in=False,
+                                                 need_w=True)
+        if not fwd_tc:
+            assert torch.equal(y, y_rna), "off-grid tf32 forward differs from fp32 on tf32 weights"
+        if not dgrad_tc:
+            assert torch.equal(gi, gi_rna), "off-grid tf32 dgrad differs from fp32 on tf32 weights"
+        if not wgrad_tc:
+            assert torch.equal(gw, gw_exact), "off-grid tf32 wgrad differs from the fp32 wgrad"
     finally:
         torch.backends.cuda.matmul.fp32_precision = saved
 
