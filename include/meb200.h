@@ -494,14 +494,33 @@ int meb200_group_by_row(const int32_t *keys, uint32_t P, uint32_t M, int32_t *st
                         void *scratch, uint64_t scratch_bytes, void *stream);
 
 /* Points -> voxels.  For every output row r < M, over its entries j = perm[start[r] ..
- * start[r+1]) in order, with source row s = j / src_div and x = src[s, :] (times weight[j] when
- * weight != NULL): SUM the fp32 sum, AVG the sum over the exact count, MAX the maximum (the first
- * entry wins ties) with argmax[r, c] = s (int32 [M, C]).  A row without entries gives 0 (argmax
- * -1).  src: [n_src, C] in `dtype`, out: [M, C] in `dtype`.  Also the backward of a slice (SUM) and
- * of interpolation (SUM, weight = the interpolation weights, src_div = 2^D). */
+ * start[r+1]) in order, with source row s = src_row[j] (int32 [P]) when src_row != NULL, else
+ * s = j / src_div, and x = src[s, :] (times weight[j] when weight != NULL): SUM the fp32 sum, AVG
+ * the sum over the exact count, MAX the maximum (the first entry wins ties) with argmax[r, c] = the
+ * winning entry j (int32 [M, C]; its source row s when src_row == NULL and src_div == 1).  A row
+ * without entries gives 0 (argmax -1).  src: [n_src, C] in `dtype`, out:
+ * [M, C] in `dtype`; src_row values must lie in [0, n_src) (meb200_check_pairs).  Also the
+ * backward of a slice (SUM), of interpolation (SUM, weight = the interpolation weights, src_div =
+ * 2^D), and, with src_row = the column of each COO entry, a sparse matrix times a dense matrix
+ * (SUM, weight = the values), its row average (AVG) and max pooling over a pair list (MAX). */
 int meb200_field_reduce(const void *src, int dtype, uint32_t n_src, uint32_t C, const int32_t *perm,
-                        const int32_t *start, uint32_t M, const float *weight, uint32_t src_div,
-                        int mode, void *out, int32_t *argmax, void *stream);
+                        const int32_t *start, uint32_t M, const float *weight,
+                        const int32_t *src_row, uint32_t src_div, int mode, void *out,
+                        int32_t *argmax, void *stream);
+
+/* Range check of a pair list (int32 [P] each): every rows[p] in [0, n_rows) and cols[p] in
+ * [0, n_cols), else MEB200_ERR_INVALID.  The status word (d_status: DEVICE uint32, cleared by the
+ * call) is read back after a stream synchronise: the one blocking point of a call on a pair list
+ * the caller hands in. */
+int meb200_check_pairs(const int32_t *rows, const int32_t *cols, uint32_t P, uint32_t n_rows,
+                       uint32_t n_cols, uint32_t *d_status, void *stream);
+
+/* mask[r, c] = src_row[argmax[r, c]] * C + c, or -1 where argmax is -1 (argmax: int32 [M, C], the
+ * winning entries of a MAX meb200_field_reduce over a [n_src, C] source with per-entry source rows
+ * src_row; mask: [M, C] int32 or int64 by index_bits): the flat argmax of direct max pooling.  For
+ * int32, n_src * C must be at most 2^31 (the largest index n_src * C - 1 fits). */
+int meb200_flat_mask(const int32_t *argmax, const int32_t *src_row, uint32_t M, uint32_t C,
+                     uint32_t n_src, int index_bits, void *mask, void *stream);
 
 /* Voxels -> points: out[i, :] = g[inv[i], :] scaled per mode (inv: int64 [n]; -1 -> 0):
  * AVG  times 1 / (start[r+1] - start[r]);  MAX  kept where argmax[r, c] == i, else 0;

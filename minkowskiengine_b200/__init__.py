@@ -11,7 +11,8 @@ unpooling (MinkowskiPoolingTranspose), global pooling, broadcast, batch and inst
 normalisation, pruning, union and arithmetic between sparse tensors on different coordinate maps,
 TensorField (point features quantised to voxels or splatted onto their corners, sliced back and
 interpolated), dense-tensor interop (SparseTensor.dense, MinkowskiToDenseTensor, to_sparse,
-to_sparse_all, dense_coordinates), and the thin torch wrappers (cat / sum / mean / var, the stack containers,
+to_sparse_all, dense_coordinates), COO sparse-times-dense products (spmm, spmm_average) and max
+pooling over an explicit pair list, and the thin torch wrappers (cat / sum / mean / var, the stack containers,
 MinkowskiToFeature) that MinkUNet, the ResNet classifiers and generative networks need.
 CUDA tensors only; all device work runs in csrc/libmeb200.so (include/meb200.h).
 """
@@ -36,7 +37,8 @@ from .convolution import (MinkowskiConvolution, MinkowskiConvolutionFunction,
                           MinkowskiGenerativeConvolutionTranspose)
 from .channelwise_convolution import (MinkowskiChannelwiseConvolution,
                                       MinkowskiChannelwiseConvolutionFunction)
-from .pooling import (MinkowskiAvgPooling, MinkowskiGlobalAvgPooling, MinkowskiGlobalMaxPooling,
+from .pooling import (MinkowskiAvgPooling, MinkowskiDirectMaxPoolingFunction,
+                      MinkowskiGlobalAvgPooling, MinkowskiGlobalMaxPooling,
                       MinkowskiGlobalPooling, MinkowskiGlobalPoolingFunction,
                       MinkowskiGlobalSumPooling, MinkowskiLocalPoolingFunction,
                       MinkowskiLocalPoolingTransposeFunction, MinkowskiMaxPooling,
@@ -56,4 +58,6 @@ from .pruning import MinkowskiPruning, MinkowskiPruningFunction
 from .union import MinkowskiUnion, MinkowskiUnionFunction
 from .dense import (MinkowskiDenseToRowsFunction, MinkowskiToDenseFunction, MinkowskiToDenseTensor,
                     dense_coordinates, to_sparse, to_sparse_all)
+from .sparse_matrix_functions import (MinkowskiSPMMAverageFunction, MinkowskiSPMMFunction, spmm,
+                                      spmm_average)
 from . import modules, utils  # noqa: F401

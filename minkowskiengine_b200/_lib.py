@@ -90,8 +90,10 @@ PROTOTYPES = {
                                            _vp, _vp, _vp, _vp, C.POINTER(_u32), _vp]),
     "meb200_group_by_row_scratch_bytes": (_u64, [_u32, _u32]),
     "meb200_group_by_row": (_i32, [_vp, _u32, _u32, _vp, _vp, _vp, _u64, _vp]),
-    "meb200_field_reduce": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _u32, _vp, _u32, _i32, _vp, _vp,
-                                   _vp]),
+    "meb200_field_reduce": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _u32, _vp, _vp, _u32, _i32, _vp,
+                                   _vp, _vp]),
+    "meb200_check_pairs": (_i32, [_vp, _vp, _u32, _u32, _u32, _vp, _vp]),
+    "meb200_flat_mask": (_i32, [_vp, _vp, _u32, _u32, _u32, _i32, _vp, _vp]),
     "meb200_field_expand": (_i32, [_vp, _i32, _u32, _u32, _vp, _u32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "meb200_interp_map": (_i32, [_vp, _u32, _u32, C.POINTER(C.c_int32), _vp, _vp, _u32, _vp, _vp,
                                  _vp]),

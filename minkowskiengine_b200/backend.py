@@ -1982,9 +1982,10 @@ def group_by_row(keys, M):
     return start, perm
 
 
-def field_reduce(src, group, M, mode, weight=None, src_div=1):
+def field_reduce(src, group, M, mode, weight=None, src_div=1, src_row=None):
     """[M, C] reduction of the rows of `src` over a grouping (meb200_field_reduce) -> (out, argmax
-    int32 [M, C] for MAX else None)."""
+    int32 [M, C] for MAX else None).  Entry j reads row src_row[j] when src_row (int32, range
+    checked by the caller) is given, else row j // src_div."""
     src = src.contiguous()
     start, perm = group
     C = src.size(1)
@@ -1993,7 +1994,8 @@ def field_reduce(src, group, M, mode, weight=None, src_div=1):
         if mode == _lib.FIELD_MAX else None
     _lib.check(_lib.load().meb200_field_reduce(
         _lib.ptr(src), _lib.dtype_code(src.dtype), src.size(0), C, _lib.ptr(perm), _lib.ptr(start),
-        M, _lib.ptr(weight), src_div, mode, _lib.ptr(out), _lib.ptr(argmax), _lib.current_stream()))
+        M, _lib.ptr(weight), _lib.ptr(src_row), src_div, mode, _lib.ptr(out), _lib.ptr(argmax),
+        _lib.current_stream()))
     return out, argmax
 
 
@@ -2021,4 +2023,176 @@ def interp_forward(F, rows, w):
     _lib.check(_lib.load().meb200_interp_forward(
         _lib.ptr(F), _lib.dtype_code(F.dtype), F.size(0), F.size(1), _lib.ptr(rows), _lib.ptr(w), n,
         K, _lib.ptr(out), _lib.current_stream()))
+    return out
+
+
+# ---- COO sparse matrix times dense matrix, direct max pooling (pybind/extern.hpp:497-506, 654-665)
+_INDEX_LIMIT = 0x7FFFFFFF       # rows, columns and flat mask sizes are int32 keys below this
+
+
+def _index32(t):
+    """int32 form of an index tensor: int32 as it is; int64 and float as the reference's `.int()`
+    (float truncated towards zero), with values outside int32 clamped to -1 or 2^31 - 1 so that
+    they stay out of range instead of wrapping into it.  The caller's tensor is never written."""
+    t = t.reshape(-1)
+    if t.dtype == torch.int32:
+        return t.contiguous()
+    return t.long().clamp(-1, 2 ** 31 - 1).int()
+
+
+def _check_dim(n, what):
+    _assert(0 <= int(n) < _INDEX_LIMIT, what, "must lie in [0, 2^31 - 1), got", n)
+    return int(n)
+
+
+def _pair_list(rows, cols, n_rows, n_cols, device):
+    """int32 (rows, cols) of a pair list on `device`, every rows[p] in [0, n_rows) and cols[p] in
+    [0, n_cols) (meb200_check_pairs: one kernel and one host synchronisation), else RuntimeError."""
+    _assert(rows.is_cuda and cols.is_cuda, "index tensors must be CUDA (this backend has no CPU path)")
+    _assert(rows.device == device and cols.device == device, "all inputs must be on", device)
+    r, c = _index32(rows), _index32(cols)
+    _assert(r.numel() == c.numel(), "Invalid length", r.numel(), c.numel())
+    _assert(r.numel() < _INDEX_LIMIT, "too many entries:", r.numel())
+    status = torch.empty(1, dtype=torch.int32, device=device)
+    _lib.check(_lib.load().meb200_check_pairs(_lib.ptr(r), _lib.ptr(c), r.numel(), n_rows, n_cols,
+                                              _lib.ptr(status), _lib.current_stream()))
+    return r, c
+
+
+def _check_mat(mat, what="mat"):
+    _assert(mat.is_cuda, what, "must be CUDA (this backend has no CPU path)")
+    _assert(mat.dim() == 2, what, "must be a matrix, got shape", tuple(mat.shape))
+    _lib.dtype_code(mat.dtype)      # fp32 / bf16 / fp16, else BackendError
+    return mat.contiguous()
+
+
+def _coo_reduce(r, c, M, mat, mode, weight=None, group=None):
+    """[M, C] reduction over the entries (r[p], c[p]) of the rows mat[c[p]] into rows r[p], in entry
+    order (meb200_group_by_row + meb200_field_reduce with src_row = c) -> (out, argmax for MAX).
+    Without entries or channels nothing is launched: the output is 0 and argmax -1."""
+    C = mat.size(1)
+    if r.numel() == 0 or M == 0 or C == 0:
+        out = torch.zeros((M, C), dtype=mat.dtype, device=mat.device)
+        argmax = torch.full((M, C), -1, dtype=torch.int32, device=mat.device) \
+            if mode == _lib.FIELD_MAX else None
+        return out, argmax
+    if group is None:
+        group = group_by_row(r, M)
+    return field_reduce(mat, group, M, mode, weight=weight, src_row=c)
+
+
+def coo_spmm_int32(rows, cols, vals, dim_i, dim_j, mat, spmm_algorithm_id=1, is_sorted=False):
+    """[dim_i, C] = A @ mat for the COO matrix A (dim_i x dim_j) with entries vals[p] at
+    (rows[p], cols[p]): out[r] = sum over the entries of row r, in entry order, of
+    fp32(vals[p]) * mat[cols[p]], accumulated in fp32 and rounded once to mat's dtype.  Duplicate
+    entries are summed; a row without entries is 0.  Out-of-range indices raise RuntimeError, which
+    costs one host synchronisation.  `spmm_algorithm_id` (a cuSPARSE algorithm in the reference) and
+    `is_sorted` are accepted and ignored: the result does not depend on either."""
+    mat = _check_mat(mat)
+    dim_i, dim_j = _check_dim(dim_i, "dim_i"), _check_dim(dim_j, "dim_j")
+    _assert(mat.size(0) == dim_j, "mat must have dim_j =", dim_j, "rows, got", mat.size(0))
+    _assert(vals.dtype == mat.dtype, "dtype mismatch", vals.dtype, mat.dtype)
+    _assert(vals.device == mat.device, "device mismatch", vals.device, mat.device)
+    r, c = _pair_list(rows, cols, dim_i, dim_j, mat.device)
+    _assert(vals.numel() == r.numel(), "Invalid length", vals.numel(), r.numel())
+    w = vals.reshape(-1).float().contiguous()    # bf16 / fp16 values widen exactly
+    return _coo_reduce(r, c, dim_i, mat, _lib.FIELD_SUM, weight=w)[0]
+
+
+def coo_spmm_average_int32(rows, cols, dim_i, dim_j, mat, spmm_algorithm_id=1):
+    """[result, COO, vals]: result[r] = the mean of mat[cols[p]] over the entries of row r (the
+    fp32 sum over the exact count, rounded once; 0 without entries); COO = int64 [2, P] of the
+    entries stably sorted by row; vals = 1 / (entries of the row) in mat's dtype, so that
+    coo_spmm_int32(COO[1], COO[0], vals, dim_j, dim_i, g) is the backward.  Out-of-range indices
+    raise RuntimeError (one host synchronisation); `spmm_algorithm_id` is ignored."""
+    mat = _check_mat(mat)
+    dim_i, dim_j = _check_dim(dim_i, "dim_i"), _check_dim(dim_j, "dim_j")
+    _assert(mat.size(0) == dim_j, "mat must have dim_j =", dim_j, "rows, got", mat.size(0))
+    r, c = _pair_list(rows, cols, dim_i, dim_j, mat.device)
+    if r.numel() == 0:
+        out = torch.zeros((dim_i, mat.size(1)), dtype=mat.dtype, device=mat.device)
+        return [out, torch.zeros((2, 0), dtype=torch.int64, device=mat.device),
+                torch.zeros(0, dtype=mat.dtype, device=mat.device)]
+    start, perm = group_by_row(r, dim_i)
+    out, _ = _coo_reduce(r, c, dim_i, mat, _lib.FIELD_AVG, group=(start, perm))
+    order = perm.long()
+    coo = torch.stack((r[order], c[order])).long()
+    count = start[1:] - start[:-1]
+    vals = (1 / count[coo[0]]).to(mat.dtype)
+    return [out, coo, vals]
+
+
+def _direct_max_pool(in_map, out_map, in_feat, out_nrows, need_mask):
+    """Direct max pooling forward -> (out, mask or None, winner, out_rows, in_rows): winner int32
+    [out_nrows, C] is the winning pair of every output element (-1 for none), out_rows / in_rows the
+    range-checked int32 maps."""
+    _assert(in_feat.is_cuda, "in_feat must be CUDA (this backend has no CPU path)")
+    _assert(in_feat.dim() == 2, "in_feat must be a matrix, got shape", tuple(in_feat.shape))
+    n_in, C = _check_dim(in_feat.size(0), "in_nrows"), _check_dim(in_feat.size(1), "C")
+    M = _check_dim(out_nrows, "out_nrows")
+    bits = 64 if in_map.dtype == torch.int64 else 32
+    lib = _lib.load()
+    if need_mask:   # the size check of the flat mask (no launch without rows), before any copy
+        _lib.check(lib.meb200_flat_mask(None, None, 0, C, n_in, bits, None, _lib.current_stream()))
+    in_feat = _check_mat(in_feat, "in_feat")
+    o, i = _pair_list(out_map, in_map, M, n_in, in_feat.device)
+    out, winner = _coo_reduce(o, i, M, in_feat, _lib.FIELD_MAX)
+    mask = None
+    if need_mask:
+        mask = torch.empty((M, C), dtype=torch.int64 if bits == 64 else torch.int32,
+                           device=in_feat.device)
+        if o.numel() == 0:
+            mask.fill_(-1)
+        else:
+            _lib.check(lib.meb200_flat_mask(_lib.ptr(winner), _lib.ptr(i), M, C, n_in, bits,
+                                            _lib.ptr(mask), _lib.current_stream()))
+    return out, mask, winner, o, i
+
+
+def direct_max_pool_fw(in_map, out_map, in_feat, out_nrows, is_sorted=False):
+    """(out [out_nrows, C], mask [out_nrows, C]): out[o, c] = the maximum of in_feat[i, c] over the
+    pairs (in_map[p], out_map[p]) = (i, o), the first pair in list order winning a tie, and
+    mask[o, c] = i * C + c of that pair, in in_map's integer dtype (int32 for float maps).  An
+    output row without pairs is 0 with mask -1.  Out-of-range maps raise RuntimeError (one host
+    synchronisation), as does an int32 mask that cannot hold in_nrows * C - 1; `is_sorted` is
+    ignored."""
+    out, mask, _, _, _ = _direct_max_pool(in_map, out_map, in_feat, out_nrows, True)
+    return out, mask
+
+
+def direct_max_pool_bw(grad_out_feat, mask_index, in_nrows):
+    """grad_in [in_nrows, C]: grad_out[o, c] added at the flat input element mask[o, c] of the
+    forward, each (o, c) once.  The elements are grouped by their flat index (a stable radix sort of
+    out_nrows * C int32 keys) and each input element sums its own in ascending (o, c) order, so the
+    result is bit-identical run to run without atomics.  Mask entries outside [0, in_nrows * C), -1
+    among them, send no gradient.  The int32 keys limit in_nrows * C to below 2^31 - 1 whatever the
+    mask's dtype, which is stricter than the reference: MinkowskiDirectMaxPoolingFunction does not
+    go through here and has no such limit (direct_max_pool_pairs_bw)."""
+    g = _check_mat(grad_out_feat, "grad_out_feat")
+    _assert(mask_index.is_cuda and mask_index.device == g.device, "mask must be on", g.device)
+    _assert(tuple(mask_index.shape) == tuple(g.shape), "mask shape", tuple(mask_index.shape),
+            "differs from grad_out_feat", tuple(g.shape))
+    n_in, C = _check_dim(in_nrows, "in_nrows"), g.size(1)
+    M = n_in * C
+    _assert(M < _INDEX_LIMIT, "the flat mask in_nrows * C =", M, "must be below 2^31 - 1 here")
+    if g.numel() == 0 or M == 0:
+        return torch.zeros((n_in, C), dtype=g.dtype, device=g.device)
+    group = group_by_row(_index32(mask_index), M)
+    out, _ = field_reduce(g.view(-1, 1), group, M, _lib.FIELD_SUM)
+    return out.view(n_in, C)
+
+
+def direct_max_pool_pairs_bw(grad_out_feat, winner, out_rows, in_rows, in_nrows):
+    """The backward of _direct_max_pool from its winning pairs: every pair p takes
+    grad_out[out_rows[p], c] where it won (meb200_field_expand MAX over the P pairs, [P, C]), and
+    each input row sums its pairs in pair order (meb200_group_by_row over in_rows +
+    meb200_field_reduce SUM).  Each (o, c) has one winning pair, so it counts once even when a pair
+    repeats; bit-identical run to run, no atomics.  It sorts P keys where direct_max_pool_bw sorts
+    out_nrows * C (BASELINE.md §16)."""
+    g = grad_out_feat.contiguous()
+    C = g.size(1)
+    if in_rows.numel() == 0 or C == 0:
+        return torch.zeros((in_nrows, C), dtype=g.dtype, device=g.device)
+    per_pair = field_expand(g, out_rows.long(), _lib.FIELD_MAX, argmax=winner)
+    out, _ = field_reduce(per_pair, group_by_row(in_rows, in_nrows), in_nrows, _lib.FIELD_SUM)
     return out

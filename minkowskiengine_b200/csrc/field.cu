@@ -95,7 +95,8 @@ template <typename T, int V, int MODE, bool WEIGHTED>
 __global__ void __launch_bounds__(256)
 k_field_reduce(const T *__restrict__ src, uint32_t C, const int32_t *__restrict__ perm,
                const int32_t *__restrict__ start, uint32_t M, const float *__restrict__ weight,
-               uint32_t src_div, T *__restrict__ out, int32_t *__restrict__ argmax) {
+               const int32_t *__restrict__ src_row, uint32_t src_div, T *__restrict__ out,
+               int32_t *__restrict__ argmax) {
   uint32_t CV = C / V;
   uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= (uint64_t)M * CV) return;
@@ -110,7 +111,7 @@ k_field_reduce(const T *__restrict__ src, uint32_t C, const int32_t *__restrict_
   }
   for (int32_t j = b; j < e; ++j) {
     uint32_t p = (uint32_t)__ldg(perm + j);
-    uint32_t s = p / src_div;
+    uint32_t s = src_row != nullptr ? (uint32_t)__ldg(src_row + p) : p / src_div;
     float x[V];
     load_f32<T, V>(src + (size_t)s * C + c, x);
     if (WEIGHTED) {
@@ -123,7 +124,7 @@ k_field_reduce(const T *__restrict__ src, uint32_t C, const int32_t *__restrict_
       if (MODE == MEB200_FIELD_MAX) {
         if (j == b || x[v] > acc[v]) {  // strict: the first point of the voxel wins a tie
           acc[v] = x[v];
-          arg[v] = (int32_t)s;
+          arg[v] = (int32_t)p;
         }
       } else {
         acc[v] = __fadd_rn(acc[v], x[v]);
@@ -140,6 +141,29 @@ k_field_reduce(const T *__restrict__ src, uint32_t C, const int32_t *__restrict_
 #pragma unroll
     for (int v = 0; v < V; ++v) argmax[(size_t)r * C + c + v] = arg[v];
   }
+}
+
+// Status bits of a pair list: 1 = a row outside [0, n_rows), 2 = a column outside [0, n_cols).
+__global__ void __launch_bounds__(256)
+k_check_pairs(const int32_t *__restrict__ rows, const int32_t *__restrict__ cols, uint32_t P,
+              uint32_t n_rows, uint32_t n_cols, uint32_t *__restrict__ bad) {
+  uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  uint32_t status = ((uint32_t)__ldg(rows + p) >= n_rows ? 1u : 0u) |
+                    ((uint32_t)__ldg(cols + p) >= n_cols ? 2u : 0u);  // negatives wrap past the end
+  if (status != 0) atomicOr(bad, status);  // flags, not a sum: any order, same word
+}
+
+// The MAX argmax (the winning entry, -1 for none) as the flat index src_row[entry] * C + c of a
+// [n_src, C] input.
+template <typename I>
+__global__ void __launch_bounds__(256)
+k_flat_mask(const int32_t *__restrict__ argmax, const int32_t *__restrict__ src_row, uint64_t n,
+            uint32_t C, I *__restrict__ mask) {
+  uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  int32_t a = __ldg(argmax + t);
+  mask[t] = a < 0 ? (I)-1 : (I)__ldg(src_row + a) * (I)C + (I)(t % C);
 }
 
 // ---- voxels -> points ---------------------------------------------------------------------------
@@ -272,14 +296,14 @@ k_interp_fwd(const T *__restrict__ F, uint32_t C, const int32_t *__restrict__ ro
 // ---- host dispatch ------------------------------------------------------------------------------
 template <typename T, int V>
 static void reduce_launch(const void *src, uint32_t C, const int32_t *perm, const int32_t *start,
-                          uint32_t M, const float *weight, uint32_t src_div, int mode, void *out,
-                          int32_t *argmax, cudaStream_t st) {
+                          uint32_t M, const float *weight, const int32_t *src_row, uint32_t src_div,
+                          int mode, void *out, int32_t *argmax, cudaStream_t st) {
   unsigned blocks = cdiv((uint64_t)M * (C / V), 256);
   const T *s = (const T *)src;
   T *o = (T *)out;
 #define MEB_REDUCE(MODE, W)                                                                 \
-  k_field_reduce<T, V, MODE, W><<<blocks, 256, 0, st>>>(s, C, perm, start, M, weight, src_div, o, \
-                                                        argmax)
+  k_field_reduce<T, V, MODE, W><<<blocks, 256, 0, st>>>(s, C, perm, start, M, weight, src_row, \
+                                                        src_div, o, argmax)
   if (mode == MEB200_FIELD_MAX) {
     MEB_REDUCE(MEB200_FIELD_MAX, false);
   } else if (mode == MEB200_FIELD_AVG) {
@@ -398,8 +422,9 @@ int meb200_group_by_row(const int32_t *keys, uint32_t P, uint32_t M, int32_t *st
 }
 
 int meb200_field_reduce(const void *src, int dtype, uint32_t n_src, uint32_t C, const int32_t *perm,
-                        const int32_t *start, uint32_t M, const float *weight, uint32_t src_div,
-                        int mode, void *out, int32_t *argmax, void *stream) {
+                        const int32_t *start, uint32_t M, const float *weight,
+                        const int32_t *src_row, uint32_t src_div, int mode, void *out,
+                        int32_t *argmax, void *stream) {
   if (M == 0 || C == 0) return MEB200_OK;
   MEB_CHECK_ARG(mode == MEB200_FIELD_SUM || mode == MEB200_FIELD_AVG || mode == MEB200_FIELD_MAX,
                 "mode %d is not a reduction", mode);
@@ -410,7 +435,42 @@ int meb200_field_reduce(const void *src, int dtype, uint32_t n_src, uint32_t C, 
   cudaStream_t s = (cudaStream_t)stream;
   MEB_DISPATCH_DTYPE(dtype, MEB_DISPATCH_VEC(T, C, aligned(16, src, out),
                                              reduce_launch<T, V>(src, C, perm, start, M, weight,
-                                                                 src_div, mode, out, argmax, s)));
+                                                                 src_row, src_div, mode, out,
+                                                                 argmax, s)));
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
+}
+
+int meb200_check_pairs(const int32_t *rows, const int32_t *cols, uint32_t P, uint32_t n_rows,
+                       uint32_t n_cols, uint32_t *d_status, void *stream) {
+  if (P == 0) return MEB200_OK;
+  MEB_CHECK_ARG(rows && cols && d_status, "null buffer");
+  cudaStream_t s = (cudaStream_t)stream;
+  MEB_CUDA(cudaMemsetAsync(d_status, 0, 4, s));
+  k_check_pairs<<<cdiv(P, 256), 256, 0, s>>>(rows, cols, P, n_rows, n_cols, d_status);
+  MEB_LAUNCH_OK();
+  uint32_t h = 0;
+  MEB_CUDA(cudaMemcpyAsync(&h, d_status, 4, cudaMemcpyDeviceToHost, s));
+  MEB_CUDA(cudaStreamSynchronize(s));
+  MEB_CHECK_ARG((h & 1u) == 0, "a row index is outside [0, %u)", n_rows);
+  MEB_CHECK_ARG((h & 2u) == 0, "a column index is outside [0, %u)", n_cols);
+  return MEB200_OK;
+}
+
+int meb200_flat_mask(const int32_t *argmax, const int32_t *src_row, uint32_t M, uint32_t C,
+                     uint32_t n_src, int index_bits, void *mask, void *stream) {
+  MEB_CHECK_ARG(index_bits == 32 || index_bits == 64, "index_bits=%d", index_bits);
+  uint64_t flat = (uint64_t)n_src * C;  // the largest index is flat - 1
+  MEB_CHECK_ARG(index_bits == 64 || flat <= 0x80000000ull,
+                "the flat mask n_src * C = %llu does not fit int32", (unsigned long long)flat);
+  uint64_t n = (uint64_t)M * C;
+  if (n == 0) return MEB200_OK;
+  MEB_CHECK_ARG(argmax && src_row && mask, "null buffer");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (index_bits == 32)
+    k_flat_mask<int32_t><<<cdiv(n, 256), 256, 0, s>>>(argmax, src_row, n, C, (int32_t *)mask);
+  else
+    k_flat_mask<int64_t><<<cdiv(n, 256), 256, 0, s>>>(argmax, src_row, n, C, (int64_t *)mask);
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }

@@ -234,3 +234,27 @@ class MinkowskiGlobalMaxPooling(MinkowskiGlobalPooling):
 
     def __init__(self, mode=PoolingMode.GLOBAL_MAX_POOLING_PYTORCH_INDEX):
         MinkowskiGlobalPooling.__init__(self, mode=mode)
+
+
+class MinkowskiDirectMaxPoolingFunction(Function):
+    """Max pooling over an explicit pair list (reference: MinkowskiPooling.py:752-780):
+    out[o, c] = the maximum of in_feat[i, c] over the pairs (in_map[p], out_map[p]) = (i, o).
+    The first pair in list order wins a tie; an output row without pairs is 0 and sends no
+    gradient; a repeated pair counts once.  The backward walks the winning pairs rather than the
+    reference's flat mask, which the forward does not build.  Maps may be int32, int64 or float;
+    out-of-range maps raise RuntimeError (one host synchronisation); `is_sorted` is ignored."""
+
+    @staticmethod
+    def forward(ctx, in_map: torch.Tensor, out_map: torch.Tensor, in_feat: torch.Tensor,
+                out_nrows: int, is_sorted: bool = False):
+        out_feat, _, winner, out_rows, in_rows = _C._direct_max_pool(in_map, out_map, in_feat,
+                                                                     out_nrows, False)
+        ctx.in_nrows = in_feat.size(0)
+        ctx.save_for_backward(winner, out_rows, in_rows)
+        return out_feat
+
+    @staticmethod
+    def backward(ctx, grad_out_feat):
+        winner, out_rows, in_rows = ctx.saved_tensors
+        grad = _C.direct_max_pool_pairs_bw(grad_out_feat, winner, out_rows, in_rows, ctx.in_nrows)
+        return None, None, grad, None, None
