@@ -70,11 +70,12 @@ __device__ __forceinline__ uint8_t *align1k(uint8_t *p) {
 // =====================================================================================
 struct FwdParams {
   const void *A;          // [n_a, c_red] gathered operand (stem: [n_a, 4])
-  const void *B;          // [K][*][c_red] operand B (reduction contiguous), at this slice's row 0
+  const void *B;          // [K][*][c_red] operand B (reduction contiguous), at this launch's row 0
   const int32_t *nbr;     // [K, n_rows]
-  void *out;              // [n_rows, out_ld], at this slice's column 0
+  void *out;              // [n_rows, out_ld], at this launch's column 0
   uint64_t b_k_stride;    // elements between the offsets of B
-  uint32_t c_red, c_cols, K, n_rows;
+  uint32_t c_red, K, n_rows;
+  uint32_t c_cols;        // columns of one CTA: column slice blockIdx.y starts at blockIdx.y * c_cols
   uint32_t n_a;           // rows of A (gather indices >= n_a read as zero rows)
   uint32_t out_ld, bk, out_f32;
   uint32_t stem_K;        // > 0: network stem, virtual channel 4 k + c = A[nbr[k][r]][c], k < stem_K
@@ -85,6 +86,7 @@ struct FwdParams {
 };
 
 // NT wgmma instructions of N = NI columns each cover the c_cols = NI * NT columns of the slice.
+// grid = (128-row tiles, column slices).
 template <typename T, int NI, int NT>
 __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -100,7 +102,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
   const uint32_t tmask = ordered ? __ldg(p.tile_mask + blockIdx.x) : 0u;
   const uint32_t nch = p.c_red / bk, n_st = (ordered ? __popc(tmask) : p.K) * nch;
   const T *A = reinterpret_cast<const T *>(p.A);
-  const T *B = reinterpret_cast<const T *>(p.B);
+  const T *B = reinterpret_cast<const T *>(p.B) + (size_t)blockIdx.y * p.c_cols * p.c_red;
+  const uint32_t col0 = blockIdx.y * p.c_cols;
   const uint32_t ar = tid >> 1, arow = row0 + ar;     // two threads per tile row of A
   const bool row_ok = arow < p.n_rows;
 
@@ -183,7 +186,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
     for (int i = 0; i < NT; ++i)
 #pragma unroll
       for (int j = 0; j < NI / 8; ++j) {
-        const uint32_t col = i * NI + 8 * j + 2 * t;
+        const uint32_t col = col0 + i * NI + 8 * j + 2 * t;
         const float v0 = acc[i][4 * j + 2 * h], v1 = acc[i][4 * j + 2 * h + 1];
         if (kIsTf32<T> || p.out_f32)
           *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + (size_t)orow * p.out_ld + col) =
@@ -643,27 +646,31 @@ static int ensure_big_smem(const void *fn) {
   }
 
 template <typename T, int NI, int NT>
-static int launch_fwd(const FwdParams &p, cudaStream_t stream) {
+static int launch_fwd(const FwdParams &p, uint32_t slices, cudaStream_t stream) {
   auto kern = k_conv_wg<T, NI, NT>;
   MEB_BIG_SMEM(kern);
-  kern<<<cdiv(p.n_rows, tc::kFwdRows), kThreads, tc::fwd_ring_bytes(p.bk * sizeof(T), p.c_cols),
-         stream>>>(p);
+  const dim3 grid(cdiv(p.n_rows, tc::kFwdRows), slices);
+  kern<<<grid, kThreads, tc::fwd_ring_bytes(p.bk * sizeof(T), p.c_cols), stream>>>(p);
   count_tc_launch();
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
 template <typename T>
-static int dispatch_fwd(const FwdParams &p, cudaStream_t stream) {
-#define MEB_L(NI, NT) launch_fwd<T, NI, NT>(p, stream)
+static int dispatch_fwd(const FwdParams &p, uint32_t slices, cudaStream_t stream) {
+#define MEB_L(NI, NT) launch_fwd<T, NI, NT>(p, slices, stream)
   MEB_COLS_DISPATCH(p.c_cols, MEB_L)
 #undef MEB_L
   set_error("conv tc: %u output columns per launch", p.c_cols);
   return MEB200_ERR_UNSUPPORTED;
 }
-static int run_fwd(int dtype, const FwdParams &p, cudaStream_t stream) {
-  if (dtype == MEB200_TF32) return dispatch_fwd<float>(p, stream);
-  return dtype == MEB200_BF16 ? dispatch_fwd<__nv_bfloat16>(p, stream)
-                              : dispatch_fwd<__half>(p, stream);
+// p.c_cols = all the launch's columns (<= 256): the launch runs them in the chooser's slices
+static int run_fwd(int dtype, FwdParams p, cudaStream_t stream) {
+  const uint32_t cols = p.c_cols;
+  p.c_cols = tc::fwd_col_slice(p.n_rows, cols, (uint32_t)num_sms());
+  const uint32_t slices = cols / p.c_cols;
+  if (dtype == MEB200_TF32) return dispatch_fwd<float>(p, slices, stream);
+  return dtype == MEB200_BF16 ? dispatch_fwd<__nv_bfloat16>(p, slices, stream)
+                              : dispatch_fwd<__half>(p, slices, stream);
 }
 
 template <typename T, int NI, int NT>
@@ -761,7 +768,7 @@ int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, c
   }
   const uint8_t *Wb = reinterpret_cast<const uint8_t *>(B);
   const bool ordered = order != nullptr && K <= kMaxOrderK;
-  // one launch per slice of <= 256 output columns
+  // one launch per <= 256 output columns
   const size_t out_esz = out_dtype == MEB200_F32 ? 4 : 2, esz = operand_bytes(dtype);
   for (uint32_t n0 = 0; n0 < c_cols; n0 += tc::kMaxCols) {
     FwdParams p{};

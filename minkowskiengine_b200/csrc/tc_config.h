@@ -1,6 +1,6 @@
 // Host-side launch configuration of the wgmma kernels (plain C++, no CUDA): stage widths,
 // shared-memory footprints and row splits.  Kept separate so it can be unit-tested on a machine
-// without a GPU (tests/test_tc_config.py).
+// without a GPU (tests/test_tc_config.py, tests/test_tc_col_slices.py).
 #pragma once
 #include <stdint.h>
 
@@ -30,6 +30,28 @@ inline uint32_t fwd_ring_bytes(uint32_t width, uint32_t c_cols) {
 // 16-bit elements: reduction channels per stage (64, 32 or 16), 0 = unsupported
 inline uint32_t fwd_bk(uint32_t c_red) { return fwd_stage_bytes(c_red, 2) / 2; }
 inline uint32_t fwd_smem_bytes(uint32_t bk, uint32_t c_cols) { return fwd_ring_bytes(bk * 2, c_cols); }
+
+// N of the wgmma instructions that cover c_cols columns: the widest of 64, 32, 16 dividing it
+// (MEB_COLS_DISPATCH in conv_tc.cu)
+inline uint32_t wgmma_n(uint32_t c_cols) {
+  return c_cols % 64 == 0 ? 64 : (c_cols % 32 == 0 ? 32 : 16);
+}
+
+// forward / dgrad: columns each CTA computes of a launch's c_cols (<= kMaxCols) output columns;
+// the launch runs c_cols / slice CTAs per 128-row tile (blockIdx.y = slice).  A launch with few
+// row tiles (the coarse levels of a U-Net) takes the narrowest slice that keeps its CTAs within
+// one per SM: more CTAs, each with a fraction of the MMAs and of the weight bytes, for the same
+// gathered rows (which such small levels keep in L2).  A CTA's time is mostly its stages'
+// gathers and barriers, not its MMAs, so slices that spill into a second wave of CTAs cost more
+// than they save (measured on an H100: BASELINE.md section 17).  The slice is a multiple of
+// wgmma_n(c_cols) dividing c_cols, so an output element is the same sequence of m64nNk16
+// instructions on the same operands either way: slicing does not change a bit.
+inline uint32_t fwd_col_slice(uint32_t n_rows, uint32_t c_cols, uint32_t n_sms) {
+  const uint64_t tiles = cdiv_u(n_rows, kFwdRows), n = wgmma_n(c_cols);
+  for (uint32_t s = n; s < c_cols; s += n)
+    if (c_cols % s == 0 && tiles * (c_cols / s) <= n_sms) return s;
+  return c_cols;
+}
 
 // one stage = A [64 rows x 128 channels] + B [64 rows x c_out], 16-bit elements
 inline uint32_t wgrad_smem_bytes(uint32_t c_out) {

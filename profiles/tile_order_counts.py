@@ -6,7 +6,11 @@ the bench's clouds, with and without the tile order of meb200_kernel_map.  CPU o
 Per stride level of MinkUNet34C, for the k3 table of the level and for the k2s2 tables between
 the level and the next: `dense` = every offset for every tile (no order), `natural` = only the
 offsets a tile reaches in the map's own row order, `sorted` = the same after the stable sort by
-neighbour mask, `bound` = pairs / 128 (every tile full of pairs).
+neighbour mask, `sorted, 256 rows` = the same sorted order cut into 256-row tiles, `bound` =
+pairs / 128 (every tile full of pairs).  A per-layer table then gives the bytes one forward call
+copies from L2 into shared memory: A = the gathered rows (pairs x c_red x 2), B = the offset's
+weight slice for all columns, once per stage (stages x c_cols x c_red x 2), at 128- and 256-row
+tiles.
 
 A second table counts the pair-mode weight gradient's 64-pair stages on the same tables (pair-list
 chunks of 262144 rows, one 128-channel tile, CTA time proportional to its stages, CTAs placed in
@@ -53,9 +57,9 @@ def _masks(out_c, in_c, offsets):
     return m
 
 
-def _stages(masks):
-    t = np.zeros((len(masks) + TILE - 1) // TILE, dtype=np.int64)
-    np.bitwise_or.at(t, np.arange(len(masks)) // TILE, masks)
+def _stages(masks, tile=TILE):
+    t = np.zeros((len(masks) + tile - 1) // tile, dtype=np.int64)
+    np.bitwise_or.at(t, np.arange(len(masks)) // tile, masks)
     return int(sum(bin(int(v)).count("1") for v in t))
 
 
@@ -63,12 +67,19 @@ def _row(name, masks, K):
     n = len(masks)
     pairs = int(sum(bin(int(v)).count("1") for v in masks))
     dense = (n + TILE - 1) // TILE * K
-    nat, srt = _stages(masks), _stages(masks[np.argsort(masks, kind="stable")])
-    print(f"| {name} | {n:,} | {pairs / n:.2f} | {dense:,} | {nat:,} | **{srt:,}** | {pairs / TILE:,.0f} |")
-    return dense, srt, pairs / TILE
+    srt_masks = masks[np.argsort(masks, kind="stable")]
+    nat, srt, srt256 = _stages(masks), _stages(srt_masks), _stages(srt_masks, 2 * TILE)
+    print(f"| {name} | {n:,} | {pairs / n:.2f} | {dense:,} | {nat:,} | **{srt:,}** | {srt256:,} | "
+          f"{pairs / TILE:,.0f} |")
+    return pairs, srt, srt256
 
 
 WG_STAGE, WG_CHUNK, SMS = 64, 262144, 132
+# MinkUNet34C k3 layers of the byte table: (name, stride level, c_red, c_cols); a forward reduces
+# over c_in into c_out columns (the dgrad of c_in -> c_out reduces over c_out into c_in columns)
+LAYER_BYTES = [("block8 96→96", 1, 96, 96), ("block8 128→96", 1, 128, 96),
+               ("block7 96→96", 2, 96, 96), ("block4 256→256", 16, 256, 256),
+               ("block3 128→128", 8, 128, 128)]
 
 
 def _wgrad_stages(masks, K):
@@ -119,16 +130,16 @@ def main():
     coords = coords.numpy()
     k3 = [(x, y, z) for x in (-1, 0, 1) for y in (-1, 0, 1) for z in (-1, 0, 1)]
     k2 = [(x, y, z) for x in (0, 1) for y in (0, 1) for z in (0, 1)]
-    print("| table | rows | nbrs/row | dense | natural | sorted by mask | bound |")
-    print("|---|---|---|---|---|---|---|")
+    print("| table | rows | nbrs/row | dense | natural | sorted by mask | sorted, 256 rows | bound |")
+    print("|---|---|---|---|---|---|---|---|")
     levels = [coords]
     for ts in (2, 4, 8, 16):
         levels.append(_strided(levels[-1], ts))
-    tables = []
+    tables, counts = [], {}
     for i, c in enumerate(levels):
         ts = 2 ** i
         tables.append((f"k3, stride {ts}", _masks(c, c, np.array(k3) * ts), 27))
-        _row(*tables[-1])
+        counts[ts] = _row(*tables[-1])
         if i + 1 < len(levels):
             coarse = levels[i + 1]
             # strided k2s2: coarse rows gather fine rows; transposed: fine rows gather one coarse row
@@ -137,6 +148,15 @@ def main():
             tables.append((f"k2s2 transposed {2 * ts} → {ts}",
                            _masks(c, coarse, -np.array(k2) * ts), 8))
             _row(*tables[-1])
+    print()
+    print("L2 -> shared-memory bytes of one forward call, GB (16-bit operands):")
+    print()
+    print("| layer (k3) | stride | c_red → c_cols | A | B, 128-row tiles | B, 256-row tiles |")
+    print("|---|---|---|---|---|---|")
+    for name, ts, c_red, c_cols in LAYER_BYTES:
+        pairs, st128, st256 = counts[ts]
+        print(f"| {name} | {ts} | {c_red} → {c_cols} | {pairs * c_red * 2 / 1e9:.2f} | "
+              f"{st128 * c_cols * c_red * 2 / 1e9:.2f} | {st256 * c_cols * c_red * 2 / 1e9:.2f} |")
     print()
     print(f"wgrad stages (makespan of the slowest of {a.resident} CTA slots):")
     print()
