@@ -262,7 +262,12 @@ __device__ __forceinline__ void wgrad_unit(const WgParams &p, uint32_t k, uint32
     wg_range(p, k, c, lo, hi);
     n_st += (hi - lo + tc::kWgRows - 1) / tc::kWgRows;
   }
-  // producer cursor: stage [pos, min(pos + 64, end)) of chunk wc
+  // Thread tid copies tile row ar = tid / 4 of both operands, chunks (tid & 3) + 4m.  Its two
+  // index words per stage are loaded a stage before the copies that use them (fetch), so that no
+  // copy waits on a global load: the loads of stage s + 3 are in flight over stage s's MMAs and
+  // the next barrier.
+  const uint32_t ar = tid >> 2;
+  // index cursor: the next stage to fetch is [pos, min(pos + 64, end)) of chunk wc
   uint32_t wc = 0, pos = 0, end = 0;
   auto open = [&]() {
     for (; wc < n_chunks; ++wc) {
@@ -271,48 +276,61 @@ __device__ __forceinline__ void wgrad_unit(const WgParams &p, uint32_t k, uint32
     }
   };
   open();
-
-  const uint32_t ar = tid >> 2;         // four threads per A row
-  auto load = [&](uint32_t s) {
-    const uint32_t base = s0 + (s % kStages) * stage_bytes;
-    const uint32_t e = pos;             // this stage's first pair
-    if (p.stem_K == 0) {
-      int32_t src = -1;
-      if (e + ar < end)
-        src = p.pin != nullptr ? __ldg(p.pin + e + ar) : __ldg(p.nbr + (size_t)k * p.n_out + e + ar);
-      const bool ok = src >= 0 && (uint32_t)src < p.n_in;
-      const T *rp = In + (size_t)(ok ? src : 0) * p.c_in + ci0;
-#pragma unroll
-      for (uint32_t m = 0; m < 4; ++m) {
-        const uint32_t j = (tid & 3u) + 4 * m;
-        const bool okj = ok && ci0 + 8 * j < p.c_in;
-        cp_async16(base + cm_off(ar, j, kChA), okj ? rp + 8 * j : In, okj ? 16u : 0u);
+  // row ar of the next stage: src = input row (unused in stem mode), o = dOut row; -1 past the end
+  struct Words { int32_t src, o; };
+  auto fetch = [&]() {
+    Words w{-1, -1};
+    const uint32_t r = pos + ar;
+    if (r < end) {
+      if (p.pin != nullptr) {
+        w.src = __ldg(p.pin + r);
+        w.o = __ldg(p.pout + r);
+      } else {
+        if (p.stem_K == 0) w.src = __ldg(p.nbr + (size_t)k * p.n_out + r);
+        w.o = (int32_t)r;
       }
-    } else {
-#pragma unroll
-      for (uint32_t m = 0; m < 4; ++m) {
-        const uint32_t j = (tid & 3u) + 4 * m;
-#pragma unroll
-        for (uint32_t h = 0; h < 2; ++h) {
-          const uint32_t kk = (ci0 + 8 * j) / 4 + h;
-          const int32_t src = (e + ar < end && kk < p.stem_K)
-                                  ? __ldg(p.nbr + (size_t)kk * p.n_out + e + ar) : -1;
-          const bool ok = src >= 0 && (uint32_t)src < p.n_in;
-          cp_async8(base + cm_off(ar, j, kChA) + 8 * h, In + (size_t)(ok ? src : 0) * 4, ok ? 8u : 0u);
-        }
-      }
-    }
-    const uint32_t nb = tc::kWgRows * chB;
-    for (uint32_t i = tid; i < nb; i += kThreads) {
-      const uint32_t r = i / chB, j = i - r * chB;
-      int32_t o = -1;
-      if (e + r < end) o = p.pin != nullptr ? __ldg(p.pout + e + r) : (int32_t)(e + r);
-      const bool ok = o >= 0 && (uint32_t)o < p.n_out;
-      cp_async16(base + a_bytes + cm_off(r, j, chB),
-                 G + (size_t)(ok ? o : 0) * p.c_out + col0 + 8 * j, ok ? 16u : 0u);
     }
     pos += tc::kWgRows;
     if (pos >= end) { ++wc; open(); }
+    return w;
+  };
+  // chunk j = j0 + 4m of row ar lies at cm_off(ar, j0, chunks) + 512 m
+  const uint32_t j0 = tid & 3u;
+  auto copy = [&](uint32_t s, Words w) {
+    const uint32_t base = s0 + (s % kStages) * stage_bytes;
+    if (p.stem_K == 0) {
+      const bool ok = w.src >= 0 && (uint32_t)w.src < p.n_in;
+      const T *rp = In + (size_t)(ok ? w.src : 0) * p.c_in + ci0 + 8 * j0;
+      const uint32_t dst = base + cm_off(ar, j0, kChA);
+#pragma unroll
+      for (uint32_t m = 0; m < 4; ++m) {
+        const bool okj = ok && ci0 + 8 * (j0 + 4 * m) < p.c_in;
+        cp_async16(dst + 512 * m, okj ? rp + 32 * m : In, okj ? 16u : 0u);
+      }
+    } else {
+      // chunk j = virtual channels ci0 + 8j..: offsets kk = (ci0 + 8j) / 4 + {0, 1}, 8 bytes each.
+      // The table is walked by pointer steps (one offset, then seven), which keeps the compiler
+      // from holding the eight 64-bit offsets kk * n_out in registers across the loop.
+      const uint32_t kk0 = ci0 / 4 + 2 * j0;
+      const int32_t *tp = p.nbr + (size_t)kk0 * p.n_out + (w.o >= 0 ? w.o : 0);
+      const uint32_t dst = base + cm_off(ar, j0, kChA);
+#pragma unroll
+      for (uint32_t m = 0; m < 4; ++m) {
+#pragma unroll
+        for (uint32_t h = 0; h < 2; ++h) {
+          const int32_t src = (w.o >= 0 && kk0 + 8 * m + h < p.stem_K) ? __ldg(tp) : -1;
+          const bool ok = src >= 0 && (uint32_t)src < p.n_in;
+          cp_async8(dst + 512 * m + 8 * h, In + (size_t)(ok ? src : 0) * 4, ok ? 8u : 0u);
+          tp += (size_t)(h == 0 ? 1 : 7) * p.n_out;
+        }
+      }
+    }
+    const bool ok = w.o >= 0 && (uint32_t)w.o < p.n_out;
+    const T *gp = G + (size_t)(ok ? w.o : 0) * p.c_out + col0 + 8 * j0;
+    const uint32_t dst = base + a_bytes + cm_off(ar, j0, chB);
+#pragma unroll
+    for (uint32_t m = 0; m < (chB + 3) / 4; ++m)
+      if (j0 + 4 * m < chB) cp_async16(dst + 512 * m, gp + 32 * m, ok ? 16u : 0u);
   };
 
   float acc[NT][NI / 2];
@@ -321,17 +339,27 @@ __device__ __forceinline__ void wgrad_unit(const WgParams &p, uint32_t k, uint32
 #pragma unroll
     for (int q = 0; q < NI / 2; ++q) acc[i][q] = 0.f;
 
+  Words first[kStages - 2];
+#pragma unroll
+  for (uint32_t s = 0; s < kStages - 2; ++s)
+    if (s < n_st) first[s] = fetch();
+#pragma unroll
   for (uint32_t s = 0; s < kStages - 2; ++s) {
-    if (s < n_st) load(s);
+    if (s < n_st) copy(s, first[s]);
     cp_async_commit();
   }
+  Words next{-1, -1};                   // stage s + 2's words at the top of iteration s
+  if (kStages - 2 < n_st) next = fetch();
   // (a warpgroup whose 64 channels lie past c_in multiplies the zero-filled half of the tile:
   // branching around wgmma would serialise the instructions of the whole kernel)
   for (uint32_t s = 0; s < n_st; ++s) {
     cp_async_wait<kStages - 3>();
     fence_proxy_async();
     __syncthreads();
-    if (s + kStages - 2 < n_st) load(s + kStages - 2);
+    if (s + kStages - 2 < n_st) {       // into the slot of stage s - 2
+      copy(s + kStages - 2, next);
+      if (s + kStages - 1 < n_st) next = fetch();
+    }
     cp_async_commit();
     // MN-major: the next 8 channels are 128 B on (sbo), the next 8 rows one row of chunks (lbo)
     const uint32_t a0 = s0 + (s % kStages) * stage_bytes + wg * 8 * 128;
@@ -421,7 +449,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_tf32(const WgParams p) {
   constexpr uint32_t R = tc::kWgRowsTf32, SA = tc::kWgChannels + tc::kWgPadTf32;
   const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint32_t k = blockIdx.z, ci0 = blockIdx.y * tc::kWgChannels;
-  const uint32_t SB = p.c_out + tc::kWgPadTf32, chB = p.c_out / 4;
+  const uint32_t SB = p.c_out + tc::kWgPadTf32;
+  constexpr uint32_t chB = 4 * NB;      // 16-byte chunks of a dOut row (c_out = 16 NB)
   const uint32_t stage_floats = R * (SA + SB);
   const uint32_t n_chunks = p.pin != nullptr ? p.n_chunks : 1u;
   const float *In = reinterpret_cast<const float *>(p.in);
@@ -433,6 +462,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_tf32(const WgParams p) {
     wg_range(p, k, c, lo, hi);
     n_st += (hi - lo + R - 1) / R;
   }
+  // as in wgrad_unit: thread tid copies row ar = tid / 8 of both operands, chunks (tid & 7) + 8m
+  // of 4 channels, from index words fetched a stage ahead
+  const uint32_t ar = tid >> 3;
   uint32_t wc = 0, pos = 0, end = 0;
   auto open = [&]() {
     for (; wc < n_chunks; ++wc) {
@@ -441,33 +473,40 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_tf32(const WgParams p) {
     }
   };
   open();
-
-  const uint32_t ar = tid >> 3;         // eight threads per In row, 4 chunks of 4 channels each
-  auto load = [&](uint32_t s) {
+  struct Words { int32_t src, o; };
+  auto fetch = [&]() {
+    Words w{-1, -1};
+    const uint32_t r = pos + ar;
+    if (r < end) {
+      if (p.pin != nullptr) {
+        w.src = __ldg(p.pin + r);
+        w.o = __ldg(p.pout + r);
+      } else {
+        w.src = __ldg(p.nbr + (size_t)k * p.n_out + r);
+        w.o = (int32_t)r;
+      }
+    }
+    pos += R;
+    if (pos >= end) { ++wc; open(); }
+    return w;
+  };
+  auto copy = [&](uint32_t s, Words w) {
     const uint32_t base = smem_u32(sm + (s % kStages) * stage_floats);
-    const uint32_t e = pos;
-    int32_t src = -1;
-    if (e + ar < end)
-      src = p.pin != nullptr ? __ldg(p.pin + e + ar) : __ldg(p.nbr + (size_t)k * p.n_out + e + ar);
-    const bool ok = src >= 0 && (uint32_t)src < p.n_in;
-    const float *rp = In + (size_t)(ok ? src : 0) * p.c_in + ci0;
+    const bool ok = w.src >= 0 && (uint32_t)w.src < p.n_in;
+    const float *rp = In + (size_t)(ok ? w.src : 0) * p.c_in + ci0;
 #pragma unroll
     for (uint32_t m = 0; m < 4; ++m) {
       const uint32_t j = (tid & 7u) + 8 * m;
       const bool okj = ok && ci0 + 4 * j < p.c_in;
       cp_async16(base + (ar * SA + 4 * j) * 4, okj ? rp + 4 * j : In, okj ? 16u : 0u);
     }
-    const uint32_t nb = R * chB;
-    for (uint32_t i = tid; i < nb; i += kThreads) {
-      const uint32_t r = i / chB, j = i - r * chB;
-      int32_t o = -1;
-      if (e + r < end) o = p.pin != nullptr ? __ldg(p.pout + e + r) : (int32_t)(e + r);
-      const bool okr = o >= 0 && (uint32_t)o < p.n_out;
-      cp_async16(base + (R * SA + r * SB + 4 * j) * 4, G + (size_t)(okr ? o : 0) * p.c_out + 4 * j,
-                 okr ? 16u : 0u);
+    const bool okr = w.o >= 0 && (uint32_t)w.o < p.n_out;
+    const float *gp = G + (size_t)(okr ? w.o : 0) * p.c_out;
+#pragma unroll
+    for (uint32_t m = 0; m < (chB + 7) / 8; ++m) {
+      const uint32_t j = (tid & 7u) + 8 * m;
+      if (j < chB) cp_async16(base + (R * SA + ar * SB + 4 * j) * 4, gp + 4 * j, okr ? 16u : 0u);
     }
-    pos += R;
-    if (pos >= end) { ++wc; open(); }
   };
 
   float acc[2][NB][4];
@@ -478,16 +517,26 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_tf32(const WgParams p) {
 #pragma unroll
       for (int q = 0; q < 4; ++q) acc[mi][ni][q] = 0.f;
 
+  Words first[kStages - 2];
+#pragma unroll
+  for (uint32_t s = 0; s < kStages - 2; ++s)
+    if (s < n_st) first[s] = fetch();
+#pragma unroll
   for (uint32_t s = 0; s < kStages - 2; ++s) {
-    if (s < n_st) load(s);
+    if (s < n_st) copy(s, first[s]);
     cp_async_commit();
   }
+  Words next{-1, -1};                   // stage s + 2's words at the top of iteration s
+  if (kStages - 2 < n_st) next = fetch();
   const uint32_t g = lane >> 2, t = lane & 3;
   const uint32_t m0 = (warp & 3) * 32, n0 = (warp >> 2) * NB * 8;
   for (uint32_t s = 0; s < n_st; ++s) {
     cp_async_wait<kStages - 3>();
     __syncthreads();                    // stage s landed everywhere; stage s - 2 is no longer read
-    if (s + kStages - 2 < n_st) load(s + kStages - 2);
+    if (s + kStages - 2 < n_st) {
+      copy(s + kStages - 2, next);
+      if (s + kStages - 1 < n_st) next = fetch();
+    }
     cp_async_commit();
     const uint32_t *sA = reinterpret_cast<const uint32_t *>(sm + (s % kStages) * stage_floats);
     const uint32_t *sB = sA + R * SA;
