@@ -341,6 +341,24 @@ int meb200_origin_group(const int32_t *coords, uint32_t n, uint32_t ncols,
                         const int32_t *origin_coords, const uint32_t *origin_table,
                         uint32_t origin_capacity, uint32_t B, int32_t *row_seg, int32_t *order,
                         int32_t *seg_start, int32_t *tile_start, void *scratch, void *stream);
+/* The same grouping for the n points of a tensor field: field float32 [n, ncols], a point's cloud
+ * is the origin row of (lroundf(field[i, 0]), 0, ..., 0); outputs and scratch as
+ * meb200_origin_group.  d_bad (DEVICE uint32 status word, cleared by the call; NULL when the
+ * batch column is known valid) is set to 1 when a batch value is not finite or its rounding lies
+ * outside int32; such a point gets row_seg -1 and is in no segment. */
+int meb200_field_origin_group(const float *field, uint32_t n, uint32_t ncols,
+                              const int32_t *origin_coords, const uint32_t *origin_table,
+                              uint32_t origin_capacity, uint32_t B, int32_t *row_seg,
+                              int32_t *order, int32_t *seg_start, int32_t *tile_start,
+                              uint32_t *d_bad, void *scratch, void *stream);
+/* The origin map of a tensor field: the candidate rows (lroundf(field[i, 0]), 0, ..., 0) written to
+ * ocoords (int32 [n, ncols]) and inserted by meb200_insert_and_map (the other arguments as there).
+ * The validity of the batch column reaches the host with the unique count, in the same read; a
+ * batch value that is not finite or outside int32 returns MEB200_ERR_DOMAIN. */
+int meb200_field_origin_insert(const float *field, uint32_t n, uint32_t ncols, int32_t *ocoords,
+                               uint32_t *table, uint32_t capacity, int32_t *unique_coords,
+                               int64_t *unique_index, int64_t *inverse_map, void *scratch,
+                               uint32_t *h_num_unique, void *stream);
 
 /* out[s, c] (fp32 [B, C]) = SUM / AVG / MAX over the rows i of segment s of a[i, c], or of
  * a[i, c] * b[i, c] when b != NULL (SUM / AVG only).  Each tile of a segment stores fp32 partials

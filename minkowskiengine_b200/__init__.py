@@ -10,7 +10,7 @@ MinkowskiConvolutionTranspose, MinkowskiChannelwiseConvolution (depthwise), loca
 unpooling (MinkowskiPoolingTranspose), global pooling, broadcast, batch and instance
 normalisation, pruning, union and arithmetic between sparse tensors on different coordinate maps,
 TensorField (point features quantised to voxels or splatted onto their corners, sliced back and
-interpolated), dense-tensor interop (SparseTensor.dense, MinkowskiToDenseTensor, to_sparse,
+interpolated, and pooled per cloud or broadcast onto directly), dense-tensor interop (SparseTensor.dense, MinkowskiToDenseTensor, to_sparse,
 to_sparse_all, dense_coordinates), COO sparse-times-dense products (spmm, spmm_average) and max
 pooling over an explicit pair list, and the thin torch wrappers (cat / sum / mean / var, the stack containers,
 MinkowskiToFeature) that MinkUNet, the ResNet classifiers and generative networks need.

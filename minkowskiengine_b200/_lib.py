@@ -70,6 +70,10 @@ PROTOTYPES = {
     "meb200_origin_group_scratch_bytes": (_u64, [_u32, _u32]),
     "meb200_origin_group": (_i32, [_vp, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp,
                                    _vp]),
+    "meb200_field_origin_group": (_i32, [_vp, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _vp, _vp,
+                                         _vp, _vp, _vp, _vp]),
+    "meb200_field_origin_insert": (_i32, [_vp, _u32, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp,
+                                          C.POINTER(_u32), _vp]),
     "meb200_segment_max_tiles": (_u32, [_u32, _u32]),
     "meb200_segment_workspace_bytes": (_u64, [_u32, _u32, _u32]),
     "meb200_segment_reduce": (_i32, [_vp, _vp, _i32, _u32, _u32, _vp, _vp, _vp, _u32, _i32, _vp, _vp,

@@ -520,6 +520,10 @@ class CoordinateMapManagerGPU_c10:
         self._inserted = []     # keys of the maps made by insert_and_map, in order
         self._origin_covers = 0  # ... how many of them the origin map was built from
         self._groupings = {}    # map key -> _OriginGrouping
+        # field key -> _OriginGrouping of its points: apart from _groupings, because a field key and
+        # a map key may be the same tuple
+        self._field_groupings = {}
+        self._origin_fields = set()  # field keys the origin map was built from
         self._prunes = {}       # (in key, out key) -> (unique_index, inverse_map) of a pruned map
         self._unions = {}       # tuple of input keys -> _UnionMap
         self._fields = {}       # field key -> float32 [N, D+1] point coordinates
@@ -586,7 +590,7 @@ class CoordinateMapManagerGPU_c10:
         """Registers a map made from input coordinates (insert_and_map, or the quantisation of a
         tensor field): the first one starts the predicted pyramid and kernel maps, and every one
         counts towards the origin map."""
-        first = not self._maps
+        first = not self._inserted   # (an origin map built from fields may exist already)
         self._maps[key] = cmap
         self._inserted.append(key)
         if first:
@@ -779,21 +783,54 @@ class CoordinateMapManagerGPU_c10:
     def _origin(self):
         """reference: coordinate_map_manager.cpp:474-508.  The origin map holds one row
         (b, 0, ..., 0) per batch index of the inserted maps, in ASCENDING batch order; built once
-        (the one host read is its row count B) and cached under the key ([0]*D, "")."""
-        _assert(len(self._inserted) > 0, "No coordinate map found")
-        ncols = self._maps[self._inserted[0]].ncols
+        (the one host read is its row count B) and cached under the key ([0]*D, "").  A manager
+        that holds only tensor fields builds it from the batch columns of its fields (reference:
+        origin_field, coordinate_map_manager.cpp), rounded with lroundf as the quantisation
+        rounds them; a batch value that is not finite or outside int32 raises ValueError."""
+        if self._inserted:
+            ncols = self._maps[self._inserted[0]].ncols
+        else:
+            _assert(len(self._fields) > 0, "No coordinate map found")
+            ncols = next(iter(self._fields.values())).size(1)
         key = self._origin_key(ncols)
         if key in self._maps:
             return key
-        batch = torch.cat([self._maps[k].coords[:, 0] for k in self._inserted])
-        cand = torch.zeros((batch.numel(), ncols), dtype=torch.int32, device=batch.device)
-        cand[:, 0] = batch
-        cmap, _, _ = _CoordinateMap.build(cand, key[0])
+        if self._inserted:
+            batch = torch.cat([self._maps[k].coords[:, 0] for k in self._inserted])
+            cand = torch.zeros((batch.numel(), ncols), dtype=torch.int32, device=batch.device)
+            cand[:, 0] = batch
+            cmap, _, _ = _CoordinateMap.build(cand, key[0])
+        else:
+            cmap = self._field_origin(key[0])
         # ascending batch index: rebuild the table over the sorted rows
         coords = cmap.coords[torch.argsort(cmap.coords[:, 0])].contiguous()
         self._maps[key] = _distinct_map(coords, key[0], cmap.table)
         self._origin_covers = len(self._inserted)
         return key
+
+    def _field_origin(self, tensor_stride):
+        """The rows (lroundf(b), 0, ..., 0) of every field's points, deduplicated
+        (meb200_field_origin_insert: the validity of the batch column comes with the row count)."""
+        fks = list(self._fields)
+        field = torch.cat([self._fields[k] for k in fks]) if len(fks) > 1 else self._fields[fks[0]]
+        n, ncols = field.shape
+        ocoords = torch.empty((n, ncols), dtype=torch.int32, device=field.device)
+        table, uniq, uidx, inv, scratch = _insert_buffers(n, ncols, field.device)
+        m = ctypes.c_uint32(0)
+        rc = _lib.load().meb200_field_origin_insert(
+            _lib.ptr(field), n, ncols, _lib.ptr(ocoords), _lib.ptr(table), table.numel(),
+            _lib.ptr(uniq), _lib.ptr(uidx), _lib.ptr(inv), _lib.ptr(scratch), ctypes.byref(m),
+            _lib.current_stream())
+        if rc == _lib.ERR_DOMAIN:
+            raise ValueError(ERROR_FIELD_DOMAIN)
+        _lib.check(rc)
+        self._origin_fields.update(fks)
+        return _CoordinateMap(uniq[:int(m.value)], table, table.numel(), tensor_stride)
+
+    def origin_field(self):
+        """reference: MinkowskiCoordinateManager.py:273.  The one origin map of the manager, which
+        pooling a field and pooling a map share."""
+        return self.origin()
 
     def origin(self):
         k = self._origin()
@@ -834,10 +871,51 @@ class CoordinateMapManagerGPU_c10:
         self._groupings[ik] = grp
         return grp
 
-    def origin_map(self, key):
-        """reference: origin_map_th, coordinate_map_manager.cpp:828-885 -> (batch_indices int64
-        [B], [row indices (int64) of batch index b for b in 0..max batch index])."""
-        grp = self._origin_grouping(key)
+    def _field_grouping(self, field_key):
+        """Points of field `field_key` grouped by cloud (meb200_field_origin_group), cached per field.
+        The first grouping reads back, in one read, whether the batch column is valid and whether
+        every point found its cloud; a field the origin map was built from needs neither."""
+        fk, field = self._field(field_key)
+        grp = self._field_groupings.get(fk)
+        if grp is not None:
+            return grp
+        okey = self._origin()
+        omap = self._maps[okey]
+        _assert(field.size(1) == omap.ncols, "coordinate size mismatch")
+        lib = _lib.load()
+        n, B, dev = field.size(0), omap.size, field.device
+        grp = _OriginGrouping()
+        grp.n, grp.B = n, B
+        grp.row_seg = torch.empty(n, dtype=torch.int32, device=dev)
+        grp.order = torch.empty(n, dtype=torch.int32, device=dev)
+        starts = torch.empty((2, B + 1), dtype=torch.int32, device=dev)
+        grp.seg_start, grp.tile_start = starts[0], starts[1]
+        scratch = torch.empty(int(lib.meb200_origin_group_scratch_bytes(n, B)), dtype=torch.uint8,
+                              device=dev)
+        check = fk not in self._origin_fields
+        bad = torch.empty(1, dtype=torch.int32, device=dev) \
+            if check and fk not in self._field_valid else None
+        _lib.check(lib.meb200_field_origin_group(
+            _lib.ptr(field), n, field.size(1), _lib.ptr(omap.coords), _lib.ptr(omap.table),
+            omap.capacity, B, _lib.ptr(grp.row_seg), _lib.ptr(grp.order), _lib.ptr(grp.seg_start),
+            _lib.ptr(grp.tile_start), _lib.ptr(bad), _lib.ptr(scratch), _lib.current_stream()))
+        if check:
+            words = (grp.seg_start[B:] if bad is None else torch.cat([bad, grp.seg_start[B:]]))
+            words = words.tolist()
+            if bad is not None and words[0] != 0:
+                raise ValueError(ERROR_FIELD_DOMAIN)
+            _assert(words[-1] == n, "the tensor field holds batch indices that are not in the "
+                    "origin map")
+        self._field_groupings[fk] = grp
+        return grp
+
+    def _grouping(self, key, is_field=False):
+        """Per-cloud grouping of the rows of map `key`, or of the points of field `key`."""
+        return self._field_grouping(key) if is_field else self._origin_grouping(key)
+
+    def _origin_rows(self, grp):
+        """(batch_indices int64 [B], [row indices (int64) of batch index b for b in 0..max batch
+        index]) of a grouping."""
         okey = self._origin()
         batch = self._maps[okey].coords[:, 0].long()
         starts = grp.seg_start.tolist()
@@ -847,6 +925,15 @@ class CoordinateMapManagerGPU_c10:
         for s, b in enumerate(batch.tolist()):
             rows[b] = order[starts[s]:starts[s + 1]]
         return batch, rows
+
+    def origin_map(self, key):
+        """reference: origin_map_th, coordinate_map_manager.cpp:828-885 -> (batch_indices int64
+        [B], [row indices (int64) of batch index b for b in 0..max batch index])."""
+        return self._origin_rows(self._origin_grouping(key))
+
+    def origin_field_map(self, field_key):
+        """reference: origin_field_map_th -> origin_map's form for the points of a field."""
+        return self._origin_rows(self._field_grouping(field_key))
 
     # -- pruning and union -------------------------------------------------------------
     def _prune(self, in_key, keep):
@@ -1112,13 +1199,17 @@ class _UnionMap:
 
 
 # ----------------------------------------------------------------------------------------
-def _check_feats(in_feat, manager, in_key, name="in_feat"):
+def _check_feats(in_feat, manager, in_key, name="in_feat", is_field=False):
+    """`is_field`: `in_key` names a tensor field (its rows are the field's points), not a map."""
     _assert(in_feat.is_cuda, f"{name} must be CUDA (this backend has no CPU path)")
     _assert(in_feat.is_contiguous(), f"{name} must be contiguous")
     _assert(in_feat.dim() == 2, f"{name}.dim():", in_feat.dim())
-    _assert(manager.exists(in_key), ERROR_MAP_NOT_FOUND)
-    _assert(in_feat.size(0) == manager.size(in_key), "Invalid in_feat size", in_feat.size(0),
-            "!=", manager.size(in_key))
+    if is_field:
+        n = manager.get_coordinate_field(in_key).size(0)
+    else:
+        _assert(manager.exists(in_key), ERROR_MAP_NOT_FOUND)
+        n = manager.size(in_key)
+    _assert(in_feat.size(0) == n, "Invalid in_feat size", in_feat.size(0), "!=", n)
 
 
 def _workspace(n_out, c_in, c_out, K, code, device):
@@ -1768,18 +1859,19 @@ def _check_glob(manager, in_feat, glob_feat, glob_key):
             "for both in_feat and in_feat_glob.")
 
 
-def GlobalPoolingForwardGPU(in_feat, pooling_mode, in_key, out_key, manager):
+def GlobalPoolingForwardGPU(in_feat, pooling_mode, in_key, out_key, manager, is_field=False):
     """reference: GlobalPoolingForwardCPU src/global_pooling_cpu.cpp:43-200 -> (out_feat [B, C],
     num_nonzero [B] (sum / avg, feature dtype) | max_index int32 [B, C] (flat row*C + c)).
     Mutates `out_key` (-> the origin key) when it is unset.  All nine GLOBAL_* modes are accepted;
     the _DEFAULT / _KERNEL / _PYTORCH_INDEX variants select a strategy in the reference, not a
-    result, and run the same kernels here."""
-    _check_feats(in_feat, manager, in_key)
+    result, and run the same kernels here.  `is_field`: `in_key` is a tensor field key and the
+    rows are its points (a field key may equal a map key, so the caller says which it holds)."""
+    _check_feats(in_feat, manager, in_key, is_field=is_field)
     _assert(pooling_mode in _GLOBAL_CODE, "Invalid pooling mode", pooling_mode)
     okey = manager._origin()
     if not out_key.is_key_set():
         out_key.set_key(list(okey[0]), okey[1])
-    grp = manager._origin_grouping(in_key)
+    grp = manager._grouping(in_key, is_field)
     mode = _GLOBAL_CODE[pooling_mode]
     if mode == _lib.SEG_MAX:
         aux = torch.empty((grp.B, in_feat.size(1)), dtype=torch.int32, device=in_feat.device)
@@ -1792,14 +1884,14 @@ def GlobalPoolingForwardGPU(in_feat, pooling_mode, in_key, out_key, manager):
 
 
 def GlobalPoolingBackwardGPU(in_feat, grad_out_feat, num_nonzero, pooling_mode, in_key, out_key,
-                             manager):
+                             manager, is_field=False):
     """reference: GlobalPoolingBackwardCPU src/global_pooling_cpu.cpp:221-330.  The average's
     divisor is the exact per-cloud row count of the grouping (num_nonzero may be rounded in
     bf16 / fp16); the max gradient goes to the row max_index names, whatever the cloud count."""
-    _check_feats(in_feat, manager, in_key)
+    _check_feats(in_feat, manager, in_key, is_field=is_field)
     _assert(pooling_mode in _GLOBAL_CODE, "Invalid pooling mode", pooling_mode)
     _assert(manager.exists(out_key), ERROR_MAP_NOT_FOUND)
-    grp = manager._origin_grouping(in_key)
+    grp = manager._grouping(in_key, is_field)
     _assert(grad_out_feat.dim() == 2 and grad_out_feat.size(0) == grp.B,
             "Invalid grad_out size", tuple(grad_out_feat.shape))
     _assert(in_feat.size(1) == grad_out_feat.size(1), "Input feature size and kernel size mismatch")
@@ -1816,27 +1908,28 @@ def GlobalPoolingBackwardGPU(in_feat, grad_out_feat, num_nonzero, pooling_mode, 
     return _broadcast(None, g, grp, _lib.BCAST_COPY, in_feat.dtype, n=grp.n, C=in_feat.size(1))
 
 
-def BroadcastForwardGPU(in_feat, in_feat_glob, broadcast_mode, in_key, glob_key, manager):
+def BroadcastForwardGPU(in_feat, in_feat_glob, broadcast_mode, in_key, glob_key, manager,
+                        is_field=False):
     """reference: BroadcastForwardCPU src/broadcast_cpu.cpp:44-90:
-    out[i] = in_feat[i] + / * in_feat_glob[cloud of i]."""
-    _check_feats(in_feat, manager, in_key)
+    out[i] = in_feat[i] + / * in_feat_glob[cloud of i].  `is_field`: `in_key` is a tensor field."""
+    _check_feats(in_feat, manager, in_key, is_field=is_field)
     _assert(broadcast_mode in _BCAST_CODE, "Invalid broadcast mode", broadcast_mode)
     _check_glob(manager, in_feat, in_feat_glob, glob_key)
-    grp = manager._origin_grouping(in_key)
+    grp = manager._grouping(in_key, is_field)
     return _broadcast(in_feat, _f32c(in_feat_glob), grp, _BCAST_CODE[broadcast_mode])
 
 
 def BroadcastBackwardGPU(in_feat, in_feat_glob, grad_out_feat, broadcast_mode, in_key, glob_key,
-                         manager):
+                         manager, is_field=False):
     """reference: BroadcastBackwardCPU src/broadcast_cpu.cpp:92-150 (broadcast_kernel.hpp):
     add: dx = dy, dg[b] = sum_{i in b} dy;  mul: dx = dy * g[b(i)], dg[b] = sum_{i in b} dy * x."""
-    _check_feats(in_feat, manager, in_key)
+    _check_feats(in_feat, manager, in_key, is_field=is_field)
     _assert(broadcast_mode in _BCAST_CODE, "Invalid broadcast mode", broadcast_mode)
     _check_glob(manager, in_feat, in_feat_glob, glob_key)
     grad_out_feat = grad_out_feat.contiguous()
     _assert(grad_out_feat.shape == in_feat.shape and grad_out_feat.dtype == in_feat.dtype,
             "Incompatible grad_out_feat")
-    grp = manager._origin_grouping(in_key)
+    grp = manager._grouping(in_key, is_field)
     if broadcast_mode == BroadcastMode.ELEMENTWISE_ADDITON:
         grad_in = grad_out_feat
         grad_glob = _segment_reduce(grad_out_feat, grp, _lib.SEG_SUM)

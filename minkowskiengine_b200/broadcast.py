@@ -1,6 +1,7 @@
 """Broadcast of per-cloud rows back to the rows of each cloud (reference: MinkowskiBroadcast.py).
 Row s of the global tensor belongs to the cloud with the s-th smallest batch index (the origin
-map's order)."""
+map's order).  The input may be a SparseTensor or a TensorField; a field's output is a TensorField
+on the same field key (the per-cloud feature of a point network, brought back to its points)."""
 import torch
 from torch.autograd import Function
 from torch.nn import Module
@@ -11,27 +12,30 @@ from .common import MinkowskiModuleBase
 from .coordinate_manager import CoordinateManager
 from .enums import BroadcastMode
 from .sparse_tensor import SparseTensor
+from .tensor_field import TensorField, same_kind
 
 
 class MinkowskiBroadcastFunction(Function):
     @staticmethod
     def forward(ctx, input_features: torch.Tensor, input_features_global: torch.Tensor,
                 operation_type: BroadcastMode, in_coords_key: CoordinateMapKey,
-                glob_coords_key: CoordinateMapKey, coords_manager: CoordinateManager):
+                glob_coords_key: CoordinateMapKey, coords_manager: CoordinateManager,
+                is_field: bool = False):
         assert isinstance(operation_type, BroadcastMode)
         input_features = input_features.contiguous()
         input_features_global = input_features_global.contiguous()
         ctx.saved_vars = (input_features, input_features_global, operation_type, in_coords_key,
-                          glob_coords_key, coords_manager)
+                          glob_coords_key, coords_manager, is_field)
         return _C.BroadcastForwardGPU(input_features, input_features_global, operation_type,
-                                      in_coords_key, glob_coords_key, coords_manager._manager)
+                                      in_coords_key, glob_coords_key, coords_manager._manager,
+                                      is_field=is_field)
 
     @staticmethod
     def backward(ctx, grad_out_feat):
-        x, g, op, in_key, glob_key, manager = ctx.saved_vars
+        x, g, op, in_key, glob_key, manager, is_field = ctx.saved_vars
         grad_in, grad_glob = _C.BroadcastBackwardGPU(x, g, grad_out_feat.contiguous(), op, in_key,
-                                                     glob_key, manager._manager)
-        return grad_in, grad_glob, None, None, None, None
+                                                     glob_key, manager._manager, is_field=is_field)
+        return grad_in, grad_glob, None, None, None, None, None
 
 
 class MinkowskiBroadcastBase(MinkowskiModuleBase):
@@ -41,13 +45,12 @@ class MinkowskiBroadcastBase(MinkowskiModuleBase):
         self.operation_type = operation_type
         self.broadcast = MinkowskiBroadcastFunction
 
-    def forward(self, input: SparseTensor, input_glob: SparseTensor):
-        assert isinstance(input, SparseTensor)
+    def forward(self, input, input_glob: SparseTensor):
+        assert isinstance(input, (SparseTensor, TensorField))
         output = self.broadcast.apply(input.F, input_glob.F, self.operation_type,
                                       input.coordinate_map_key, input_glob.coordinate_map_key,
-                                      input.coordinate_manager)
-        return SparseTensor(output, coordinate_map_key=input.coordinate_map_key,
-                            coordinate_manager=input.coordinate_manager)
+                                      input.coordinate_manager, isinstance(input, TensorField))
+        return same_kind(input, output)
 
     def __repr__(self):
         return self.__class__.__name__
@@ -71,8 +74,8 @@ class _BroadcastCopy(Function):
     """y[i] = g[cloud of i]; dg[s] = sum of dy over cloud s (the native broadcast / reduction)."""
 
     @staticmethod
-    def forward(ctx, glob_features, in_key, manager, n):
-        grp = manager._origin_grouping(in_key)
+    def forward(ctx, glob_features, in_key, manager, n, is_field=False):
+        grp = manager._grouping(in_key, is_field)
         ctx.grp = grp
         ctx.dtype = glob_features.dtype
         return _C._broadcast(None, _C._f32c(glob_features), grp, _C._lib.BCAST_COPY,
@@ -81,15 +84,16 @@ class _BroadcastCopy(Function):
     @staticmethod
     def backward(ctx, grad_out):
         g = _C._segment_reduce(grad_out.contiguous(), ctx.grp, _C._lib.SEG_SUM)
-        return g.to(ctx.dtype), None, None, None
+        return g.to(ctx.dtype), None, None, None, None
 
 
 def _broadcast_copy(input, input_glob):
     mgr = input.coordinate_manager._manager
-    _C._check_feats(input.F, mgr, input.coordinate_map_key)
+    is_field = isinstance(input, TensorField)
+    _C._check_feats(input.F, mgr, input.coordinate_map_key, is_field=is_field)
     _C._check_glob(mgr, input.F, input_glob.F, input_glob.coordinate_map_key)
     return _BroadcastCopy.apply(input_glob.F.contiguous(), input.coordinate_map_key, mgr,
-                                len(input))
+                                input.F.size(0), is_field)
 
 
 class MinkowskiBroadcast(Module):
@@ -98,20 +102,16 @@ class MinkowskiBroadcast(Module):
     def __repr__(self):
         return self.__class__.__name__
 
-    def forward(self, input: SparseTensor, input_glob: SparseTensor):
-        assert isinstance(input, SparseTensor)
+    def forward(self, input, input_glob: SparseTensor):
+        assert isinstance(input, (SparseTensor, TensorField))
         assert isinstance(input_glob, SparseTensor)
-        return SparseTensor(_broadcast_copy(input, input_glob),
-                            coordinate_map_key=input.coordinate_map_key,
-                            coordinate_manager=input.coordinate_manager)
+        return same_kind(input, _broadcast_copy(input, input_glob))
 
 
 class MinkowskiBroadcastConcatenation(MinkowskiBroadcast):
     """y_u = [x1_u, x2[cloud of u]]."""
 
-    def forward(self, input: SparseTensor, input_glob: SparseTensor):
-        assert isinstance(input, SparseTensor)
+    def forward(self, input, input_glob: SparseTensor):
+        assert isinstance(input, (SparseTensor, TensorField))
         assert isinstance(input_glob, SparseTensor)
-        cat = torch.cat((input.F, _broadcast_copy(input, input_glob)), dim=1)
-        return SparseTensor(cat, coordinate_map_key=input.coordinate_map_key,
-                            coordinate_manager=input.coordinate_manager)
+        return same_kind(input, torch.cat((input.F, _broadcast_copy(input, input_glob)), dim=1))

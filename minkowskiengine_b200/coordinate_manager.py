@@ -141,6 +141,17 @@ class CoordinateManager:
         (reference: MinkowskiCoordinateManager.py:423)."""
         return self._manager.origin_map(key)
 
+    def origin_field(self) -> CoordinateMapKey:
+        """Key of the origin map for pooling tensor fields: the same map as `origin()`, built
+        from the fields' batch columns (lroundf) when the manager holds no coordinate map
+        (reference: MinkowskiCoordinateManager.py:273)."""
+        return self._manager.origin_field()
+
+    def origin_field_map(self, key: CoordinateMapKey):
+        """`origin_map`'s form for the points of the field `key`
+        (reference: MinkowskiCoordinateManager.py:426)."""
+        return self._manager.origin_field_map(key)
+
     def origin_map_size(self) -> int:
         """Number of clouds B (rows of the origin map)."""
         return self._manager.origin_map_size()

@@ -163,6 +163,15 @@ __device__ __forceinline__ uint32_t hash_coord(const int32_t (&c)[NC]) {
   return h;
 }
 
+// Batch index of a float field coordinate: lroundf (half away from zero).  *ok is cleared when the
+// value is not finite or its rounding lies outside int32 (the quantisation and the origin map of
+// a field share this rule).
+__device__ __forceinline__ int32_t quantize_batch(float b, bool *ok) {
+  bool in = b > -2147483648.5f && b < 2147483647.5f;
+  *ok &= in;
+  return in ? (int32_t)lroundf(b) : 0;
+}
+
 // Lookup in an open-addressing table of row indices; keys live in `coords`.
 template <int NC>
 __device__ __forceinline__ int32_t table_find(const int32_t *__restrict__ coords,

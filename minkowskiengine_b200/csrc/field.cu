@@ -25,12 +25,6 @@ __device__ __forceinline__ int32_t quantize_axis(float x, int32_t s, bool *ok) {
   return in ? (int32_t)v : 0;
 }
 
-__device__ __forceinline__ int32_t quantize_batch(float b, bool *ok) {
-  bool in = b > -2147483648.5f && b < 2147483647.5f;
-  *ok &= in;
-  return in ? (int32_t)lroundf(b) : 0;
-}
-
 template <int NC>
 __global__ void __launch_bounds__(256)
 k_quantize_field(const float *__restrict__ field, uint32_t n, IntVec ts, int32_t *__restrict__ out,

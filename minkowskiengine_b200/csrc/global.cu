@@ -35,6 +35,40 @@ k_origin_lookup(const int32_t *__restrict__ coords, uint32_t n, const int32_t *_
   row_seg[i] = table_find<NC>(origin, table, mask, key);
 }
 
+// The same for the float points of a tensor field, batch index lroundf(field[i, 0]).  A batch
+// value that is not finite or outside int32 gets -1 and sets *bad (when bad != NULL).
+template <int NC>
+__global__ void __launch_bounds__(256)
+k_field_origin_lookup(const float *__restrict__ field, uint32_t n,
+                      const int32_t *__restrict__ origin, const uint32_t *__restrict__ table,
+                      uint32_t mask, int32_t *__restrict__ row_seg, uint32_t *__restrict__ bad) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  bool ok = true;
+  int32_t key[NC];
+#pragma unroll
+  for (int j = 0; j < NC; ++j) key[j] = 0;
+  key[0] = quantize_batch(__ldg(field + (size_t)i * NC), &ok);
+  row_seg[i] = ok ? table_find<NC>(origin, table, mask, key) : -1;
+  if (!ok && bad != nullptr) atomicOr(bad, 1u);   // a flag, not a sum: any order, same word
+}
+
+// Origin candidates of a field: row i = (lroundf(field[i, 0]), 0, ..., 0), *bad as above.
+template <int NC>
+__global__ void __launch_bounds__(256)
+k_field_origin_coords(const float *__restrict__ field, uint32_t n, int32_t *__restrict__ out,
+                      uint32_t *__restrict__ bad) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  bool ok = true;
+  int32_t c[NC];
+#pragma unroll
+  for (int j = 1; j < NC; ++j) c[j] = 0;
+  c[0] = quantize_batch(__ldg(field + (size_t)i * NC), &ok);
+  store_coord<NC>(out, i, c);
+  if (!ok) atomicOr(bad, 1u);
+}
+
 // counts[s * n_tiles + t] = rows of segment s in group tile t (shared-memory integer counters:
 // the totals do not depend on the order of the increments)
 __global__ void __launch_bounds__(32)
@@ -331,6 +365,37 @@ k_broadcast_fma(const T *__restrict__ x, const T *__restrict__ z, const float *_
 // ---- host dispatch ---------------------------------------------------------------------------
 static uint32_t group_tiles(uint32_t n) { return (n + kGroupTile - 1) / kGroupTile; }
 
+static int check_group_args(uint32_t n, const int32_t *origin_coords, const uint32_t *origin_table,
+                            uint32_t origin_capacity, uint32_t B, const int32_t *row_seg,
+                            const int32_t *order, const int32_t *seg_start,
+                            const int32_t *tile_start, const void *scratch) {
+  MEB_CHECK_ARG(B >= 1 && B <= kMaxSegments, "B = %u clouds (supported: 1..%u)", B, kMaxSegments);
+  MEB_CHECK_ARG(origin_coords && origin_table && seg_start && tile_start, "null buffer");
+  MEB_CHECK_ARG(n == 0 || (row_seg && order && scratch), "null buffer");
+  MEB_CHECK_ARG(origin_capacity && (origin_capacity & (origin_capacity - 1)) == 0,
+                "capacity %u is not a power of two", origin_capacity);
+  return MEB200_OK;
+}
+
+// The counting sort of the n rows by their row_seg (written by a lookup): counts per group tile,
+// the scan, the stable scatter.  Shared by the grouping of a coordinate map and of a field.
+static int group_rows(const int32_t *row_seg, uint32_t n, uint32_t B, int32_t *order,
+                      int32_t *seg_start, int32_t *tile_start, void *scratch, cudaStream_t s) {
+  uint32_t nt = group_tiles(n);
+  int32_t *counts = (int32_t *)scratch;
+  if (n > 0) {
+    k_group_count<<<nt, 32, B * sizeof(int32_t), s>>>(row_seg, n, B, nt, counts);
+    MEB_LAUNCH_OK();
+  }
+  k_group_scan<<<1, 1024, 0, s>>>(counts, nt * B, B, nt, seg_start, tile_start);
+  MEB_LAUNCH_OK();
+  if (n > 0) {
+    k_group_scatter<<<nt, 32, B * sizeof(int32_t), s>>>(row_seg, n, B, nt, counts, order);
+    MEB_LAUNCH_OK();
+  }
+  return MEB200_OK;
+}
+
 template <typename T, int V, int MODE>
 static void seg_reduce_launch(const void *a, const void *b, uint32_t C, const int32_t *order,
                               const int32_t *seg_start, const int32_t *tile_start, uint32_t B,
@@ -427,27 +492,62 @@ int meb200_origin_group(const int32_t *coords, uint32_t n, uint32_t ncols,
                         const int32_t *origin_coords, const uint32_t *origin_table,
                         uint32_t origin_capacity, uint32_t B, int32_t *row_seg, int32_t *order,
                         int32_t *seg_start, int32_t *tile_start, void *scratch, void *stream) {
-  MEB_CHECK_ARG(B >= 1 && B <= kMaxSegments, "B = %u clouds (supported: 1..%u)", B, kMaxSegments);
-  MEB_CHECK_ARG(origin_coords && origin_table && seg_start && tile_start, "null buffer");
-  MEB_CHECK_ARG(n == 0 || (coords && row_seg && order && scratch), "null buffer");
-  MEB_CHECK_ARG(origin_capacity && (origin_capacity & (origin_capacity - 1)) == 0,
-                "capacity %u is not a power of two", origin_capacity);
+  int rc = check_group_args(n, origin_coords, origin_table, origin_capacity, B, row_seg, order,
+                            seg_start, tile_start, scratch);
+  if (rc != MEB200_OK) return rc;
+  MEB_CHECK_ARG(n == 0 || coords, "null buffer");
   cudaStream_t s = (cudaStream_t)stream;
-  uint32_t nt = group_tiles(n);
-  int32_t *counts = (int32_t *)scratch;
   if (n > 0) {
     MEB_DISPATCH_NCOLS(ncols, (k_origin_lookup<NC><<<cdiv(n, 256), 256, 0, s>>>(
                                   coords, n, origin_coords, origin_table, origin_capacity - 1,
                                   row_seg)));
     MEB_LAUNCH_OK();
-    k_group_count<<<nt, 32, B * sizeof(int32_t), s>>>(row_seg, n, B, nt, counts);
+  }
+  return group_rows(row_seg, n, B, order, seg_start, tile_start, scratch, s);
+}
+
+int meb200_field_origin_group(const float *field, uint32_t n, uint32_t ncols,
+                              const int32_t *origin_coords, const uint32_t *origin_table,
+                              uint32_t origin_capacity, uint32_t B, int32_t *row_seg,
+                              int32_t *order, int32_t *seg_start, int32_t *tile_start,
+                              uint32_t *d_bad, void *scratch, void *stream) {
+  int rc = check_group_args(n, origin_coords, origin_table, origin_capacity, B, row_seg, order,
+                            seg_start, tile_start, scratch);
+  if (rc != MEB200_OK) return rc;
+  MEB_CHECK_ARG(n == 0 || field, "null buffer");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (d_bad != nullptr) MEB_CUDA(cudaMemsetAsync(d_bad, 0, 4, s));
+  if (n > 0) {
+    MEB_DISPATCH_NCOLS(ncols, (k_field_origin_lookup<NC><<<cdiv(n, 256), 256, 0, s>>>(
+                                  field, n, origin_coords, origin_table, origin_capacity - 1,
+                                  row_seg, d_bad)));
     MEB_LAUNCH_OK();
   }
-  k_group_scan<<<1, 1024, 0, s>>>(counts, nt * B, B, nt, seg_start, tile_start);
-  MEB_LAUNCH_OK();
+  return group_rows(row_seg, n, B, order, seg_start, tile_start, scratch, s);
+}
+
+int meb200_field_origin_insert(const float *field, uint32_t n, uint32_t ncols, int32_t *ocoords,
+                               uint32_t *table, uint32_t capacity, int32_t *unique_coords,
+                               int64_t *unique_index, int64_t *inverse_map, void *scratch,
+                               uint32_t *h_num_unique, void *stream) {
+  MEB_CHECK_ARG(h_num_unique != nullptr, "h_num_unique");
+  cudaStream_t s = (cudaStream_t)stream;
   if (n > 0) {
-    k_group_scatter<<<nt, 32, B * sizeof(int32_t), s>>>(row_seg, n, B, nt, counts, order);
+    MEB_CHECK_ARG(field && ocoords && scratch, "null buffer");
+    uint32_t *bad = insert_flag_word(scratch, n);
+    MEB_CUDA(cudaMemsetAsync(bad, 0, 4, s));
+    MEB_DISPATCH_NCOLS(ncols, (k_field_origin_coords<NC><<<cdiv(n, 256), 256, 0, s>>>(
+                                  field, n, ocoords, bad)));
     MEB_LAUNCH_OK();
+  }
+  uint32_t h[2] = {0, 0};
+  int rc = insert_and_map(ocoords, nullptr, n, ncols, table, capacity, unique_coords,
+                          unique_index, inverse_map, scratch, h, n > 0 ? 2 : 1, s);
+  if (rc != MEB200_OK) return rc;
+  *h_num_unique = h[0];
+  if (h[1] != 0) {
+    set_error("a field batch coordinate is not finite, or lies outside int32");
+    return MEB200_ERR_DOMAIN;
   }
   return MEB200_OK;
 }

@@ -9,6 +9,7 @@ from .coordinate_manager import CoordinateManager
 from .enums import PoolingMode
 from .kernel_generator import KernelGenerator
 from .sparse_tensor import SparseTensor, _get_coordinate_map_key
+from .tensor_field import TensorField
 
 
 class MinkowskiLocalPoolingFunction(Function):
@@ -167,13 +168,15 @@ class MinkowskiPoolingTranspose(MinkowskiPoolingBase):
 
 
 class MinkowskiGlobalPoolingFunction(Function):
-    """Per-cloud reduction to the origin map (reference: MinkowskiPooling.py:583-630)."""
+    """Per-cloud reduction to the origin map (reference: MinkowskiPooling.py:583-630).
+    `is_field=True`: `in_coordinate_map_key` is the key of a TensorField and the rows are its
+    points."""
 
     @staticmethod
     def forward(ctx, input_features: torch.Tensor, pooling_mode: PoolingMode,
                 in_coordinate_map_key: CoordinateMapKey,
                 out_coordinate_map_key: CoordinateMapKey = None,
-                coordinate_manager: CoordinateManager = None):
+                coordinate_manager: CoordinateManager = None, is_field: bool = False):
         if out_coordinate_map_key is None:
             out_coordinate_map_key = CoordinateMapKey(
                 in_coordinate_map_key.get_coordinate_size())
@@ -183,9 +186,10 @@ class MinkowskiGlobalPoolingFunction(Function):
         ctx.out_coords_key = out_coordinate_map_key
         ctx.coordinate_manager = coordinate_manager
         ctx.pooling_mode = pooling_mode
+        ctx.is_field = is_field
         out_feat, num_nonzero = _C.GlobalPoolingForwardGPU(
             input_features, pooling_mode, in_coordinate_map_key, out_coordinate_map_key,
-            coordinate_manager._manager)
+            coordinate_manager._manager, is_field=is_field)
         ctx.num_nonzero = num_nonzero
         return out_feat
 
@@ -194,13 +198,16 @@ class MinkowskiGlobalPoolingFunction(Function):
         grad_out_feat = grad_out_feat.contiguous()
         grad_in_feat = _C.GlobalPoolingBackwardGPU(
             ctx.input_features, grad_out_feat, ctx.num_nonzero, ctx.pooling_mode,
-            ctx.in_coords_key, ctx.out_coords_key, ctx.coordinate_manager._manager)
+            ctx.in_coords_key, ctx.out_coords_key, ctx.coordinate_manager._manager,
+            is_field=ctx.is_field)
         return grad_in_feat, None, None, None, None, None
 
 
 class MinkowskiGlobalPooling(MinkowskiModuleBase):
     """Reduces every cloud to one row at its origin (b, 0, ..., 0); output row s is the cloud
-    with the s-th smallest batch index (reference: MinkowskiPooling.py:633-677)."""
+    with the s-th smallest batch index (reference: MinkowskiPooling.py:633-677).  The input may be
+    a SparseTensor or a TensorField (its points, batch index lroundf of the first coordinate);
+    both land on the manager's one origin map."""
 
     def __init__(self, mode: PoolingMode = PoolingMode.GLOBAL_AVG_POOLING_PYTORCH_INDEX):
         super().__init__()
@@ -208,10 +215,17 @@ class MinkowskiGlobalPooling(MinkowskiModuleBase):
         self.pooling_mode = mode
         self.pooling = MinkowskiGlobalPoolingFunction
 
-    def forward(self, input: SparseTensor, coordinates=None):
-        out_key = _get_coordinate_map_key(input, coordinates)
+    def forward(self, input, coordinates=None):
+        is_field = isinstance(input, TensorField)
+        if is_field:
+            if coordinates is not None:
+                raise ValueError("global pooling of a TensorField writes to the origin map: "
+                                 "`coordinates` cannot be given")
+            out_key = CoordinateMapKey(input.coordinate_field_map_key.get_coordinate_size())
+        else:
+            out_key = _get_coordinate_map_key(input, coordinates)
         output = self.pooling.apply(input.F, self.pooling_mode, input.coordinate_map_key, out_key,
-                                    input._manager)
+                                    input._manager, is_field)
         return SparseTensor(output, coordinate_map_key=out_key,
                             coordinate_manager=input.coordinate_manager)
 
