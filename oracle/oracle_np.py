@@ -67,6 +67,21 @@ def stride_map_coords(coords, tensor_stride, kernel_stride):
     return unique_rows(stride_coordinate(coords, out_ts)), out_ts
 
 
+def stride_region_coords(coords, offsets, out_tensor_stride, is_transpose):
+    """CoordinateMapCPU::stride_region (src/coordinate_map_cpu.hpp:446-487): every input row
+    moved by every region offset; the forward (expanding) form keeps only the coordinates that
+    are multiples of the out tensor stride, the transposed form keeps them all.  Returns the
+    unique coordinates in canonical order."""
+    coords = np.asarray(coords, np.int32)
+    offs = np.asarray(offsets, np.int32)
+    cand = np.repeat(coords, len(offs), axis=0)
+    cand[:, 1:] += np.tile(offs, (len(coords), 1))
+    if not is_transpose:
+        s = np.asarray(out_tensor_stride, np.int32)[None, :]
+        cand = cand[(cand[:, 1:] % s == 0).all(axis=1)]
+    return unique_rows(cand)
+
+
 def region_offsets(region_type, kernel_size, dilation, tensor_stride, custom=None):
     """kernel_region::coordinate_at (src/kernel_region.hpp:198-247) as an offset table
     [K, D]; volume per set_volume (:250-270)."""

@@ -54,6 +54,19 @@ def oracle_conv_layer(in_coords, tensor_stride, kernel_size, stride, dilation, t
     return out_coords, im, om
 
 
+def layer_out_ts(meta):
+    """The output tensor stride of a layer fixture (tests/golden/ref_layer_*.npz), but for one
+    deliberate difference: the reference's convolution passes `expand_coordinates` to
+    `_get_coordinate_map_key` in the place of its `tensor_stride` argument
+    (MinkowskiConvolution.py:311-313), so output coordinates given as a tensor are inserted at
+    tensor stride 0 there.  This package inserts them at tensor stride 1, the default of that
+    argument; the map and the features are the same."""
+    if meta["given"] == "tensor":
+        assert meta["out_ts"] == [0] * meta["D"]
+        return [1] * meta["D"]
+    return meta["out_ts"]
+
+
 def rel_err(a, b):
     a = np.asarray(a, np.float64); b = np.asarray(b, np.float64)
     return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
