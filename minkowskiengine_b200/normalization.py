@@ -127,7 +127,9 @@ class _BatchNormFunction(torch.autograd.Function):
                 residual = residual.contiguous()
             y = torch.empty_like(x)
             if use_running:
-                mean = running_mean.detach().float().contiguous()
+                # a copy: backward reads it, and a training forward in between rewrites the
+                # buffer from the kernel, unseen by autograd's version counter
+                mean = running_mean.detach().clone()
                 invstd = torch.rsqrt(running_var.detach().float() + eps)
             else:
                 mean = torch.empty(C, dtype=torch.float32, device=dev)

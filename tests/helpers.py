@@ -81,11 +81,16 @@ def one_rounding_bound(ref, A, dtype, acc=1.0):
     delta = A * (acc * 2.0 ** -20)
     if dtype == torch.float32:
         return delta
+    return half_ulp(ref.abs() + delta, dtype) + delta
+
+
+def half_ulp(v, dtype):
+    """Half an ulp of bf16 / fp16 at the magnitudes `v` (float64, >= 0): the largest error of one
+    rounding to `dtype` of a value of magnitude at most v."""
     p, emin = {torch.bfloat16: (7, -126), torch.float16: (10, -14)}[dtype]
-    v = ref.abs() + delta
     _, e = torch.frexp(v)                        # v = m * 2^e, m in [0.5, 1)
     e = torch.where(v > 0, e - 1, torch.full_like(e, emin)).clamp(min=emin)
-    return torch.ldexp(torch.full_like(v, 0.5), e - p) + delta
+    return torch.ldexp(torch.full_like(v, 0.5), e - p)
 
 
 # The wgmma kernels' fp32 accumulation of bf16 / fp16 products is less accurate than the CUDA
