@@ -44,8 +44,23 @@ def _bn_relu(ME):
     return bn_relu
 
 
+def _conv_bn_relu(ME):
+    """relu(norm(conv(x)) [+ residual]) on module handles that provide it
+    (minkowskiengine_b200.fused_conv_bn_relu: one pass in eval mode under no_grad, the convolution
+    then fused_bn_relu otherwise), the reference's separate ops otherwise."""
+    fused = getattr(ME, "fused_conv_bn_relu", None)
+    bn_relu = _bn_relu(ME)
+
+    def conv_bn_relu(conv, norm, relu, x, residual=None):
+        if fused is not None:
+            return fused(conv, norm, x, residual)
+        return bn_relu(norm, relu, conv(x), residual)
+    return conv_bn_relu
+
+
 def _basic_block(ME):
     bn_relu = _bn_relu(ME)
+    conv_bn_relu = _conv_bn_relu(ME)
 
     class BasicBlock(nn.Module):
         expansion = 1
@@ -63,12 +78,15 @@ def _basic_block(ME):
             self.downsample = downsample
 
         def forward(self, x):
-            residual = x
-            out = bn_relu(self.norm1, self.relu, self.conv1(x))
-            out = self.conv2(out)
-            if self.downsample is not None:
-                residual = self.downsample(x)
-            return bn_relu(self.norm2, self.relu, out, residual)
+            out = conv_bn_relu(self.conv1, self.norm1, self.relu, x)
+            if self.downsample is None:
+                return conv_bn_relu(self.conv2, self.norm2, self.relu, out, x)
+            if self.training:
+                # training fuses nothing here: keep conv2 ahead of the downsample, the order in
+                # which the block has always launched its layers
+                out = self.conv2(out)
+                return bn_relu(self.norm2, self.relu, out, self.downsample(x))
+            return conv_bn_relu(self.conv2, self.norm2, self.relu, out, self.downsample(x))
 
     return BasicBlock
 
@@ -80,7 +98,7 @@ def minkunet(name, ME, in_channels=3, out_channels=20, D=3):
     layers = _LAYERS[base]
     planes = (_PLANES_34 if base == "MinkUNet34" else _PLANES)[variant]
     block = _basic_block(ME)
-    bn_relu = _bn_relu(ME)
+    conv_bn_relu = _conv_bn_relu(ME)
     init_dim = 32
 
     class MinkUNet(nn.Module):
@@ -149,26 +167,26 @@ def minkunet(name, ME, in_channels=3, out_channels=20, D=3):
 
         def forward(self, x):
             relu = self.relu
-            out = bn_relu(self.bn0, relu, self.conv0p1s1(x))
+            out = conv_bn_relu(self.conv0p1s1, self.bn0, relu, x)
             out_p1 = out
-            out = bn_relu(self.bn1, relu, self.conv1p1s2(out_p1))
+            out = conv_bn_relu(self.conv1p1s2, self.bn1, relu, out_p1)
             out_b1p2 = self.block1(out)
-            out = bn_relu(self.bn2, relu, self.conv2p2s2(out_b1p2))
+            out = conv_bn_relu(self.conv2p2s2, self.bn2, relu, out_b1p2)
             out_b2p4 = self.block2(out)
-            out = bn_relu(self.bn3, relu, self.conv3p4s2(out_b2p4))
+            out = conv_bn_relu(self.conv3p4s2, self.bn3, relu, out_b2p4)
             out_b3p8 = self.block3(out)
-            out = bn_relu(self.bn4, relu, self.conv4p8s2(out_b3p8))
+            out = conv_bn_relu(self.conv4p8s2, self.bn4, relu, out_b3p8)
             out = self.block4(out)
-            out = bn_relu(self.bntr4, relu, self.convtr4p16s2(out))
+            out = conv_bn_relu(self.convtr4p16s2, self.bntr4, relu, out)
             out = ME.cat(out, out_b3p8)
             out = self.block5(out)
-            out = bn_relu(self.bntr5, relu, self.convtr5p8s2(out))
+            out = conv_bn_relu(self.convtr5p8s2, self.bntr5, relu, out)
             out = ME.cat(out, out_b2p4)
             out = self.block6(out)
-            out = bn_relu(self.bntr6, relu, self.convtr6p4s2(out))
+            out = conv_bn_relu(self.convtr6p4s2, self.bntr6, relu, out)
             out = ME.cat(out, out_b1p2)
             out = self.block7(out)
-            out = bn_relu(self.bntr7, relu, self.convtr7p2s2(out))
+            out = conv_bn_relu(self.convtr7p2s2, self.bntr7, relu, out)
             out = ME.cat(out, out_p1)
             out = self.block8(out)
             return self.final(out)

@@ -195,11 +195,23 @@ int meb200_kernel_map_pairs(const int32_t *nbr, uint32_t K, uint32_t n_rows, uin
  * qualifies, otherwise the small-cin or SIMT kernels on w_cast.
  * out_order (may be NULL): the tile order of out_nbr from meb200_kernel_map; the tensor-core
  * kernel then runs only the offsets each tile of 128 output rows reaches (read when K <= 32).
+ * epi (may be NULL): an epilogue every kernel applies to its fp32 accumulator before the one
+ * conversion to out_dtype (see meb200_conv_epilogue); NULL writes the accumulator as it is.
  */
+/* Per-channel affine map, residual and ReLU folded into a convolution's output (eval-mode batch
+ * norm after a convolution): out[o, c] = relu?(acc[o, c] * scale[c] + shift[c] + residual[o, c]),
+ * in fp32 (the product and shift as one fused multiply-add), rounded once to out_dtype.  A row
+ * without neighbours has acc = 0.  Host struct; its pointers are device pointers. */
+typedef struct meb200_conv_epilogue {
+  const float *scale;                 /* [c_out] fp32 */
+  const float *shift;                 /* [c_out] fp32 */
+  const void *residual;               /* [n_out, c_out] in out_dtype, or NULL */
+  int32_t relu;                       /* != 0: clamp at zero after the residual */
+} meb200_conv_epilogue;
 int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
                         const void *w_cast, const void *w_t, uint32_t K, uint32_t c_out,
                         const int32_t *out_nbr, uint32_t n_out, void *out, int out_dtype,
-                        const int32_t *out_order, void *stream);
+                        const int32_t *out_order, const meb200_conv_epilogue *epi, void *stream);
 
 /* grad_in[i,:] = sum_k grad_out[in_nbr[k,i],:] @ W[k]^T   (fully written)
  * grad_weight[k] = sum_o in[out_nbr[k,o],:]^T @ grad_out[o,:]   (fully written, fp32)
@@ -264,12 +276,13 @@ int meb200_conv_pack_weights_batched(const meb200_pack_job *jobs_dev, uint32_t n
  *   workspace      meb200_conv_workspace_bytes(n_out, V, c_out, 1, dtype) bytes, 16-byte aligned,
  *                  for the row-split partial sums, as in meb200_conv_backward (less, NULL or
  *                  unaligned is legal and means fewer splits, down to one)
+ *   epi            (forward, may be NULL) as in meb200_conv_forward
  * bf16 / fp16 only; c_out a multiple of 16, <= 256. */
 uint32_t meb200_conv_stem_virtual_channels(uint32_t K);
 int meb200_conv_stem_supported(int dtype, uint32_t K, uint32_t c_out);
 int meb200_conv_stem_forward(const void *in4, int dtype, uint32_t K, const void *weight_v,
                              uint32_t c_out, const int32_t *out_nbr, uint32_t n_out, void *out,
-                             int out_dtype, void *stream);
+                             int out_dtype, const meb200_conv_epilogue *epi, void *stream);
 int meb200_conv_stem_wgrad(const void *in4, const void *grad_out, int dtype, uint32_t K,
                            uint32_t c_out, const int32_t *out_nbr, uint32_t n_out,
                            float *grad_weight_v, void *workspace, uint64_t workspace_bytes,

@@ -44,7 +44,7 @@ PROTOTYPES = {
     "meb200_kernel_map": (_i32, [_vp, _u32, _vp, _u32, _vp, _u32, _u32, _vp, _u32, _vp, _vp,
                                  _vp, _vp, _vp, _vp, _vp]),
     "meb200_conv_forward": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _u32, _vp,
-                                   _i32, _vp, _vp]),
+                                   _i32, _vp, _vp, _vp]),
     "meb200_conv_backward": (_i32, [_vp, _vp, _i32, _u32, _u32, _vp, _u32, _u32, _vp, _vp,
                                     _u32, _vp, _i32, _vp, _vp, _vp, _vp, _u32, _vp, _u64, _vp,
                                     _vp]),
@@ -53,7 +53,8 @@ PROTOTYPES = {
     "meb200_conv_pack_weights_batched": (_i32, [_vp, _u32, _u32, _i32, _vp]),
     "meb200_conv_stem_virtual_channels": (_u32, [_u32]),
     "meb200_conv_stem_supported": (_i32, [_i32, _u32, _u32]),
-    "meb200_conv_stem_forward": (_i32, [_vp, _i32, _u32, _vp, _u32, _vp, _u32, _vp, _i32, _vp]),
+    "meb200_conv_stem_forward": (_i32, [_vp, _i32, _u32, _vp, _u32, _vp, _u32, _vp, _i32, _vp,
+                                        _vp]),
     "meb200_conv_stem_wgrad": (_i32, [_vp, _vp, _i32, _u32, _u32, _vp, _u32, _vp, _vp, _u64, _vp]),
     "meb200_pair_list_chunks": (_u32, [_u32, _u32]),
     "meb200_pair_list_scratch_bytes": (_u64, [_u32, _u32, _u32]),
@@ -121,16 +122,17 @@ PROTOTYPES = {
                                               C.c_uint64, _u32, _u32, _u32, _vp, _vp, _vp, _vp]),
 }
 
-# meb200_conv_backward gained its `in_order` pointer just before the stream.  Callers written
-# against the argument list it had before (the direct-call test helper among them) still work: a
-# call one argument short gets NULL there (no order: every tile runs every offset).  Any other
-# argument count goes to ctypes unchanged and fails there.  The backend passes the full list.
-_ORDER_ADDED = ("meb200_conv_backward",)
+# These calls gained an optional pointer just before the stream: meb200_conv_backward its
+# `in_order`, the two forwards their `epi`.  Callers written against the argument list they had
+# before (the direct-call test helpers among them) still work: a call one argument short gets NULL
+# there (no order: every tile runs every offset; no epilogue).  Any other argument count goes to
+# ctypes unchanged and fails there.  The backend passes the full list.
+_POINTER_ADDED = ("meb200_conv_backward", "meb200_conv_forward", "meb200_conv_stem_forward")
 
 _lib = None
 
 
-def _order_optional(fn, n_args):
+def _pointer_optional(fn, n_args):
     def call(*args):
         if len(args) == n_args - 1:
             args = args[:-1] + (None, args[-1])
@@ -158,8 +160,8 @@ def load():
         fn = getattr(lib, name)  # AttributeError -> loud failure on a stale library
         fn.restype = res
         fn.argtypes = args
-    for name in _ORDER_ADDED:
-        setattr(lib, name, _order_optional(getattr(lib, name), len(PROTOTYPES[name][1])))
+    for name in _POINTER_ADDED:
+        setattr(lib, name, _pointer_optional(getattr(lib, name), len(PROTOTYPES[name][1])))
     _lib = lib
     return lib
 

@@ -13,6 +13,7 @@ from .common import MinkowskiModuleBase
 from .coordinate_manager import CoordinateManager
 from .enums import ConvolutionMode, RegionType
 from .kernel_generator import KernelGenerator
+from .normalization import MinkowskiBatchNorm, _bn_tail, _eval_scale_shift, _native_ok
 from .sparse_tensor import SparseTensor, _get_coordinate_map_key
 
 
@@ -204,3 +205,78 @@ class MinkowskiGenerativeConvolutionTranspose(MinkowskiConvolutionBase):
             kernel_generator, is_transpose=True, expand_coordinates=True,
             convolution_mode=convolution_mode, dimension=dimension)
         self.reset_parameters(True)
+
+
+_FUSED_CONVS = (MinkowskiConvolution, MinkowskiConvolutionTranspose,
+                MinkowskiGenerativeConvolutionTranspose)
+
+
+def _fuses(conv, norm, feats, res):
+    """Whether conv -> norm [+ res] can run as one convolution with an epilogue, from everything
+    but the residual's coordinate map: norm in eval mode with running statistics (and a shape and
+    dtype the native batch norm takes), no gradient needed, a conv that is not a plain matrix
+    product (kernel volume 1, stride 1), a residual in the output dtype."""
+    bn = norm.bn
+    if bn.training or conv.use_mm:
+        return False
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (
+            feats, conv.kernel, conv.bias, bn.weight, bn.bias, res)):
+        return False
+    if res is not None and res.dtype != feats.dtype:
+        return False
+    return _native_ok(bn, feats.new_empty((0, conv.out_channels)))
+
+
+def _output_key(conv, input):
+    """The key of conv(input)'s output map, made as the forward makes it."""
+    kg = conv.kernel_generator
+    manager = input._manager._manager
+    out_key = _get_coordinate_map_key(input, None, expand_coordinates=kg.expand_coordinates)
+    region = (kg.region_type, kg.kernel_size, kg.kernel_dilation, kg.region_offsets)
+    if conv.is_transpose:
+        _C._set_transposed_key(manager, input.coordinate_map_key, out_key, kg.kernel_stride,
+                               region, kg.expand_coordinates)
+    else:
+        _C._set_strided_key(manager, input.coordinate_map_key, out_key, kg.kernel_stride,
+                            region if kg.expand_coordinates else None)
+    return out_key
+
+
+def fused_conv_bn_relu(conv, norm, input, residual=None, relu=True):
+    """relu?(norm(conv(input)) [+ residual]) on the convolution's output map.
+
+    `conv`: a MinkowskiConvolution, MinkowskiConvolutionTranspose or
+    MinkowskiGenerativeConvolutionTranspose; `norm`: a MinkowskiBatchNorm or MinkowskiSyncBatchNorm.
+    When `norm` is in eval mode with running statistics and no gradient is needed, eval batch norm
+    is one affine map per channel, and the convolution applies it (with its own bias folded in),
+    the residual and the ReLU to its fp32 accumulator before its one rounding to the output dtype:
+    the normalised tensor is written once instead of written, read back and written again.  In
+    every other case (training, a K = 1 stride-1 layer, a shape the native batch norm does not
+    take, a residual on another map or in another dtype) this is exactly
+    fused_bn_relu(norm, conv(input), residual), or norm(conv(input)) when relu is False and there
+    is no residual."""
+    if not isinstance(conv, _FUSED_CONVS):
+        raise TypeError(f"fused_conv_bn_relu: {type(conv).__name__} is not a MinkowskiConvolution, "
+                        "MinkowskiConvolutionTranspose or MinkowskiGenerativeConvolutionTranspose")
+    if not isinstance(norm, MinkowskiBatchNorm):
+        raise TypeError(f"fused_conv_bn_relu: {type(norm).__name__} is not a MinkowskiBatchNorm "
+                        "or MinkowskiSyncBatchNorm")
+    assert isinstance(input, SparseTensor)
+    res = residual.F if residual is not None else None
+    out_key = _output_key(conv, input) if _fuses(conv, norm, input.F, res) else None
+    if res is not None and out_key is not None and residual.coordinate_map_key != out_key:
+        out_key = None
+    if out_key is None:
+        out = conv(input)
+        if residual is None and not relu:
+            return norm(out)
+        return _bn_tail(norm, out, residual, relu)
+    assert input.D == conv.dimension
+    kg = conv.kernel_generator
+    scale, shift = _eval_scale_shift(norm.bn, conv.bias)
+    forward = _C.ConvolutionTransposeForwardGPU if conv.is_transpose else _C.ConvolutionForwardGPU
+    feats = forward(input.F.contiguous(), conv.kernel, kg.kernel_size, kg.kernel_stride,
+                    kg.kernel_dilation, kg.region_type, kg.region_offsets, kg.expand_coordinates,
+                    conv.convolution_mode, input.coordinate_map_key, out_key, input._manager._manager,
+                    epilogue=(scale, shift, None if res is None else res.contiguous(), relu))
+    return SparseTensor(feats, coordinate_map_key=out_key, coordinate_manager=input._manager)

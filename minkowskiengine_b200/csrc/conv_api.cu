@@ -11,6 +11,12 @@ using namespace meb200;
 // dtype of the feature storage: TF32 convolutions keep fp32 features
 static int storage_dtype(int dtype) { return dtype == MEB200_TF32 ? MEB200_F32 : dtype; }
 
+// NULL, or scale and shift given; the tensor-core kernels read pairs of columns (8 bytes)
+static bool epilogue_ok(const meb200_conv_epilogue *epi) {
+  return epi == nullptr || (epi->scale && epi->shift && aligned(8, epi->scale, epi->shift) &&
+                            (epi->residual == nullptr || aligned(8, epi->residual)));
+}
+
 extern "C" {
 
 uint64_t meb200_conv_workspace_bytes(uint32_t n_out, uint32_t c_in, uint32_t c_out, uint32_t K,
@@ -29,7 +35,8 @@ int meb200_conv_wgrad_uses_pairs(int dtype, uint32_t c_in, uint32_t c_out, uint3
 int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
                         const void *w_cast, const void *w_t, uint32_t K, uint32_t c_out,
                         const int32_t *out_nbr, uint32_t n_out, void *out, int out_dtype,
-                        const int32_t *out_order, void *stream_) {
+                        const int32_t *out_order, const meb200_conv_epilogue *epi,
+                        void *stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (n_out == 0) return MEB200_OK;
   MEB_CHECK_ARG(in_dtype >= 0 && in_dtype <= 3 && out_dtype >= 0 && out_dtype <= 2, "dtype");
@@ -38,19 +45,20 @@ int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_
   MEB_CHECK_ARG(out && w_cast && (w_t || in_dtype == MEB200_F32) && out_nbr && (in || n_in == 0),
                 "null buffer");
   MEB_CHECK_ARG(c_in > 0 && c_out > 0 && K > 0, "empty channel/kernel dims");
+  MEB_CHECK_ARG(epilogue_ok(epi), "epilogue: scale and shift required, 8-byte aligned pointers");
   if (conv_tc_supported(in_dtype, c_in, c_out)) {
     int rc = conv_forward_tc(in, in_dtype, n_in, c_in, w_t, K, c_out, out_nbr, out_order, n_out,
-                             out, out_dtype, stream);
+                             out, out_dtype, epi, stream);
     if (rc != MEB200_ERR_UNSUPPORTED) return rc;
   }
   const int fdt = storage_dtype(in_dtype);      // the CUDA-core kernels: exact fp32 for TF32
   if (conv_small_cin_supported(c_in, c_out)) {
     int rc = conv_small_cin_forward(in, fdt, c_in, w_cast, K, c_out, out_nbr, n_out, out,
-                                    out_dtype, stream);
+                                    out_dtype, epi, stream);
     if (rc != MEB200_ERR_UNSUPPORTED) return rc;
   }
   return conv_forward_simt(in, fdt, n_in, c_in, w_cast, K, c_out, /*trans_w=*/false,
-                           out_nbr, n_out, out, out_dtype, stream);
+                           out_nbr, n_out, out, out_dtype, epi, stream);
 }
 
 static bool packed_dtype(int dtype) {
@@ -83,15 +91,16 @@ int meb200_conv_stem_supported(int dtype, uint32_t K, uint32_t c_out) {
 
 int meb200_conv_stem_forward(const void *in4, int dtype, uint32_t K, const void *weight_v,
                              uint32_t c_out, const int32_t *out_nbr, uint32_t n_out, void *out,
-                             int out_dtype, void *stream_) {
+                             int out_dtype, const meb200_conv_epilogue *epi, void *stream_) {
   if (n_out == 0) return MEB200_OK;
   MEB_CHECK_ARG(out_dtype == MEB200_F32 || out_dtype == dtype, "output dtype must be fp32 or the input dtype");
   MEB_CHECK_ARG(in4 && weight_v && out_nbr && out, "null buffer");
+  MEB_CHECK_ARG(epilogue_ok(epi), "epilogue: scale and shift required, 8-byte aligned pointers");
   if (!conv_stem_tc_supported(dtype, K, c_out)) {
     set_error("stem forward: shape/dtype outside the tensor-core path (K=%u c_out=%u)", K, c_out);
     return MEB200_ERR_UNSUPPORTED;
   }
-  return conv_stem_forward_tc(in4, dtype, K, weight_v, c_out, out_nbr, n_out, out, out_dtype,
+  return conv_stem_forward_tc(in4, dtype, K, weight_v, c_out, out_nbr, n_out, out, out_dtype, epi,
                               (cudaStream_t)stream_);
 }
 
@@ -129,10 +138,10 @@ int meb200_conv_backward(const void *in, const void *grad_out, int dtype, uint32
     int rc = MEB200_ERR_UNSUPPORTED;
     if (conv_tc_supported(dtype, c_out, c_in))
       rc = conv_forward_tc(grad_out, dtype, n_out, c_out, w_cast, K, c_in, in_nbr, in_order, n_in,
-                           grad_in, grad_in_dtype, stream);
+                           grad_in, grad_in_dtype, nullptr, stream);
     if (rc == MEB200_ERR_UNSUPPORTED)
       rc = conv_forward_simt(grad_out, fdt, n_out, c_out, w_cast, K, c_in, /*trans_w=*/true,
-                             in_nbr, n_in, grad_in, grad_in_dtype, stream);
+                             in_nbr, n_in, grad_in, grad_in_dtype, nullptr, stream);
     if (rc != MEB200_OK) return rc;
   }
   if (grad_weight != nullptr) {

@@ -14,14 +14,26 @@ namespace meb200 {
 
 constexpr int TM = 64, TN = 64, TK = 16;
 
+// The forward's epilogue (meb200_conv_epilogue) on the accumulator of output element (o, c):
+// fmaf(acc, scale, shift) + residual, then the ReLU, all in fp32, as the eval batch norm applies it.
+template <typename TOut>
+__device__ __forceinline__ float epilogue(const meb200_conv_epilogue &e, float acc, uint32_t o,
+                                          uint32_t c, uint32_t c_out) {
+  float v = fmaf(acc, __ldg(e.scale + c), __ldg(e.shift + c));
+  if (e.residual != nullptr)
+    v += to_f32<TOut>(reinterpret_cast<const TOut *>(e.residual)[(size_t)o * c_out + c]);
+  return e.relu ? fmaxf(v, 0.f) : v;
+}
+
 // out[r, n] = sum_k sum_c A[nbr[k][r], c] * Wk(c, n)
 //   TRANS_W = false: Wk(c, n) = W[k][c][n]   (W is [K, c_a, c_n])        -> forward
 //   TRANS_W = true : Wk(c, n) = W[k][n][c]   (W is [K, c_n, c_a])        -> dgrad
-template <typename TIn, typename TOut, bool TRANS_W>
+// EPI: the forward's epilogue `epi` before the conversion (not read otherwise).
+template <typename TIn, typename TOut, bool TRANS_W, bool EPI>
 __global__ void __launch_bounds__(256)
 k_conv_gather_gemm(const TIn *__restrict__ A, uint32_t c_a, const TIn *__restrict__ W, uint32_t K,
                    uint32_t c_n, const int32_t *__restrict__ nbr, uint32_t n_rows,
-                   TOut *__restrict__ out) {
+                   TOut *__restrict__ out, const meb200_conv_epilogue epi) {
   __shared__ float As[TK][TM + 4];
   __shared__ float Bs[TK][TN + 4];
   __shared__ int32_t s_idx[TM];
@@ -92,7 +104,10 @@ k_conv_gather_gemm(const TIn *__restrict__ A, uint32_t c_a, const TIn *__restric
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       uint32_t n = n0 + tx * 4 + j;
-      if (n < c_n) out[(size_t)r * c_n + n] = from_f32<TOut>(acc[i][j]);
+      if (n >= c_n) continue;
+      float v = acc[i][j];
+      if constexpr (EPI) v = epilogue<TOut>(epi, v, r, n, c_n);
+      out[(size_t)r * c_n + n] = from_f32<TOut>(v);
     }
   }
 }
@@ -200,11 +215,11 @@ __device__ __forceinline__ void store_row(TOut *__restrict__ dst, const float (&
     if ((uint32_t)i < c_out) dst[i] = from_f32<TOut>(acc[i]);
 }
 
-template <typename T, typename TOut, int CO>
+template <typename T, typename TOut, int CO, bool EPI>
 __global__ void __launch_bounds__(128)
 k_conv_small_cin_fwd(const T *__restrict__ in, uint32_t c_in, const T *__restrict__ W, uint32_t K,
                      uint32_t c_out, const int32_t *__restrict__ nbr, uint32_t n_out,
-                     TOut *__restrict__ out) {
+                     TOut *__restrict__ out, const meb200_conv_epilogue epi) {
   extern __shared__ float Ws[];  // [K][c_in][CO], zero padded past c_out
   for (uint32_t e = threadIdx.x; e < K * c_in * CO; e += blockDim.x) {
     uint32_t co = e % CO, kc = e / CO;
@@ -257,6 +272,13 @@ k_conv_small_cin_fwd(const T *__restrict__ in, uint32_t c_in, const T *__restric
       }
 #pragma unroll
       for (int j = 0; j < SK; ++j) idx[j] = nxt[j];
+    }
+    if constexpr (EPI) {
+      if (live) {
+#pragma unroll
+        for (int i = 0; i < CO; ++i)
+          if ((uint32_t)i < c_out) acc[i] = epilogue<TOut>(epi, acc[i], o, i, c_out);
+      }
     }
     if (live) store_row<TOut, CO>(out + (size_t)o * c_out, acc, c_out);
   }
@@ -379,35 +401,44 @@ bool conv_small_cin_supported(uint32_t c_in, uint32_t c_out) {
   return c_in >= 1 && c_in <= 4 && c_out <= 64;
 }
 
+template <typename T, typename TOut, int CO, bool EPI>
+static int launch_small_fwd_kernel(unsigned grid, size_t smem, const void *in, uint32_t c_in,
+                                   const void *W, uint32_t K, uint32_t c_out, const int32_t *nbr,
+                                   uint32_t n_out, void *out, const meb200_conv_epilogue &epi,
+                                   cudaStream_t stream) {
+  auto kern = k_conv_small_cin_fwd<T, TOut, CO, EPI>;
+  MEB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  kern<<<grid, 128, smem, stream>>>((const T *)in, c_in, (const T *)W, K, c_out, nbr, n_out,
+                                    (TOut *)out, epi);
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
+}
+
 template <typename T, typename TOut>
 static int launch_small_fwd(const void *in, uint32_t c_in, const void *W, uint32_t K,
                             uint32_t c_out, const int32_t *nbr, uint32_t n_out, void *out,
-                            cudaStream_t stream) {
+                            const meb200_conv_epilogue *epi, cudaStream_t stream) {
   const int CO = c_out <= 32 ? 32 : 64;
   size_t smem = (size_t)K * c_in * CO * sizeof(float);
   if (smem > 200 * 1024) return MEB200_ERR_UNSUPPORTED;
   // persistent CTAs: as many as fit beside each other (shared memory bound), W staged once each
   unsigned per_sm = (unsigned)std::max<size_t>(1, std::min<size_t>(8, (220 * 1024) / (smem + 1024)));
   unsigned grid = std::min<unsigned>(cdiv(n_out, 128), per_sm * num_sms());
-  if (CO == 32) {
-    auto kern = k_conv_small_cin_fwd<T, TOut, 32>;
-    MEB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    kern<<<grid, 128, smem, stream>>>((const T *)in, c_in, (const T *)W, K, c_out, nbr, n_out, (TOut *)out);
-  } else {
-    auto kern = k_conv_small_cin_fwd<T, TOut, 64>;
-    MEB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    kern<<<grid, 128, smem, stream>>>((const T *)in, c_in, (const T *)W, K, c_out, nbr, n_out, (TOut *)out);
-  }
-  MEB_LAUNCH_OK();
-  return MEB200_OK;
+  const meb200_conv_epilogue e = epi != nullptr ? *epi : meb200_conv_epilogue{};
+#define MEB_L(CO_, EPI_) launch_small_fwd_kernel<T, TOut, CO_, EPI_>(grid, smem, in, c_in, W, K, \
+                                                                      c_out, nbr, n_out, out, e, stream)
+  if (CO == 32) return epi != nullptr ? MEB_L(32, true) : MEB_L(32, false);
+  return epi != nullptr ? MEB_L(64, true) : MEB_L(64, false);
+#undef MEB_L
 }
 
 int conv_small_cin_forward(const void *in, int in_dtype, uint32_t c_in, const void *W, uint32_t K,
                            uint32_t c_out, const int32_t *nbr, uint32_t n_out, void *out,
-                           int out_dtype, cudaStream_t stream) {
+                           int out_dtype, const meb200_conv_epilogue *epi, cudaStream_t stream) {
   if (n_out == 0) return MEB200_OK;
   MEB_DISPATCH_DTYPE_OUT(in_dtype, out_dtype,
-                         return launch_small_fwd<T, TO>(in, c_in, W, K, c_out, nbr, n_out, out, stream));
+                         return launch_small_fwd<T, TO>(in, c_in, W, K, c_out, nbr, n_out, out, epi,
+                                                        stream));
 }
 
 // Row slices k_conv_small_cin_wgrad plans: one 8-warp CTA per SM (register tiles), aiming at
@@ -460,14 +491,18 @@ int conv_small_cin_wgrad(const void *in, const void *grad_out, int dtype, uint32
 template <typename TIn, typename TOut>
 static int launch_gg(const void *A, uint32_t c_a, const void *W, uint32_t K, uint32_t c_n,
                      bool trans_w, const int32_t *nbr, uint32_t n_rows, void *out,
-                     cudaStream_t stream) {
+                     const meb200_conv_epilogue *epi, cudaStream_t stream) {
   dim3 grid(cdiv(n_rows, TM), cdiv(c_n, TN));
+  const meb200_conv_epilogue e = epi != nullptr ? *epi : meb200_conv_epilogue{};
   if (trans_w)
-    k_conv_gather_gemm<TIn, TOut, true><<<grid, 256, 0, stream>>>(
-        (const TIn *)A, c_a, (const TIn *)W, K, c_n, nbr, n_rows, (TOut *)out);
+    k_conv_gather_gemm<TIn, TOut, true, false><<<grid, 256, 0, stream>>>(
+        (const TIn *)A, c_a, (const TIn *)W, K, c_n, nbr, n_rows, (TOut *)out, e);
+  else if (epi != nullptr)
+    k_conv_gather_gemm<TIn, TOut, false, true><<<grid, 256, 0, stream>>>(
+        (const TIn *)A, c_a, (const TIn *)W, K, c_n, nbr, n_rows, (TOut *)out, e);
   else
-    k_conv_gather_gemm<TIn, TOut, false><<<grid, 256, 0, stream>>>(
-        (const TIn *)A, c_a, (const TIn *)W, K, c_n, nbr, n_rows, (TOut *)out);
+    k_conv_gather_gemm<TIn, TOut, false, false><<<grid, 256, 0, stream>>>(
+        (const TIn *)A, c_a, (const TIn *)W, K, c_n, nbr, n_rows, (TOut *)out, e);
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
@@ -475,12 +510,12 @@ static int launch_gg(const void *A, uint32_t c_a, const void *W, uint32_t K, uin
 int conv_forward_simt(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
                       const void *weight, uint32_t K, uint32_t c_out, bool trans_w,
                       const int32_t *nbr, uint32_t n_out, void *out, int out_dtype,
-                      cudaStream_t stream) {
+                      const meb200_conv_epilogue *epi, cudaStream_t stream) {
   (void)n_in;
   if (n_out == 0) return MEB200_OK;
   MEB_DISPATCH_DTYPE_OUT(in_dtype, out_dtype,
                          return launch_gg<T, TO>(in, c_in, weight, K, c_out, trans_w, nbr, n_out,
-                                                 out, stream));
+                                                 out, epi, stream));
 }
 
 // Row splits k_conv_wgrad plans: enough CTAs for ~4 waves, each split at least 8 * TK rows.

@@ -5,10 +5,11 @@
 
 namespace meb200 {
 
+// epi (may be NULL; forward only, trans_w = false): the epilogue of meb200_conv_epilogue.
 int conv_forward_simt(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
                       const void *weight, uint32_t K, uint32_t c_out, bool trans_w,
                       const int32_t *nbr, uint32_t n_out, void *out, int out_dtype,
-                      cudaStream_t stream);
+                      const meb200_conv_epilogue *epi, cudaStream_t stream);
 
 // Weight gradients reduce over row splits (workspace_splits / launch_split_sum in common.cuh).
 // The size below fits every split the plan wants, for the kernel conv_small_cin_supported()
@@ -24,7 +25,7 @@ int conv_wgrad_simt(const void *in, const void *grad_out, int dtype, uint32_t c_
 bool conv_small_cin_supported(uint32_t c_in, uint32_t c_out);
 int conv_small_cin_forward(const void *in, int in_dtype, uint32_t c_in, const void *W, uint32_t K,
                            uint32_t c_out, const int32_t *nbr, uint32_t n_out, void *out,
-                           int out_dtype, cudaStream_t stream);
+                           int out_dtype, const meb200_conv_epilogue *epi, cudaStream_t stream);
 int conv_small_cin_wgrad(const void *in, const void *grad_out, int dtype, uint32_t c_in, uint32_t K,
                          uint32_t c_out, const int32_t *out_nbr, uint32_t n_out, float *grad_weight,
                          void *workspace, uint64_t workspace_bytes, cudaStream_t stream);

@@ -50,6 +50,8 @@ constexpr bool kIsTf32 = std::is_same<T, float>::value;   // fp32 storage, tf32 
 
 template <typename T>
 __device__ __forceinline__ uint32_t pack2(float a, float b);
+template <typename T>
+__device__ __forceinline__ float2 unpack2(uint32_t u);
 template <>
 __device__ __forceinline__ uint32_t pack2<__nv_bfloat16>(float a, float b) {
   __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
@@ -59,6 +61,15 @@ template <>
 __device__ __forceinline__ uint32_t pack2<__half>(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<uint32_t *>(&h);
+}
+
+template <>
+__device__ __forceinline__ float2 unpack2<__nv_bfloat16>(uint32_t u) {
+  return __bfloat1622float2(*reinterpret_cast<__nv_bfloat162 *>(&u));
+}
+template <>
+__device__ __forceinline__ float2 unpack2<__half>(uint32_t u) {
+  return __half22float2(*reinterpret_cast<__half2 *>(&u));
 }
 
 __device__ __forceinline__ uint8_t *align1k(uint8_t *p) {
@@ -83,11 +94,17 @@ struct FwdParams {
   // tile t runs the offsets of tile_mask[t] and writes slot s to row slot_row[s]
   const int32_t *slot_row;
   const uint32_t *tile_mask;
+  // epilogue of the EPI kernels (meb200_conv_epilogue): scale / shift at this launch's column 0,
+  // res (may be NULL) laid out as out
+  const float *scale, *shift;
+  const void *res;
+  uint32_t relu;
 };
 
 // NT wgmma instructions of N = NI columns each cover the c_cols = NI * NT columns of the slice.
-// grid = (128-row tiles, column slices).
-template <typename T, int NI, int NT>
+// grid = (128-row tiles, column slices).  EPI: apply the epilogue of p before the conversion (a
+// template parameter, so that the plain forward and the dgrad compile as if it did not exist).
+template <typename T, int NI, int NT, bool EPI>
 __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t s0 = smem_u32(align1k(smem_raw));
@@ -187,7 +204,28 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
 #pragma unroll
       for (int j = 0; j < NI / 8; ++j) {
         const uint32_t col = col0 + i * NI + 8 * j + 2 * t;
-        const float v0 = acc[i][4 * j + 2 * h], v1 = acc[i][4 * j + 2 * h + 1];
+        float v0 = acc[i][4 * j + 2 * h], v1 = acc[i][4 * j + 2 * h + 1];
+        if constexpr (EPI) {
+          // plain loads, ordered after the previous pair's store: the compiler then cannot hoist
+          // the loads of the whole tile ahead of the stores (which spills the widest tiles)
+          const float2 sc = *reinterpret_cast<const float2 *>(p.scale + col);
+          const float2 sh = *reinterpret_cast<const float2 *>(p.shift + col);
+          v0 = fmaf(v0, sc.x, sh.x);
+          v1 = fmaf(v1, sc.y, sh.y);
+          if (p.res != nullptr) {
+            const size_t e2 = ((size_t)orow * p.out_ld + col) / 2;     // the pair's index
+            float2 rv;
+            if (kIsTf32<T> || p.out_f32) rv = reinterpret_cast<const float2 *>(p.res)[e2];
+            else if constexpr (!kIsTf32<T>)
+              rv = unpack2<T>(reinterpret_cast<const uint32_t *>(p.res)[e2]);
+            v0 += rv.x;
+            v1 += rv.y;
+          }
+          if (p.relu) {
+            v0 = fmaxf(v0, 0.f);
+            v1 = fmaxf(v1, 0.f);
+          }
+        }
         if (kIsTf32<T> || p.out_f32)
           *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + (size_t)orow * p.out_ld + col) =
               make_float2(v0, v1);
@@ -694,9 +732,9 @@ static int ensure_big_smem(const void *fn) {
     case 16: return L(64, 4);  default: break;                                          \
   }
 
-template <typename T, int NI, int NT>
+template <typename T, int NI, int NT, bool EPI>
 static int launch_fwd(const FwdParams &p, uint32_t slices, cudaStream_t stream) {
-  auto kern = k_conv_wg<T, NI, NT>;
+  auto kern = k_conv_wg<T, NI, NT, EPI>;
   MEB_BIG_SMEM(kern);
   const dim3 grid(cdiv(p.n_rows, tc::kFwdRows), slices);
   kern<<<grid, kThreads, tc::fwd_ring_bytes(p.bk * sizeof(T), p.c_cols), stream>>>(p);
@@ -704,9 +742,9 @@ static int launch_fwd(const FwdParams &p, uint32_t slices, cudaStream_t stream) 
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
-template <typename T>
+template <typename T, bool EPI>
 static int dispatch_fwd(const FwdParams &p, uint32_t slices, cudaStream_t stream) {
-#define MEB_L(NI, NT) launch_fwd<T, NI, NT>(p, slices, stream)
+#define MEB_L(NI, NT) launch_fwd<T, NI, NT, EPI>(p, slices, stream)
   MEB_COLS_DISPATCH(p.c_cols, MEB_L)
 #undef MEB_L
   set_error("conv tc: %u output columns per launch", p.c_cols);
@@ -717,9 +755,24 @@ static int run_fwd(int dtype, FwdParams p, cudaStream_t stream) {
   const uint32_t cols = p.c_cols;
   p.c_cols = tc::fwd_col_slice(p.n_rows, cols, (uint32_t)num_sms());
   const uint32_t slices = cols / p.c_cols;
-  if (dtype == MEB200_TF32) return dispatch_fwd<float>(p, slices, stream);
-  return dtype == MEB200_BF16 ? dispatch_fwd<__nv_bfloat16>(p, slices, stream)
-                              : dispatch_fwd<__half>(p, slices, stream);
+  if (p.scale != nullptr) {
+    if (dtype == MEB200_TF32) return dispatch_fwd<float, true>(p, slices, stream);
+    return dtype == MEB200_BF16 ? dispatch_fwd<__nv_bfloat16, true>(p, slices, stream)
+                                : dispatch_fwd<__half, true>(p, slices, stream);
+  }
+  if (dtype == MEB200_TF32) return dispatch_fwd<float, false>(p, slices, stream);
+  return dtype == MEB200_BF16 ? dispatch_fwd<__nv_bfloat16, false>(p, slices, stream)
+                              : dispatch_fwd<__half, false>(p, slices, stream);
+}
+
+// the epilogue's pointers at output column n0 (out_esz: bytes of an output element)
+static void set_epilogue(FwdParams &p, const meb200_conv_epilogue *epi, uint32_t n0, size_t out_esz) {
+  if (epi == nullptr) return;
+  p.scale = epi->scale + n0;
+  p.shift = epi->shift + n0;
+  p.res = epi->residual != nullptr ? reinterpret_cast<const uint8_t *>(epi->residual) + n0 * out_esz
+                                   : nullptr;
+  p.relu = epi->relu != 0;
 }
 
 template <typename T, int NI, int NT>
@@ -808,7 +861,8 @@ static_assert(tc::kFwdRows == kOrderTileRows, "a tile order's tiles are the kern
 
 int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *B,
                     uint32_t K, uint32_t c_cols, const int32_t *nbr, const int32_t *order,
-                    uint32_t n_rows, void *out, int out_dtype, cudaStream_t stream) {
+                    uint32_t n_rows, void *out, int out_dtype, const meb200_conv_epilogue *epi,
+                    cudaStream_t stream) {
   if (n_rows == 0) return MEB200_OK;
   MEB_CHECK_ARG(conv_tc_supported(dtype, c_reduce, c_cols), "shape not supported by tc path");
   if (!aligned(16, A, B)) {
@@ -831,6 +885,7 @@ int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, c
     p.c_red = c_reduce; p.c_cols = c_cols - n0 < tc::kMaxCols ? c_cols - n0 : tc::kMaxCols;
     p.K = K; p.n_rows = n_rows; p.n_a = n_a; p.out_ld = c_cols;
     p.bk = tc::fwd_stage_bytes(c_reduce, esz) / esz; p.out_f32 = out_dtype == MEB200_F32;
+    set_epilogue(p, epi, n0, out_esz);
     const int rc = run_fwd(dtype, p, stream);
     if (rc != MEB200_OK) return rc;
   }
@@ -847,7 +902,7 @@ bool conv_stem_tc_supported(int dtype, uint32_t K, uint32_t c_cols) {
 
 int conv_stem_forward_tc(const void *A4, int dtype, uint32_t K, const void *Wv, uint32_t c_cols,
                          const int32_t *nbr, uint32_t n_rows, void *out, int out_dtype,
-                         cudaStream_t stream) {
+                         const meb200_conv_epilogue *epi, cudaStream_t stream) {
   if (n_rows == 0) return MEB200_OK;
   MEB_CHECK_ARG(conv_stem_tc_supported(dtype, K, c_cols), "stem forward: K=%u c_out=%u", K, c_cols);
   if (!aligned(8, A4) || !aligned(16, Wv)) {
@@ -859,6 +914,7 @@ int conv_stem_forward_tc(const void *A4, int dtype, uint32_t K, const void *Wv, 
   p.c_red = stem_virtual(K); p.c_cols = c_cols; p.K = 1; p.n_rows = n_rows; p.n_a = kNoLimit;
   p.out_ld = c_cols; p.bk = tc::fwd_bk(p.c_red); p.out_f32 = out_dtype == MEB200_F32;
   p.stem_K = K;
+  set_epilogue(p, epi, 0, out_dtype == MEB200_F32 ? 4 : 2);
   return run_fwd(dtype, p, stream);
 }
 

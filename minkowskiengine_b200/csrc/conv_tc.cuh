@@ -12,10 +12,12 @@ bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out);
 // out[r,:] = sum_k A[nbr[k][r],:] @ B[k]^T with B [K, c_cols, c_reduce] (reduction contiguous):
 // the forward passes w_t [K, c_out, c_in], the dgrad the layer's w_cast [K, c_in, c_out].
 // order (may be NULL; read when K <= 32): the tile order of nbr from meb200_kernel_map, so that
-// each 128-row tile runs only the offsets its rows reach.
+// each 128-row tile runs only the offsets its rows reach.  epi (may be NULL): the forward's
+// epilogue (meb200_conv_epilogue); the dgrad passes NULL.
 int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *B,
                     uint32_t K, uint32_t c_cols, const int32_t *nbr, const int32_t *order,
-                    uint32_t n_rows, void *out, int out_dtype, cudaStream_t stream);
+                    uint32_t n_rows, void *out, int out_dtype, const meb200_conv_epilogue *epi,
+                    cudaStream_t stream);
 
 // fp32 W[K,c_in,c_out] -> w_cast [K,c_in,c_out] and w_t [K,c_out,c_in] in bf16/fp16, or in fp32
 // words rounded to tf32 (MEB200_TF32).
@@ -55,7 +57,7 @@ int conv_wgrad_pairs(const void *in, const void *grad_out, int dtype, uint32_t c
 bool conv_stem_tc_supported(int dtype, uint32_t K, uint32_t c_cols);
 int conv_stem_forward_tc(const void *A4, int dtype, uint32_t K, const void *Wv, uint32_t c_cols,
                          const int32_t *nbr, uint32_t n_rows, void *out, int out_dtype,
-                         cudaStream_t stream);
+                         const meb200_conv_epilogue *epi, cudaStream_t stream);
 bool conv_stem_wgrad_tc_supported(int dtype, uint32_t K, uint32_t c_out);
 int conv_stem_wgrad_tc(const void *in4, const void *grad_out, int dtype, uint32_t K,
                        uint32_t c_out, const int32_t *nbr, uint32_t n_rows, float *dWv,

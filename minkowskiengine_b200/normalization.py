@@ -274,6 +274,11 @@ def fused_bn_relu(norm, input, residual=None):
     """relu(norm(input) [+ residual]) in one pass over the features — the tail of a residual
     block (reference: MinkowskiEngine/modules/resnet_block.py:52-68 runs norm, `+=` and ReLU as
     three passes).  `norm` is a MinkowskiBatchNorm / MinkowskiSyncBatchNorm module."""
+    return _bn_tail(norm, input, residual, relu=True)
+
+
+def _bn_tail(norm, input, residual, relu):
+    """relu?(norm(input) [+ residual]) in one pass over the features (fused_bn_relu)."""
     bn = norm.bn
     group = norm._group() if isinstance(norm, MinkowskiSyncBatchNorm) else None
     res = None
@@ -281,9 +286,23 @@ def fused_bn_relu(norm, input, residual=None):
         assert residual.coordinate_map_key == input.coordinate_map_key, \
             "residual and input must live on the same coordinate map"
         res = residual.F
-    out = _batch_norm(bn, input.F, group, relu=True, residual=res)
+    out = _batch_norm(bn, input.F, group, relu=relu, residual=res)
     return SparseTensor(out, coordinate_map_key=input.coordinate_map_key,
                         coordinate_manager=input.coordinate_manager)
+
+
+def _eval_scale_shift(bn, conv_bias=None):
+    """fp32 [C] (scale, shift) of eval-mode batch norm as one affine map, y = x * scale + shift,
+    by the formula the eval apply pass uses: invstd = rsqrt(running_var + eps), scale = invstd * w,
+    shift = b - running_mean * scale (w = 1, b = 0 without affine parameters).  A bias added
+    before the norm (a convolution's, [1, C] or [C]) folds in as shift += conv_bias * scale."""
+    invstd = torch.rsqrt(bn.running_var.detach().float() + bn.eps)
+    scale = invstd if bn.weight is None else invstd * _f32(bn.weight)
+    mean = bn.running_mean.detach().float()
+    shift = -(mean * scale) if bn.bias is None else _f32(bn.bias) - mean * scale
+    if conv_bias is not None:
+        shift = shift + conv_bias.detach().float().reshape(-1) * scale
+    return scale.contiguous(), shift.contiguous()
 
 
 class MinkowskiBatchNorm(nn.Module):
