@@ -243,6 +243,49 @@ int meb200_conv_wgrad_uses_pairs(int dtype, uint32_t c_in, uint32_t c_out, uint3
 uint64_t meb200_conv_workspace_bytes(uint32_t n_out, uint32_t c_in, uint32_t c_out, uint32_t K,
                                      int dtype);
 
+/* ---- fp8 (e4m3) inference forward ----------------------------------------------------------
+ * The eval forward of a convolution on the Hopper fp8 tensor cores: the features are quantised to
+ * e4m3 with one scale per tensor, the weights with one scale per output channel, the products are
+ * summed by the tensor cores and dequantised in the epilogue:
+ *   out[o, c] = relu?(fma(acc[o, c] * a_scale, epi->scale[c], epi->shift[c]) [+ residual[o, c]])
+ * with acc the sum of e4m3 products, rounded once to out_dtype (F32, BF16 or F16, the layer's
+ * feature dtype).  epi->scale must include the weight scale: w_scale[c] times any per-channel
+ * factor (eval batch norm).  Accumulation: the products of e4m3 values are exact, but the e4m3
+ * tensor cores do not add them in fp32.  Modelled as keeping 13 fraction bits at each of the
+ * n = K * c_in / 32 k-steps of 32 channels, an output errs by at most n * 2^-13 * A (A the same sum
+ * over |products|); the worst measured on an H100 is about 2^-11.7 * A at K = 27, c_in = 384,
+ * where the bf16 / fp16 kernels stay within 4 * 2^-20 * A.  Quantisation, for amax = max |x| over the
+ * finite values of the tensor (of the column of W):
+ *   scale = amax / 448,  inv = 448 / amax                (IEEE divisions rounded to nearest;
+ *                                                         both 1 when amax = 0; inv = FLT_MAX and
+ *                                                         scale = 1 / FLT_MAX when 448 / amax
+ *                                                         overflows)
+ *   q     = cvt.rn.satfinite.e4m3(x * inv)               (the product rounded to nearest in fp32;
+ *                                                         +-inf -> +-448, NaN -> NaN)
+ * Deterministic, no host synchronisation. */
+/* 1 when meb200_conv_forward_fp8 takes the shape: c_in a multiple of 32 (whole 32-byte k-steps),
+ * c_out a multiple of 16 in [16, 1024]; else 0. */
+int meb200_conv_fp8_supported(uint32_t c_in, uint32_t c_out);
+/* in_e4m3 [n_in, c_in] and a_scale (DEVICE fp32, the dequantisation factor) from
+ * meb200_quantize_e4m3; w_t_e4m3 [K, c_out, c_in] from meb200_conv_pack_weights_e4m3; epi required;
+ * out_nbr / out_order as in meb200_conv_forward. */
+int meb200_conv_forward_fp8(const void *in_e4m3, const float *a_scale, uint32_t n_in, uint32_t c_in,
+                            const void *w_t_e4m3, uint32_t K, uint32_t c_out,
+                            const int32_t *out_nbr, uint32_t n_out, void *out, int out_dtype,
+                            const int32_t *out_order, const meb200_conv_epilogue *epi, void *stream);
+/* fp32 weight [K, c_in, c_out] -> w_t_e4m3 [K, c_out, c_in] and w_scale fp32 [c_out], with amax
+ * taken per output channel over (k, c_in). */
+int meb200_conv_pack_weights_e4m3(const float *weight, uint32_t K, uint32_t c_in, uint32_t c_out,
+                                  void *w_t_e4m3, float *w_scale, void *stream);
+/* Features [n, c] in `dtype` (F32 / BF16 / F16) -> out_e4m3 [n, c] and scale_dev (DEVICE fp32 [2]:
+ * scale, then inv) in two launches: the amax (its last CTA writes the scales) and the conversion,
+ * 16 output bytes per access when both buffers are 16-byte aligned.  workspace:
+ * meb200_quantize_e4m3_workspace_bytes() bytes, zero-filled once by the caller and shared by the
+ * calls on one stream; every call leaves it zero. */
+uint64_t meb200_quantize_e4m3_workspace_bytes(void);
+int meb200_quantize_e4m3(const void *in, int dtype, uint32_t n, uint32_t c, void *out_e4m3,
+                         float *scale_dev, void *workspace, void *stream);
+
 /* Weight packing, once per optimizer step instead of once per call: fp32 master weight
  * [K, Cin, Cout] -> `dtype` (BF16/F16, or TF32: fp32 words rounded to tf32) operand copies
  * w_cast [K, Cin, Cout] and w_t [K, Cout, Cin].  The reference keeps weights in the feature dtype and needs no such step

@@ -49,6 +49,12 @@ PROTOTYPES = {
                                     _u32, _vp, _i32, _vp, _vp, _vp, _vp, _u32, _vp, _u64, _vp,
                                     _vp]),
     "meb200_conv_wgrad_uses_pairs": (_i32, [_i32, _u32, _u32, _u32]),
+    "meb200_conv_fp8_supported": (_i32, [_u32, _u32]),
+    "meb200_conv_forward_fp8": (_i32, [_vp, _vp, _u32, _u32, _vp, _u32, _u32, _vp, _u32, _vp, _i32,
+                                       _vp, _vp, _vp]),
+    "meb200_conv_pack_weights_e4m3": (_i32, [_vp, _u32, _u32, _u32, _vp, _vp, _vp]),
+    "meb200_quantize_e4m3_workspace_bytes": (_u64, []),
+    "meb200_quantize_e4m3": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _vp, _vp]),
     "meb200_conv_pack_weights": (_i32, [_vp, _u32, _u32, _u32, _i32, _vp, _vp, _vp]),
     "meb200_conv_pack_weights_batched": (_i32, [_vp, _u32, _u32, _i32, _vp]),
     "meb200_conv_stem_virtual_channels": (_u32, [_u32]),

@@ -129,6 +129,13 @@ class MinkowskiConvolutionBase(MinkowskiModuleBase):
         else:
             out_coordinate_map_key = _get_coordinate_map_key(
                 input, coordinates, expand_coordinates=self.kernel_generator.expand_coordinates)
+            if _fp8(self, input.F):
+                # the bias is the epilogue's shift: one rounding of the biased output
+                shift = None if self.bias is None else self.bias.detach().float().reshape(-1)
+                outfeat = _forward_with(self, input, out_coordinate_map_key,
+                                        (None, shift, None, False), fp8=True)
+                return SparseTensor(outfeat, coordinate_map_key=out_coordinate_map_key,
+                                    coordinate_manager=input._manager)
             outfeat = self.conv.apply(input.F, self.kernel, self.kernel_generator,
                                       self.convolution_mode, input.coordinate_map_key,
                                       out_coordinate_map_key, input._manager)
@@ -227,6 +234,29 @@ def _fuses(conv, norm, feats, res):
     return _native_ok(bn, feats.new_empty((0, conv.out_channels)))
 
 
+def _fp8(conv, feats):
+    """Whether `conv` runs its forward on e4m3 operands (backend.fp8_inference): inside the
+    context, for a layer that needs no gradient (feats, kernel or bias requiring one with grad mode
+    on; fused_conv_bn_relu checks the norm and the residual in _fuses), is not a plain matrix product (kernel volume 1, stride 1), has fp32 / bf16 /
+    fp16 features and c_in -> c_out on the e4m3 grid (which leaves out the stem, c_in <= 4)."""
+    if not _C.fp8_enabled() or conv.use_mm or feats.dtype not in _C._FP8_DTYPES:
+        return False
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (
+            feats, conv.kernel, conv.bias)):
+        return False
+    return _C.fp8_supported(conv.in_channels, conv.out_channels)
+
+
+def _forward_with(conv, input, out_key, epilogue, fp8=False):
+    """conv's native forward onto `out_key` with `epilogue` (no autograd)."""
+    kg = conv.kernel_generator
+    forward = _C.ConvolutionTransposeForwardGPU if conv.is_transpose else _C.ConvolutionForwardGPU
+    return forward(input.F.contiguous(), conv.kernel, kg.kernel_size, kg.kernel_stride,
+                   kg.kernel_dilation, kg.region_type, kg.region_offsets, kg.expand_coordinates,
+                   conv.convolution_mode, input.coordinate_map_key, out_key,
+                   input._manager._manager, epilogue=epilogue, fp8=fp8)
+
+
 def _output_key(conv, input):
     """The key of conv(input)'s output map, made as the forward makes it."""
     kg = conv.kernel_generator
@@ -272,11 +302,8 @@ def fused_conv_bn_relu(conv, norm, input, residual=None, relu=True):
             return norm(out)
         return _bn_tail(norm, out, residual, relu)
     assert input.D == conv.dimension
-    kg = conv.kernel_generator
     scale, shift = _eval_scale_shift(norm.bn, conv.bias)
-    forward = _C.ConvolutionTransposeForwardGPU if conv.is_transpose else _C.ConvolutionForwardGPU
-    feats = forward(input.F.contiguous(), conv.kernel, kg.kernel_size, kg.kernel_stride,
-                    kg.kernel_dilation, kg.region_type, kg.region_offsets, kg.expand_coordinates,
-                    conv.convolution_mode, input.coordinate_map_key, out_key, input._manager._manager,
-                    epilogue=(scale, shift, None if res is None else res.contiguous(), relu))
+    feats = _forward_with(conv, input, out_key,
+                          (scale, shift, None if res is None else res.contiguous(), relu),
+                          fp8=_fp8(conv, input.F))
     return SparseTensor(feats, coordinate_map_key=out_key, coordinate_manager=input._manager)

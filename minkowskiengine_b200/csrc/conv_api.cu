@@ -61,6 +61,46 @@ int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_
                            out_nbr, n_out, out, out_dtype, epi, stream);
 }
 
+int meb200_conv_fp8_supported(uint32_t c_in, uint32_t c_out) {
+  return conv_fp8_supported(c_in, c_out) ? 1 : 0;
+}
+
+int meb200_conv_forward_fp8(const void *in_e4m3, const float *a_scale, uint32_t n_in, uint32_t c_in,
+                            const void *w_t_e4m3, uint32_t K, uint32_t c_out,
+                            const int32_t *out_nbr, uint32_t n_out, void *out, int out_dtype,
+                            const int32_t *out_order, const meb200_conv_epilogue *epi,
+                            void *stream_) {
+  if (n_out == 0) return MEB200_OK;
+  MEB_CHECK_ARG(out_dtype >= 0 && out_dtype <= 2, "output dtype");
+  MEB_CHECK_ARG(out && w_t_e4m3 && a_scale && out_nbr && (in_e4m3 || n_in == 0), "null buffer");
+  MEB_CHECK_ARG(K > 0, "empty kernel");
+  MEB_CHECK_ARG(epi != nullptr && epilogue_ok(epi),
+                "epilogue required: scale and shift, 8-byte aligned pointers");
+  if (!conv_fp8_supported(c_in, c_out)) {
+    set_error("fp8 forward: c_in=%u c_out=%u outside the e4m3 grid", c_in, c_out);
+    return MEB200_ERR_UNSUPPORTED;
+  }
+  return conv_forward_tc(in_e4m3, kOperandE4M3, n_in, c_in, w_t_e4m3, K, c_out, out_nbr, out_order,
+                         n_out, out, out_dtype, epi, (cudaStream_t)stream_, a_scale);
+}
+
+int meb200_conv_pack_weights_e4m3(const float *weight, uint32_t K, uint32_t c_in, uint32_t c_out,
+                                  void *w_t_e4m3, float *w_scale, void *stream_) {
+  MEB_CHECK_ARG(weight && w_t_e4m3 && w_scale, "null buffer");
+  MEB_CHECK_ARG(c_in > 0 && c_out > 0 && K > 0, "empty channel/kernel dims");
+  return conv_pack_weights_e4m3(weight, K, c_in, c_out, w_t_e4m3, w_scale, (cudaStream_t)stream_);
+}
+
+uint64_t meb200_quantize_e4m3_workspace_bytes(void) { return quantize_e4m3_workspace_bytes(); }
+
+int meb200_quantize_e4m3(const void *in, int dtype, uint32_t n, uint32_t c, void *out_e4m3,
+                         float *scale_dev, void *workspace, void *stream_) {
+  MEB_CHECK_ARG(dtype >= 0 && dtype <= 2, "dtype");
+  MEB_CHECK_ARG(out_e4m3 && scale_dev && workspace && (in || (uint64_t)n * c == 0), "null buffer");
+  return quantize_e4m3(in, dtype, (uint64_t)n * c, out_e4m3, scale_dev, workspace,
+                       (cudaStream_t)stream_);
+}
+
 static bool packed_dtype(int dtype) {
   return dtype == MEB200_BF16 || dtype == MEB200_F16 || dtype == MEB200_TF32;
 }

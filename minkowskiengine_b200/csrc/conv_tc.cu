@@ -6,7 +6,8 @@
 //
 // Operands are bf16 / fp16, or fp32 words multiplied in TF32 (MEB200_TF32: k_conv_wg<float, ..>
 // for forward / dgrad, k_wgrad_tf32 for the weight gradient, whose MN-major operands tf32 wgmma
-// cannot read).
+// cannot read).  The eval forward also runs on e4m3 bytes (meb200_conv_forward_fp8:
+// k_conv_wg<__nv_fp8_e4m3, ..>, 32 channels per k-step, always with its epilogue).
 //
 // Replaces the reference's per-offset SIMT tile-matmul with per-element atomicAdd
 // (src/convolution_kernel.cu:114-180,320-496): forward and dgrad write every output row exactly
@@ -22,9 +23,12 @@
 // CTA = 2 warpgroups (256 threads).  A ring of tc::kStages stages; every thread issues the copies
 // of stage s + 2 before the MMAs of stage s, one __syncthreads per stage, and each warpgroup keeps
 // one wgmma group in flight behind the barrier.
+#include <stddef.h>
 #include <stdlib.h>
 #include <string.h>
 #include <type_traits>
+
+#include <cuda_fp8.h>
 
 #include "conv_tc.cuh"
 #include "ptx.cuh"
@@ -47,6 +51,8 @@ template <typename T>
 constexpr bool kIsBf16 = std::is_same<T, __nv_bfloat16>::value;
 template <typename T>
 constexpr bool kIsTf32 = std::is_same<T, float>::value;   // fp32 storage, tf32 MMAs
+template <typename T>
+constexpr bool kIsFp8 = std::is_same<T, __nv_fp8_e4m3>::value;   // e4m3 operands (inference)
 
 template <typename T>
 __device__ __forceinline__ uint32_t pack2(float a, float b);
@@ -89,7 +95,12 @@ struct FwdParams {
   uint32_t c_cols;        // columns of one CTA: column slice blockIdx.y starts at blockIdx.y * c_cols
   uint32_t n_a;           // rows of A (gather indices >= n_a read as zero rows)
   uint32_t out_ld, bk, out_f32;
-  uint32_t stem_K;        // > 0: network stem, virtual channel 4 k + c = A[nbr[k][r]][c], k < stem_K
+  union {
+    uint32_t stem_K;      // > 0: network stem, virtual channel 4 k + c = A[nbr[k][r]][c], k < stem_K
+    // e4m3 kernels (which have no stem mode): device fp32, the activation scale.  It shares the
+    // 8-byte slot of stem_K and its padding, so the parameter block keeps its layout.
+    const float *a_scale;
+  };
   // tile order (meb200_kernel_map, K <= 32), or both NULL: nbr is then the table in slot order,
   // tile t runs the offsets of tile_mask[t] and writes slot s to row slot_row[s]
   const int32_t *slot_row;
@@ -100,11 +111,14 @@ struct FwdParams {
   const void *res;
   uint32_t relu;
 };
+static_assert(sizeof(FwdParams) == 128 && offsetof(FwdParams, slot_row) == 80, "FwdParams layout");
 
 // NT wgmma instructions of N = NI columns each cover the c_cols = NI * NT columns of the slice.
 // grid = (128-row tiles, column slices).  EPI: apply the epilogue of p before the conversion (a
 // template parameter, so that the plain forward and the dgrad compile as if it did not exist).
-template <typename T, int NI, int NT, bool EPI>
+// TO: the 16-bit output type (out_f32: fp32), T itself except for e4m3 operands, whose kernels
+// always run the epilogue with the accumulator times *p.a_scale.
+template <typename T, int NI, int NT, bool EPI, typename TO = T>
 __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t s0 = smem_u32(align1k(smem_raw));
@@ -133,7 +147,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
       if (ordered) { ld_rem &= ld_rem - 1; ld_k = __ffs(ld_rem) - 1; } else ++ld_k;
     }
     const uint32_t base = s0 + (s % kStages) * stage_bytes;
-    if (kIsTf32<T> || p.stem_K == 0) {
+    if (kIsTf32<T> || kIsFp8<T> || p.stem_K == 0) {
       const int32_t src = row_ok ? __ldg(p.nbr + (size_t)k * p.n_rows + arow) : -1;
       const bool ok = src >= 0 && (uint32_t)src < p.n_a;
       const T *rp = A + (size_t)(ok ? src : 0) * p.c_red + c0;
@@ -184,6 +198,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
       for (int i = 0; i < NT; ++i) {
         const uint64_t db = wgmma_desc(b0 + i * NI * width + kk * 256, 128, sbo);
         if constexpr (kIsTf32<T>) wgmma_tf32<NI, 0, 0>(acc[i], da, db);
+        else if constexpr (kIsFp8<T>) wgmma_e4m3<NI>(acc[i], da, db);
         else wgmma<NI, kIsBf16<T>, 0, 0>(acc[i], da, db);
       }
     }
@@ -191,6 +206,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
     wgmma_wait<1>();
   }
   wgmma_wait<0>();
+  float a_s = 1.f;
+  if constexpr (kIsFp8<T>) a_s = __ldg(p.a_scale);
 
   const uint32_t g = lane >> 2, t = lane & 3;
   const uint32_t rbase = row0 + wg * 64 + (warp & 3) * 16 + g;
@@ -205,6 +222,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
       for (int j = 0; j < NI / 8; ++j) {
         const uint32_t col = col0 + i * NI + 8 * j + 2 * t;
         float v0 = acc[i][4 * j + 2 * h], v1 = acc[i][4 * j + 2 * h + 1];
+        if constexpr (kIsFp8<T>) {
+          v0 *= a_s;
+          v1 *= a_s;
+        }
         if constexpr (EPI) {
           // plain loads, ordered after the previous pair's store: the compiler then cannot hoist
           // the loads of the whole tile ahead of the stores (which spills the widest tiles)
@@ -217,7 +238,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
             float2 rv;
             if (kIsTf32<T> || p.out_f32) rv = reinterpret_cast<const float2 *>(p.res)[e2];
             else if constexpr (!kIsTf32<T>)
-              rv = unpack2<T>(reinterpret_cast<const uint32_t *>(p.res)[e2]);
+              rv = unpack2<TO>(reinterpret_cast<const uint32_t *>(p.res)[e2]);
             v0 += rv.x;
             v1 += rv.y;
           }
@@ -230,8 +251,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
           *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + (size_t)orow * p.out_ld + col) =
               make_float2(v0, v1);
         else if constexpr (!kIsTf32<T>)
-          *reinterpret_cast<uint32_t *>(reinterpret_cast<T *>(p.out) + (size_t)orow * p.out_ld + col) =
-              pack2<T>(v0, v1);
+          *reinterpret_cast<uint32_t *>(reinterpret_cast<TO *>(p.out) + (size_t)orow * p.out_ld + col) =
+              pack2<TO>(v0, v1);
       }
   }
 }
@@ -732,9 +753,9 @@ static int ensure_big_smem(const void *fn) {
     case 16: return L(64, 4);  default: break;                                          \
   }
 
-template <typename T, int NI, int NT, bool EPI>
+template <typename T, int NI, int NT, bool EPI, typename TO>
 static int launch_fwd(const FwdParams &p, uint32_t slices, cudaStream_t stream) {
-  auto kern = k_conv_wg<T, NI, NT, EPI>;
+  auto kern = k_conv_wg<T, NI, NT, EPI, TO>;
   MEB_BIG_SMEM(kern);
   const dim3 grid(cdiv(p.n_rows, tc::kFwdRows), slices);
   kern<<<grid, kThreads, tc::fwd_ring_bytes(p.bk * sizeof(T), p.c_cols), stream>>>(p);
@@ -742,19 +763,23 @@ static int launch_fwd(const FwdParams &p, uint32_t slices, cudaStream_t stream) 
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
-template <typename T, bool EPI>
+template <typename T, bool EPI, typename TO = T>
 static int dispatch_fwd(const FwdParams &p, uint32_t slices, cudaStream_t stream) {
-#define MEB_L(NI, NT) launch_fwd<T, NI, NT, EPI>(p, slices, stream)
+#define MEB_L(NI, NT) launch_fwd<T, NI, NT, EPI, TO>(p, slices, stream)
   MEB_COLS_DISPATCH(p.c_cols, MEB_L)
 #undef MEB_L
   set_error("conv tc: %u output columns per launch", p.c_cols);
   return MEB200_ERR_UNSUPPORTED;
 }
 // p.c_cols = all the launch's columns (<= 256): the launch runs them in the chooser's slices
-static int run_fwd(int dtype, FwdParams p, cudaStream_t stream) {
+static int run_fwd(int dtype, FwdParams p, cudaStream_t stream, int out_dtype = MEB200_F32) {
   const uint32_t cols = p.c_cols;
   p.c_cols = tc::fwd_col_slice(p.n_rows, cols, (uint32_t)num_sms());
   const uint32_t slices = cols / p.c_cols;
+  if (dtype == kOperandE4M3) {        // always with the epilogue; fp32 output through out_f32
+    return out_dtype == MEB200_F16 ? dispatch_fwd<__nv_fp8_e4m3, true, __half>(p, slices, stream)
+                                   : dispatch_fwd<__nv_fp8_e4m3, true, __nv_bfloat16>(p, slices, stream);
+  }
   if (p.scale != nullptr) {
     if (dtype == MEB200_TF32) return dispatch_fwd<float, true>(p, slices, stream);
     return dtype == MEB200_BF16 ? dispatch_fwd<__nv_bfloat16, true>(p, slices, stream)
@@ -849,7 +874,13 @@ static int run_wgrad(int dtype, WgParams p, uint32_t K_grid, uint32_t est_stages
 }
 
 // ---- forward / dgrad ----------------------------------------------------------------------------
-static uint32_t operand_bytes(int dtype) { return dtype == MEB200_TF32 ? 4 : 2; }
+static uint32_t operand_bytes(int dtype) {
+  return dtype == MEB200_TF32 ? 4 : (dtype == kOperandE4M3 ? 1 : 2);
+}
+
+bool conv_fp8_supported(uint32_t c_in, uint32_t c_out) {
+  return c_in >= 32 && c_in % 32 == 0 && c_out % 16 == 0 && c_out >= 16 && c_out <= 1024;
+}
 
 bool conv_tc_supported(int dtype, uint32_t c_reduce, uint32_t c_cols) {
   if (dtype != MEB200_BF16 && dtype != MEB200_F16 && dtype != MEB200_TF32) return false;
@@ -862,9 +893,12 @@ static_assert(tc::kFwdRows == kOrderTileRows, "a tile order's tiles are the kern
 int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *B,
                     uint32_t K, uint32_t c_cols, const int32_t *nbr, const int32_t *order,
                     uint32_t n_rows, void *out, int out_dtype, const meb200_conv_epilogue *epi,
-                    cudaStream_t stream) {
+                    cudaStream_t stream, const float *a_scale) {
   if (n_rows == 0) return MEB200_OK;
-  MEB_CHECK_ARG(conv_tc_supported(dtype, c_reduce, c_cols), "shape not supported by tc path");
+  const bool fp8 = dtype == kOperandE4M3;
+  MEB_CHECK_ARG(fp8 ? conv_fp8_supported(c_reduce, c_cols) && epi != nullptr && a_scale != nullptr
+                    : conv_tc_supported(dtype, c_reduce, c_cols),
+                "shape not supported by tc path");
   if (!aligned(16, A, B)) {
     set_error("conv tc: operands must be 16-byte aligned");
     return MEB200_ERR_UNSUPPORTED;
@@ -886,7 +920,8 @@ int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, c
     p.K = K; p.n_rows = n_rows; p.n_a = n_a; p.out_ld = c_cols;
     p.bk = tc::fwd_stage_bytes(c_reduce, esz) / esz; p.out_f32 = out_dtype == MEB200_F32;
     set_epilogue(p, epi, n0, out_esz);
-    const int rc = run_fwd(dtype, p, stream);
+    p.a_scale = a_scale;
+    const int rc = run_fwd(dtype, p, stream, out_dtype);
     if (rc != MEB200_OK) return rc;
   }
   return MEB200_OK;

@@ -7,6 +7,11 @@ namespace meb200 {
 
 // bf16/fp16/TF32 operands with channel counts the tiles cover.
 bool conv_tc_supported(int dtype, uint32_t c_reduce, uint32_t c_cols);
+
+// Operand code of the e4m3 forward (internal: not a feature dtype of the ABI).  Grid: whole 32-byte
+// k-steps of the reduction, output columns in multiples of 16.
+constexpr int kOperandE4M3 = 100;
+bool conv_fp8_supported(uint32_t c_in, uint32_t c_out);
 bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out);
 
 // out[r,:] = sum_k A[nbr[k][r],:] @ B[k]^T with B [K, c_cols, c_reduce] (reduction contiguous):
@@ -14,10 +19,22 @@ bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out);
 // order (may be NULL; read when K <= 32): the tile order of nbr from meb200_kernel_map, so that
 // each 128-row tile runs only the offsets its rows reach.  epi (may be NULL): the forward's
 // epilogue (meb200_conv_epilogue); the dgrad passes NULL.
+// dtype kOperandE4M3: A and B are e4m3 bytes, out_dtype bf16 / fp16 / fp32, and the epilogue
+// (required) runs on the accumulator times *a_scale (a device pointer).
 int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *B,
                     uint32_t K, uint32_t c_cols, const int32_t *nbr, const int32_t *order,
                     uint32_t n_rows, void *out, int out_dtype, const meb200_conv_epilogue *epi,
-                    cudaStream_t stream);
+                    cudaStream_t stream, const float *a_scale = nullptr);
+
+// fp32 W [K, c_in, c_out] -> w_t [K, c_out, c_in] in e4m3 with a scale per output channel:
+// w_scale[c] = amax_c / 448 (1 when amax_c = 0), w_t = satfinite_rn(W * (448 / amax_c)).
+int conv_pack_weights_e4m3(const float *W, uint32_t K, uint32_t c_in, uint32_t c_out, void *w_t,
+                           float *w_scale, cudaStream_t stream);
+
+// Per-tensor e4m3 quantisation of [n, c] features (meb200_quantize_e4m3).
+uint64_t quantize_e4m3_workspace_bytes();
+int quantize_e4m3(const void *in, int dtype, uint64_t count, void *out, float *scale, void *workspace,
+                  cudaStream_t stream);
 
 // fp32 W[K,c_in,c_out] -> w_cast [K,c_in,c_out] and w_t [K,c_out,c_in] in bf16/fp16, or in fp32
 // words rounded to tf32 (MEB200_TF32).

@@ -1,0 +1,186 @@
+// fp8 (e4m3) operands of the inference forward (meb200_conv_forward_fp8): per-tensor quantisation of
+// the features and per-output-channel quantisation of the weights.
+//
+// Both use the same arithmetic, so that a torch expression reproduces the bytes exactly:
+//   amax  = max |x| over the finite values (a max is exact and order-free: deterministic)
+//   scale = amax / 448, inv = 448 / amax                 (both IEEE divisions, rounded to nearest)
+//           scale = inv = 1 when amax = 0
+//           inv = FLT_MAX, scale = 1 / FLT_MAX when 448 / amax overflows (amax < 448 / FLT_MAX):
+//           scale stays the reciprocal of inv, so that q * scale still approximates x
+//   q     = cvt.rn.satfinite.e4m3(x * inv)                (the product rounded to nearest in fp32)
+// x * inv lies within rounding of [-448, 448] for a finite x, so the conversion rounds to nearest
+// even; +-inf saturates to +-448 and NaN stays NaN.  448 is the largest finite e4m3 value.
+#include <float.h>
+
+#include <algorithm>
+
+#include "common.cuh"
+#include "conv_tc.cuh"
+#include "ptx.cuh"
+
+namespace meb200 {
+
+constexpr float kE4M3Max = 448.f;
+constexpr uint32_t kQThreads = 256;
+constexpr uint32_t kQMaxCtas = 1024;
+
+// scale and inv of a tensor (or column) whose finite values have the maximum magnitude amax
+__device__ __forceinline__ void e4m3_scales(float amax, float &scale, float &inv) {
+  if (amax == 0.f) {
+    scale = inv = 1.f;
+  } else if (isinf(inv = __fdiv_rn(kE4M3Max, amax))) {
+    inv = FLT_MAX;
+    scale = __fdiv_rn(1.f, FLT_MAX);
+  } else {
+    scale = __fdiv_rn(amax, kE4M3Max);
+  }
+}
+
+__device__ __forceinline__ float finite_abs(float v) { return isfinite(v) ? fabsf(v) : 0.f; }
+
+__device__ __forceinline__ uint8_t e4m3_byte(float x, float inv) {
+  return (uint8_t)(ptx::e4m3x2_satfinite(__fmul_rn(x, inv), 0.f) & 0xFFu);
+}
+
+// Launch 1: per-CTA max of |x| over the finite values, combined with an atomic max on the fp32 bits
+// (non-negative floats order as their bit patterns).  The last CTA to finish writes scale[0] = scale,
+// scale[1] = inv and leaves the workspace zero again.  ws: [0] amax bits, [1] CTAs done (a ticket
+// that wraps to 0 at the last CTA).
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kQThreads) k_amax(const T *__restrict__ x, uint64_t count,
+                                                   float *__restrict__ scale, uint32_t *ws) {
+  constexpr uint32_t V = VEC ? 16 / sizeof(T) : 1;
+  float m = 0.f;
+  const uint64_t n_vec = count / V, stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_vec; i += stride) {
+    float f[V];
+    load_f32<T, V>(x + i * V, f);
+#pragma unroll
+    for (uint32_t j = 0; j < V; ++j) m = fmaxf(m, finite_abs(f[j]));
+  }
+  if (blockIdx.x == 0)                                    // elements past the last vector
+    for (uint64_t i = n_vec * V + threadIdx.x; i < count; i += blockDim.x)
+      m = fmaxf(m, finite_abs(to_f32<T>(x[i])));
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, d));
+  __shared__ float wm[kQThreads / 32];
+  if ((threadIdx.x & 31) == 0) wm[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  for (uint32_t w = 1; w < kQThreads / 32; ++w) m = fmaxf(m, wm[w]);
+  atomicMax(ws, __float_as_uint(m));
+  __threadfence();
+  if (atomicInc(ws + 1, gridDim.x - 1) != gridDim.x - 1) return;
+  const float amax = __uint_as_float(atomicExch(ws, 0u));  // every CTA's max has landed
+  float s, inv;
+  e4m3_scales(amax, s, inv);
+  scale[0] = s;
+  scale[1] = inv;
+}
+
+// Launch 2: q = e4m3(x * inv), 16 elements (16 output bytes) per thread and step.
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kQThreads) k_quant(const T *__restrict__ x, uint64_t count,
+                                                    const float *__restrict__ scale,
+                                                    uint8_t *__restrict__ q) {
+  const float inv = __ldg(scale + 1);
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  if constexpr (VEC) {
+    constexpr uint32_t V = 16 / sizeof(T);
+    const uint64_t n16 = count / 16;
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n16; i += stride) {
+      uint32_t w[4];
+#pragma unroll
+      for (uint32_t h = 0; h < 16 / V; ++h) {
+        float f[V];
+        load_f32<T, V>(x + i * 16 + h * V, f);
+#pragma unroll
+        for (uint32_t j = 0; j < V; j += 2) {
+          const uint32_t e = h * V + j;           // element of the 16: byte e of the store
+          const uint32_t b = ptx::e4m3x2_satfinite(__fmul_rn(f[j], inv), __fmul_rn(f[j + 1], inv));
+          if (e % 4 == 0) w[e / 4] = b; else w[e / 4] |= b << 16;
+        }
+      }
+      *reinterpret_cast<uint4 *>(q + i * 16) = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+    if (blockIdx.x == 0)
+      for (uint64_t i = n16 * 16 + threadIdx.x; i < count; i += blockDim.x)
+        q[i] = e4m3_byte(to_f32<T>(x[i]), inv);
+  } else {
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count; i += stride)
+      q[i] = e4m3_byte(to_f32<T>(x[i]), inv);
+  }
+}
+
+uint64_t quantize_e4m3_workspace_bytes() { return 16; }
+
+int quantize_e4m3(const void *in, int dtype, uint64_t count, void *out, float *scale,
+                  void *workspace, cudaStream_t stream) {
+  const bool vec = aligned(16, in, out);
+  const uint32_t ctas = (uint32_t)std::min<uint64_t>(
+      std::max<uint64_t>(cdiv(count, 16ull * kQThreads), 1), std::min<uint32_t>(kQMaxCtas, 4 * num_sms()));
+  uint32_t *ws = reinterpret_cast<uint32_t *>(workspace);
+  uint8_t *q = reinterpret_cast<uint8_t *>(out);
+  MEB_DISPATCH_DTYPE(dtype, {
+    const T *x = reinterpret_cast<const T *>(in);
+    if (vec) {
+      k_amax<T, true><<<ctas, kQThreads, 0, stream>>>(x, count, scale, ws);
+      MEB_LAUNCH_OK();
+      k_quant<T, true><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
+    } else {
+      k_amax<T, false><<<ctas, kQThreads, 0, stream>>>(x, count, scale, ws);
+      MEB_LAUNCH_OK();
+      k_quant<T, false><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
+    }
+    MEB_LAUNCH_OK();
+  });
+  return MEB200_OK;
+}
+
+// Weights: one CTA per 32 output channels.  Pass 1: the amax of each column over all K * c_in rows
+// (8 row phases per column, combined with fmaxf: order-free).  Pass 2: 32 x 32 tiles transposed
+// through shared memory into w_t [K, c_out, c_in], as k_pack_w does.
+__global__ void __launch_bounds__(256) k_pack_w_e4m3(const float *__restrict__ W, uint32_t K,
+                                                     uint32_t c_in, uint32_t c_out,
+                                                     uint8_t *__restrict__ Wt,
+                                                     float *__restrict__ w_scale) {
+  __shared__ float tile[32][33];
+  __shared__ float inv_s[32];
+  const uint32_t tx = threadIdx.x & 31, ty = threadIdx.x >> 5, co0 = blockIdx.x * 32;
+  const uint32_t co = co0 + tx;
+  const uint64_t rows = (uint64_t)K * c_in;
+  float m = 0.f;
+  if (co < c_out)
+    for (uint64_t r = ty; r < rows; r += 8) m = fmaxf(m, finite_abs(W[r * c_out + co]));
+  tile[ty][tx] = m;
+  __syncthreads();
+  if (ty == 0) {
+    for (uint32_t i = 1; i < 8; ++i) m = fmaxf(m, tile[i][tx]);
+    float s, inv;
+    e4m3_scales(m, s, inv);
+    inv_s[tx] = inv;
+    if (co < c_out) w_scale[co] = s;
+  }
+  __syncthreads();
+  for (uint32_t k = 0; k < K; ++k)
+    for (uint32_t ci0 = 0; ci0 < c_in; ci0 += 32) {
+      const size_t base = (size_t)k * c_in * c_out;
+      for (uint32_t i = ty; i < 32; i += 8)
+        if (ci0 + i < c_in && co < c_out) tile[i][tx] = W[base + (size_t)(ci0 + i) * c_out + co];
+      __syncthreads();
+      for (uint32_t i = ty; i < 32; i += 8)
+        if (co0 + i < c_out && ci0 + tx < c_in)
+          Wt[base + (size_t)(co0 + i) * c_in + ci0 + tx] = e4m3_byte(tile[tx][i], inv_s[i]);
+      __syncthreads();
+    }
+}
+
+int conv_pack_weights_e4m3(const float *W, uint32_t K, uint32_t c_in, uint32_t c_out, void *w_t,
+                           float *w_scale, cudaStream_t stream) {
+  k_pack_w_e4m3<<<cdiv(c_out, 32), 256, 0, stream>>>(W, K, c_in, c_out,
+                                                     reinterpret_cast<uint8_t *>(w_t), w_scale);
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
+}
+
+}  // namespace meb200
