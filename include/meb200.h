@@ -286,6 +286,48 @@ uint64_t meb200_quantize_e4m3_workspace_bytes(void);
 int meb200_quantize_e4m3(const void *in, int dtype, uint32_t n, uint32_t c, void *out_e4m3,
                          float *scale_dev, void *workspace, void *stream);
 
+/* ---- fp8 static scales and shadows -------------------------------------------------------------
+ * A calibrated layer quantises its input with a scale fixed in advance instead of its amax:
+ * the amax of calibration runs, turned into (scale, inv) by the formula above.  Values above the
+ * calibrated amax saturate to +-448 (satfinite).
+ * meb200_amax_accumulate: *amax_dev = max(*amax_dev, max |x| over the finite values of the [n, c]
+ *   features) in one launch (per-CTA max, then an atomic max on the fp32 bits).  *amax_dev starts
+ *   at 0 (or any earlier amax); calls accumulate, in any order, to the same bits.
+ * meb200_e4m3_scales: scale_dev[0] = scale, scale_dev[1] = inv of *amax_dev (one thread).
+ * meb200_quantize_e4m3_static: out_e4m3 = e4m3(x * scale_dev[1]), the conversion launch of
+ *   meb200_quantize_e4m3 alone. */
+int meb200_amax_accumulate(const void *in, int dtype, uint32_t n, uint32_t c, float *amax_dev,
+                           void *stream);
+int meb200_e4m3_scales(const float *amax_dev, float *scale_dev, void *stream);
+int meb200_quantize_e4m3_static(const void *in, int dtype, uint32_t n, uint32_t c, void *out_e4m3,
+                                const float *scale_dev, void *stream);
+/* The forward that also writes the SHADOW of its output: q [n_out, c_out] e4m3 bytes, at the static
+ * scale q_scale (DEVICE fp32 [2], as scale_dev above) of the layer the output feeds, stored by the
+ * epilogue in the launch that stores out:
+ *   q[o, c] = e4m3(round_out_dtype(v[o, c]) * q_scale[1])
+ * with v the final epilogue value (after the residual and the ReLU), so that q equals
+ * meb200_quantize_e4m3_static(out, q_scale) byte for byte.  The arguments are those of
+ * meb200_conv_forward / meb200_conv_forward_fp8 / meb200_conv_stem_forward, plus q and q_scale;
+ * epi is required.  Only the tensor-core kernels of bf16 / fp16 and e4m3 operands write a shadow:
+ * meb200_conv_forward_q returns MEB200_ERR_UNSUPPORTED, before it launches anything, for a shape
+ * or dtype that would run on TF32, the small-cin kernel or the SIMT gather-GEMM (and so does
+ * meb200_conv_stem_forward_q off the stem kernels).  The caller then runs meb200_conv_forward, and
+ * the next layer quantises its input with meb200_quantize_e4m3_static. */
+int meb200_conv_forward_q(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
+                          const void *w_cast, const void *w_t, uint32_t K, uint32_t c_out,
+                          const int32_t *out_nbr, uint32_t n_out, void *out, int out_dtype,
+                          const int32_t *out_order, const meb200_conv_epilogue *epi, void *q,
+                          const float *q_scale, void *stream);
+int meb200_conv_forward_fp8_q(const void *in_e4m3, const float *a_scale, uint32_t n_in,
+                              uint32_t c_in, const void *w_t_e4m3, uint32_t K, uint32_t c_out,
+                              const int32_t *out_nbr, uint32_t n_out, void *out, int out_dtype,
+                              const int32_t *out_order, const meb200_conv_epilogue *epi, void *q,
+                              const float *q_scale, void *stream);
+int meb200_conv_stem_forward_q(const void *in4, int dtype, uint32_t K, const void *weight_v,
+                               uint32_t c_out, const int32_t *out_nbr, uint32_t n_out, void *out,
+                               int out_dtype, const meb200_conv_epilogue *epi, void *q,
+                               const float *q_scale, void *stream);
+
 /* Weight packing, once per optimizer step instead of once per call: fp32 master weight
  * [K, Cin, Cout] -> `dtype` (BF16/F16, or TF32: fp32 words rounded to tf32) operand copies
  * w_cast [K, Cin, Cout] and w_t [K, Cout, Cin].  The reference keeps weights in the feature dtype and needs no such step

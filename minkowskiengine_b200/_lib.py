@@ -55,6 +55,15 @@ PROTOTYPES = {
     "meb200_conv_pack_weights_e4m3": (_i32, [_vp, _u32, _u32, _u32, _vp, _vp, _vp]),
     "meb200_quantize_e4m3_workspace_bytes": (_u64, []),
     "meb200_quantize_e4m3": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _vp, _vp]),
+    "meb200_amax_accumulate": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp]),
+    "meb200_e4m3_scales": (_i32, [_vp, _vp, _vp]),
+    "meb200_quantize_e4m3_static": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _vp]),
+    "meb200_conv_forward_q": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _u32, _vp,
+                                     _i32, _vp, _vp, _vp, _vp, _vp]),
+    "meb200_conv_forward_fp8_q": (_i32, [_vp, _vp, _u32, _u32, _vp, _u32, _u32, _vp, _u32, _vp,
+                                         _i32, _vp, _vp, _vp, _vp, _vp]),
+    "meb200_conv_stem_forward_q": (_i32, [_vp, _i32, _u32, _vp, _u32, _vp, _u32, _vp, _i32, _vp,
+                                          _vp, _vp, _vp]),
     "meb200_conv_pack_weights": (_i32, [_vp, _u32, _u32, _u32, _i32, _vp, _vp, _vp]),
     "meb200_conv_pack_weights_batched": (_i32, [_vp, _u32, _u32, _i32, _vp]),
     "meb200_conv_stem_virtual_channels": (_u32, [_u32]),

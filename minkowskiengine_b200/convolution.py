@@ -12,6 +12,7 @@ from .backend import CoordinateMapKey
 from .common import MinkowskiModuleBase
 from .coordinate_manager import CoordinateManager
 from .enums import ConvolutionMode, RegionType
+from .fp8_calibration import attach_shadow, input_operand
 from .kernel_generator import KernelGenerator
 from .normalization import MinkowskiBatchNorm, _bn_tail, _eval_scale_shift, _native_ok
 from .sparse_tensor import SparseTensor, _get_coordinate_map_key
@@ -122,6 +123,7 @@ class MinkowskiConvolutionBase(MinkowskiModuleBase):
                 coordinates: Union[torch.Tensor, CoordinateMapKey, SparseTensor] = None):
         assert isinstance(input, SparseTensor)
         assert input.D == self.dimension
+        observer = selected = None
         if self.use_mm:
             out_coordinate_map_key = input.coordinate_map_key
             kernel = self.kernel if self.kernel.dtype == input.F.dtype else self.kernel.to(input.F.dtype)
@@ -132,17 +134,22 @@ class MinkowskiConvolutionBase(MinkowskiModuleBase):
             if _fp8(self, input.F):
                 # the bias is the epilogue's shift: one rounding of the biased output
                 shift = None if self.bias is None else self.bias.detach().float().reshape(-1)
-                outfeat = _forward_with(self, input, out_coordinate_map_key,
-                                        (None, shift, None, False), fp8=True)
-                return SparseTensor(outfeat, coordinate_map_key=out_coordinate_map_key,
-                                    coordinate_manager=input._manager)
+                return _run(self, input, out_coordinate_map_key, (None, shift, None, False),
+                            fp8=True)
+            observer = _C.fp8_observer()
+            if observer is not None:
+                selected = _fp8_rule(self, input.F)
+                observer._observe(self, input, selected)
             outfeat = self.conv.apply(input.F, self.kernel, self.kernel_generator,
                                       self.convolution_mode, input.coordinate_map_key,
                                       out_coordinate_map_key, input._manager)
         if self.bias is not None:
             outfeat = outfeat + self.bias.to(outfeat.dtype)
-        return SparseTensor(outfeat, coordinate_map_key=out_coordinate_map_key,
-                            coordinate_manager=input._manager)
+        out = SparseTensor(outfeat, coordinate_map_key=out_coordinate_map_key,
+                           coordinate_manager=input._manager)
+        if selected:        # in fp8 it runs the e4m3 route, which writes shadows
+            observer._tag(self, out)
+        return out
 
     def reset_parameters(self, is_transpose=False):
         with torch.no_grad():
@@ -236,10 +243,16 @@ def _fuses(conv, norm, feats, res):
 
 def _fp8(conv, feats):
     """Whether `conv` runs its forward on e4m3 operands (backend.fp8_inference): inside the
-    context, for a layer that needs no gradient (feats, kernel or bias requiring one with grad mode
-    on; fused_conv_bn_relu checks the norm and the residual in _fuses), is not a plain matrix product (kernel volume 1, stride 1), has fp32 / bf16 /
-    fp16 features and c_in -> c_out on the e4m3 grid (which leaves out the stem, c_in <= 4)."""
-    if not _C.fp8_enabled() or conv.use_mm or feats.dtype not in _C._FP8_DTYPES:
+    context, when _fp8_rule holds."""
+    return _C.fp8_enabled() and _fp8_rule(conv, feats)
+
+
+def _fp8_rule(conv, feats):
+    """The layers fp8 inference selects (and Fp8Calibration observes): one that needs no gradient
+    (feats, kernel or bias requiring one with grad mode on; fused_conv_bn_relu checks the norm and
+    the residual in _fuses), is not a plain matrix product (kernel volume 1, stride 1), has fp32 /
+    bf16 / fp16 features and c_in -> c_out on the e4m3 grid (which leaves out the stem, c_in <= 4)."""
+    if conv.use_mm or feats.dtype not in _C._FP8_DTYPES:
         return False
     if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (
             feats, conv.kernel, conv.bias)):
@@ -247,14 +260,37 @@ def _fp8(conv, feats):
     return _C.fp8_supported(conv.in_channels, conv.out_channels)
 
 
-def _forward_with(conv, input, out_key, epilogue, fp8=False):
+def _forward_with(conv, input, out_key, epilogue, fp8=False, act=None, shadow=None):
     """conv's native forward onto `out_key` with `epilogue` (no autograd)."""
     kg = conv.kernel_generator
     forward = _C.ConvolutionTransposeForwardGPU if conv.is_transpose else _C.ConvolutionForwardGPU
     return forward(input.F.contiguous(), conv.kernel, kg.kernel_size, kg.kernel_stride,
                    kg.kernel_dilation, kg.region_type, kg.region_offsets, kg.expand_coordinates,
                    conv.convolution_mode, input.coordinate_map_key, out_key,
-                   input._manager._manager, epilogue=epilogue, fp8=fp8)
+                   input._manager._manager, epilogue=epilogue, fp8=fp8, act=act, shadow=shadow)
+
+
+def _run(conv, input, out_key, epilogue, fp8):
+    """conv(input) onto `out_key` with `epilogue`, as a SparseTensor (no autograd).  Inside
+    fp8_inference(calibration) a calibrated e4m3 layer takes its static-scale input
+    (fp8_calibration.input_operand), and a layer that fed a calibrated one also writes the shadow
+    of its output.  While observing, records the input's amax and tags the output."""
+    observer = _C.fp8_observer()
+    if observer is not None:
+        observer._observe(conv, input, _fp8_rule(conv, input.F))
+    calib = _C.fp8_calibration() if _C.fp8_enabled() else None
+    act = input_operand(calib, conv, input) if fp8 else None
+    shadow = calib._shadow_scale(conv, input.F.device) if calib is not None else None
+    feats = _forward_with(conv, input, out_key, epilogue, fp8=fp8, act=act, shadow=shadow)
+    q = None
+    if shadow is not None:
+        feats, q = feats
+    out = SparseTensor(feats, coordinate_map_key=out_key, coordinate_manager=input._manager)
+    if q is not None:
+        attach_shadow(out, q, shadow)
+    if observer is not None:
+        observer._tag(conv, out)
+    return out
 
 
 def _output_key(conv, input):
@@ -303,7 +339,5 @@ def fused_conv_bn_relu(conv, norm, input, residual=None, relu=True):
         return _bn_tail(norm, out, residual, relu)
     assert input.D == conv.dimension
     scale, shift = _eval_scale_shift(norm.bn, conv.bias)
-    feats = _forward_with(conv, input, out_key,
-                          (scale, shift, None if res is None else res.contiguous(), relu),
-                          fp8=_fp8(conv, input.F))
-    return SparseTensor(feats, coordinate_map_key=out_key, coordinate_manager=input._manager)
+    return _run(conv, input, out_key, (scale, shift, None if res is None else res.contiguous(), relu),
+                fp8=_fp8(conv, input.F))

@@ -61,6 +61,31 @@ int meb200_conv_forward(const void *in, int in_dtype, uint32_t n_in, uint32_t c_
                            out_nbr, n_out, out, out_dtype, epi, stream);
 }
 
+// The forward with a shadow: the 16-bit tensor-core route only (see include/meb200.h); anything
+// else returns MEB200_ERR_UNSUPPORTED before it launches.
+int meb200_conv_forward_q(const void *in, int in_dtype, uint32_t n_in, uint32_t c_in,
+                          const void *w_cast, const void *w_t, uint32_t K, uint32_t c_out,
+                          const int32_t *out_nbr, uint32_t n_out, void *out, int out_dtype,
+                          const int32_t *out_order, const meb200_conv_epilogue *epi, void *q,
+                          const float *q_scale, void *stream_) {
+  if (n_out == 0) return MEB200_OK;
+  MEB_CHECK_ARG(in_dtype == MEB200_BF16 || in_dtype == MEB200_F16, "shadow: bf16 / fp16 operands");
+  MEB_CHECK_ARG(out_dtype == MEB200_F32 || out_dtype == in_dtype,
+                "output dtype must be fp32 or the input dtype");
+  MEB_CHECK_ARG(out && w_t && out_nbr && q && q_scale && (in || n_in == 0), "null buffer");
+  MEB_CHECK_ARG(c_in > 0 && c_out > 0 && K > 0, "empty channel/kernel dims");
+  MEB_CHECK_ARG(epi != nullptr && epilogue_ok(epi),
+                "epilogue required: scale and shift, 8-byte aligned pointers");
+  (void)w_cast;
+  if (!conv_tc_supported(in_dtype, c_in, c_out)) {
+    set_error("shadow: c_in=%u c_out=%u outside the tensor-core route", c_in, c_out);
+    return MEB200_ERR_UNSUPPORTED;
+  }
+  const Shadow sh{reinterpret_cast<uint8_t *>(q), q_scale};
+  return conv_forward_tc(in, in_dtype, n_in, c_in, w_t, K, c_out, out_nbr, out_order, n_out, out,
+                         out_dtype, epi, (cudaStream_t)stream_, nullptr, &sh);
+}
+
 int meb200_conv_fp8_supported(uint32_t c_in, uint32_t c_out) {
   return conv_fp8_supported(c_in, c_out) ? 1 : 0;
 }
@@ -84,6 +109,27 @@ int meb200_conv_forward_fp8(const void *in_e4m3, const float *a_scale, uint32_t 
                          n_out, out, out_dtype, epi, (cudaStream_t)stream_, a_scale);
 }
 
+int meb200_conv_forward_fp8_q(const void *in_e4m3, const float *a_scale, uint32_t n_in,
+                              uint32_t c_in, const void *w_t_e4m3, uint32_t K, uint32_t c_out,
+                              const int32_t *out_nbr, uint32_t n_out, void *out, int out_dtype,
+                              const int32_t *out_order, const meb200_conv_epilogue *epi, void *q,
+                              const float *q_scale, void *stream_) {
+  if (n_out == 0) return MEB200_OK;
+  MEB_CHECK_ARG(out_dtype >= 0 && out_dtype <= 2, "output dtype");
+  MEB_CHECK_ARG(out && w_t_e4m3 && a_scale && out_nbr && q && q_scale && (in_e4m3 || n_in == 0),
+                "null buffer");
+  MEB_CHECK_ARG(K > 0, "empty kernel");
+  MEB_CHECK_ARG(epi != nullptr && epilogue_ok(epi),
+                "epilogue required: scale and shift, 8-byte aligned pointers");
+  if (!conv_fp8_supported(c_in, c_out)) {
+    set_error("fp8 forward: c_in=%u c_out=%u outside the e4m3 grid", c_in, c_out);
+    return MEB200_ERR_UNSUPPORTED;
+  }
+  const Shadow sh{reinterpret_cast<uint8_t *>(q), q_scale};
+  return conv_forward_tc(in_e4m3, kOperandE4M3, n_in, c_in, w_t_e4m3, K, c_out, out_nbr, out_order,
+                         n_out, out, out_dtype, epi, (cudaStream_t)stream_, a_scale, &sh);
+}
+
 int meb200_conv_pack_weights_e4m3(const float *weight, uint32_t K, uint32_t c_in, uint32_t c_out,
                                   void *w_t_e4m3, float *w_scale, void *stream_) {
   MEB_CHECK_ARG(weight && w_t_e4m3 && w_scale, "null buffer");
@@ -99,6 +145,26 @@ int meb200_quantize_e4m3(const void *in, int dtype, uint32_t n, uint32_t c, void
   MEB_CHECK_ARG(out_e4m3 && scale_dev && workspace && (in || (uint64_t)n * c == 0), "null buffer");
   return quantize_e4m3(in, dtype, (uint64_t)n * c, out_e4m3, scale_dev, workspace,
                        (cudaStream_t)stream_);
+}
+
+int meb200_amax_accumulate(const void *in, int dtype, uint32_t n, uint32_t c, float *amax_dev,
+                           void *stream_) {
+  MEB_CHECK_ARG(dtype >= 0 && dtype <= 2, "dtype");
+  MEB_CHECK_ARG(amax_dev && (in || (uint64_t)n * c == 0), "null buffer");
+  return amax_accumulate(in, dtype, (uint64_t)n * c, amax_dev, (cudaStream_t)stream_);
+}
+
+int meb200_e4m3_scales(const float *amax_dev, float *scale_dev, void *stream_) {
+  MEB_CHECK_ARG(amax_dev && scale_dev, "null buffer");
+  return e4m3_scales_from_amax(amax_dev, scale_dev, (cudaStream_t)stream_);
+}
+
+int meb200_quantize_e4m3_static(const void *in, int dtype, uint32_t n, uint32_t c, void *out_e4m3,
+                                const float *scale_dev, void *stream_) {
+  MEB_CHECK_ARG(dtype >= 0 && dtype <= 2, "dtype");
+  MEB_CHECK_ARG(out_e4m3 && scale_dev && (in || (uint64_t)n * c == 0), "null buffer");
+  return quantize_e4m3_static(in, dtype, (uint64_t)n * c, out_e4m3, scale_dev,
+                              (cudaStream_t)stream_);
 }
 
 static bool packed_dtype(int dtype) {
@@ -142,6 +208,24 @@ int meb200_conv_stem_forward(const void *in4, int dtype, uint32_t K, const void 
   }
   return conv_stem_forward_tc(in4, dtype, K, weight_v, c_out, out_nbr, n_out, out, out_dtype, epi,
                               (cudaStream_t)stream_);
+}
+
+int meb200_conv_stem_forward_q(const void *in4, int dtype, uint32_t K, const void *weight_v,
+                               uint32_t c_out, const int32_t *out_nbr, uint32_t n_out, void *out,
+                               int out_dtype, const meb200_conv_epilogue *epi, void *q,
+                               const float *q_scale, void *stream_) {
+  if (n_out == 0) return MEB200_OK;
+  MEB_CHECK_ARG(out_dtype == MEB200_F32 || out_dtype == dtype, "output dtype must be fp32 or the input dtype");
+  MEB_CHECK_ARG(in4 && weight_v && out_nbr && out && q && q_scale, "null buffer");
+  MEB_CHECK_ARG(epi != nullptr && epilogue_ok(epi),
+                "epilogue required: scale and shift, 8-byte aligned pointers");
+  if (!conv_stem_tc_supported(dtype, K, c_out)) {
+    set_error("stem forward: shape/dtype outside the tensor-core path (K=%u c_out=%u)", K, c_out);
+    return MEB200_ERR_UNSUPPORTED;
+  }
+  const Shadow sh{reinterpret_cast<uint8_t *>(q), q_scale};
+  return conv_stem_forward_tc(in4, dtype, K, weight_v, c_out, out_nbr, n_out, out, out_dtype, epi,
+                              (cudaStream_t)stream_, &sh);
 }
 
 int meb200_conv_stem_wgrad(const void *in4, const void *grad_out, int dtype, uint32_t K,

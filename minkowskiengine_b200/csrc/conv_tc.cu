@@ -7,7 +7,8 @@
 // Operands are bf16 / fp16, or fp32 words multiplied in TF32 (MEB200_TF32: k_conv_wg<float, ..>
 // for forward / dgrad, k_wgrad_tf32 for the weight gradient, whose MN-major operands tf32 wgmma
 // cannot read).  The eval forward also runs on e4m3 bytes (meb200_conv_forward_fp8:
-// k_conv_wg<__nv_fp8_e4m3, ..>, 32 channels per k-step, always with its epilogue).
+// k_conv_wg<__nv_fp8_e4m3, ..>, 32 channels per k-step, always with its epilogue).  k_conv_wg_q is
+// the forward with the epilogue that also stores an e4m3 shadow of its output (the _q entries).
 //
 // Replaces the reference's per-offset SIMT tile-matmul with per-element atomicAdd
 // (src/convolution_kernel.cu:114-180,320-496): forward and dgrad write every output row exactly
@@ -118,8 +119,12 @@ static_assert(sizeof(FwdParams) == 128 && offsetof(FwdParams, slot_row) == 80, "
 // template parameter, so that the plain forward and the dgrad compile as if it did not exist).
 // TO: the 16-bit output type (out_f32: fp32), T itself except for e4m3 operands, whose kernels
 // always run the epilogue with the accumulator times *p.a_scale.
-template <typename T, int NI, int NT, bool EPI, typename TO = T>
-__global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
+//
+// Q (the _q kernels): also store the shadow, the e4m3 copy of the output at the next layer's static
+// scale: q[orow, col] = e4m3(round_TO(v) * q_scale[1]), v the final epilogue value, so that the
+// bytes are those meb200_quantize_e4m3_static makes of the stored output.
+template <typename T, int NI, int NT, bool EPI, typename TO, bool Q>
+__device__ __forceinline__ void conv_wg(const FwdParams &p, uint8_t *q, const float *q_scale) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t s0 = smem_u32(align1k(smem_raw));
   const uint32_t tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
@@ -208,6 +213,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
   wgmma_wait<0>();
   float a_s = 1.f;
   if constexpr (kIsFp8<T>) a_s = __ldg(p.a_scale);
+  float q_inv = 0.f;
+  if constexpr (Q) q_inv = __ldg(q_scale + 1);
 
   const uint32_t g = lane >> 2, t = lane & 3;
   const uint32_t rbase = row0 + wg * 64 + (warp & 3) * 16 + g;
@@ -247,14 +254,42 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
             v1 = fmaxf(v1, 0.f);
           }
         }
-        if (kIsTf32<T> || p.out_f32)
+        if (kIsTf32<T> || p.out_f32) {
           *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + (size_t)orow * p.out_ld + col) =
               make_float2(v0, v1);
-        else if constexpr (!kIsTf32<T>)
+        } else if constexpr (!kIsTf32<T>) {
+          const uint32_t packed = pack2<TO>(v0, v1);
           *reinterpret_cast<uint32_t *>(reinterpret_cast<TO *>(p.out) + (size_t)orow * p.out_ld + col) =
-              pack2<TO>(v0, v1);
+              packed;
+          if constexpr (Q) {                  // the stored values, not the fp32 ones
+            const float2 r = unpack2<TO>(packed);
+            v0 = r.x;
+            v1 = r.y;
+          }
+        }
+        if constexpr (Q)
+          *reinterpret_cast<uint16_t *>(q + (size_t)orow * p.out_ld + col) =
+              e4m3x2_satfinite(__fmul_rn(v0, q_inv), __fmul_rn(v1, q_inv));
       }
   }
+}
+
+template <typename T, int NI, int NT, bool EPI, typename TO = T>
+__global__ void __launch_bounds__(kThreads, 1) k_conv_wg(const FwdParams p) {
+  conv_wg<T, NI, NT, EPI, TO, false>(p, nullptr, nullptr);
+}
+
+// The forward with its shadow (bf16 / fp16 / e4m3 operands, always with the epilogue).  The shadow
+// rides in a parameter block of its own, so FwdParams and the kernels above keep their layout.
+struct FwdQParams {
+  FwdParams f;
+  uint8_t *q;             // [n_rows, out_ld] e4m3, at this launch's column 0
+  const float *q_scale;   // device fp32 [2]: (scale, inv) of the consumer
+};
+
+template <typename T, int NI, int NT, typename TO>
+__global__ void __launch_bounds__(kThreads, 1) k_conv_wg_q(const FwdQParams p) {
+  conv_wg<T, NI, NT, true, TO, true>(p.f, p.q, p.q_scale);
 }
 
 // =====================================================================================
@@ -771,11 +806,39 @@ static int dispatch_fwd(const FwdParams &p, uint32_t slices, cudaStream_t stream
   set_error("conv tc: %u output columns per launch", p.c_cols);
   return MEB200_ERR_UNSUPPORTED;
 }
-// p.c_cols = all the launch's columns (<= 256): the launch runs them in the chooser's slices
-static int run_fwd(int dtype, FwdParams p, cudaStream_t stream, int out_dtype = MEB200_F32) {
+template <typename T, int NI, int NT, typename TO>
+static int launch_fwd_q(const FwdQParams &p, uint32_t slices, cudaStream_t stream) {
+  auto kern = k_conv_wg_q<T, NI, NT, TO>;
+  MEB_BIG_SMEM(kern);
+  const dim3 grid(cdiv(p.f.n_rows, tc::kFwdRows), slices);
+  kern<<<grid, kThreads, tc::fwd_ring_bytes(p.f.bk * sizeof(T), p.f.c_cols), stream>>>(p);
+  count_tc_launch();
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
+}
+template <typename T, typename TO = T>
+static int dispatch_fwd_q(const FwdQParams &p, uint32_t slices, cudaStream_t stream) {
+#define MEB_L(NI, NT) launch_fwd_q<T, NI, NT, TO>(p, slices, stream)
+  MEB_COLS_DISPATCH(p.f.c_cols, MEB_L)
+#undef MEB_L
+  set_error("conv tc: %u output columns per launch", p.f.c_cols);
+  return MEB200_ERR_UNSUPPORTED;
+}
+// p.c_cols = all the launch's columns (<= 256): the launch runs them in the chooser's slices.
+// shadow (q, q_scale) given: the _q kernels (16-bit or e4m3 operands, with the epilogue).
+static int run_fwd(int dtype, FwdParams p, cudaStream_t stream, int out_dtype = MEB200_F32,
+                   const Shadow *shadow = nullptr) {
   const uint32_t cols = p.c_cols;
   p.c_cols = tc::fwd_col_slice(p.n_rows, cols, (uint32_t)num_sms());
   const uint32_t slices = cols / p.c_cols;
+  if (shadow != nullptr) {
+    const FwdQParams qp{p, shadow->q, shadow->q_scale};
+    if (dtype == kOperandE4M3)
+      return out_dtype == MEB200_F16 ? dispatch_fwd_q<__nv_fp8_e4m3, __half>(qp, slices, stream)
+                                     : dispatch_fwd_q<__nv_fp8_e4m3, __nv_bfloat16>(qp, slices, stream);
+    return dtype == MEB200_BF16 ? dispatch_fwd_q<__nv_bfloat16>(qp, slices, stream)
+                                : dispatch_fwd_q<__half>(qp, slices, stream);
+  }
   if (dtype == kOperandE4M3) {        // always with the epilogue; fp32 output through out_f32
     return out_dtype == MEB200_F16 ? dispatch_fwd<__nv_fp8_e4m3, true, __half>(p, slices, stream)
                                    : dispatch_fwd<__nv_fp8_e4m3, true, __nv_bfloat16>(p, slices, stream);
@@ -893,12 +956,14 @@ static_assert(tc::kFwdRows == kOrderTileRows, "a tile order's tiles are the kern
 int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *B,
                     uint32_t K, uint32_t c_cols, const int32_t *nbr, const int32_t *order,
                     uint32_t n_rows, void *out, int out_dtype, const meb200_conv_epilogue *epi,
-                    cudaStream_t stream, const float *a_scale) {
+                    cudaStream_t stream, const float *a_scale, const Shadow *shadow) {
   if (n_rows == 0) return MEB200_OK;
   const bool fp8 = dtype == kOperandE4M3;
   MEB_CHECK_ARG(fp8 ? conv_fp8_supported(c_reduce, c_cols) && epi != nullptr && a_scale != nullptr
                     : conv_tc_supported(dtype, c_reduce, c_cols),
                 "shape not supported by tc path");
+  MEB_CHECK_ARG(shadow == nullptr || (epi != nullptr && dtype != MEB200_TF32),
+                "shadow: 16-bit or e4m3 operands with an epilogue");
   if (!aligned(16, A, B)) {
     set_error("conv tc: operands must be 16-byte aligned");
     return MEB200_ERR_UNSUPPORTED;
@@ -921,7 +986,9 @@ int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, c
     p.bk = tc::fwd_stage_bytes(c_reduce, esz) / esz; p.out_f32 = out_dtype == MEB200_F32;
     set_epilogue(p, epi, n0, out_esz);
     p.a_scale = a_scale;
-    const int rc = run_fwd(dtype, p, stream, out_dtype);
+    Shadow sh{};
+    if (shadow != nullptr) sh = Shadow{shadow->q + n0, shadow->q_scale};
+    const int rc = run_fwd(dtype, p, stream, out_dtype, shadow != nullptr ? &sh : nullptr);
     if (rc != MEB200_OK) return rc;
   }
   return MEB200_OK;
@@ -937,9 +1004,11 @@ bool conv_stem_tc_supported(int dtype, uint32_t K, uint32_t c_cols) {
 
 int conv_stem_forward_tc(const void *A4, int dtype, uint32_t K, const void *Wv, uint32_t c_cols,
                          const int32_t *nbr, uint32_t n_rows, void *out, int out_dtype,
-                         const meb200_conv_epilogue *epi, cudaStream_t stream) {
+                         const meb200_conv_epilogue *epi, cudaStream_t stream,
+                         const Shadow *shadow) {
   if (n_rows == 0) return MEB200_OK;
   MEB_CHECK_ARG(conv_stem_tc_supported(dtype, K, c_cols), "stem forward: K=%u c_out=%u", K, c_cols);
+  MEB_CHECK_ARG(shadow == nullptr || epi != nullptr, "shadow: the epilogue is required");
   if (!aligned(8, A4) || !aligned(16, Wv)) {
     set_error("stem forward: operands must be 8 / 16-byte aligned");
     return MEB200_ERR_UNSUPPORTED;
@@ -950,7 +1019,7 @@ int conv_stem_forward_tc(const void *A4, int dtype, uint32_t K, const void *Wv, 
   p.out_ld = c_cols; p.bk = tc::fwd_bk(p.c_red); p.out_f32 = out_dtype == MEB200_F32;
   p.stem_K = K;
   set_epilogue(p, epi, 0, out_dtype == MEB200_F32 ? 4 : 2);
-  return run_fwd(dtype, p, stream);
+  return run_fwd(dtype, p, stream, out_dtype, shadow);
 }
 
 bool conv_stem_wgrad_tc_supported(int dtype, uint32_t K, uint32_t c_out) {

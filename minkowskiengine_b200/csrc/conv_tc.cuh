@@ -14,6 +14,13 @@ constexpr int kOperandE4M3 = 100;
 bool conv_fp8_supported(uint32_t c_in, uint32_t c_out);
 bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out);
 
+// The shadow of a forward (the _q entries of include/meb200.h): q [n_rows, c_cols] e4m3 bytes of the
+// stored output at the scale q_scale (device fp32 [2]: scale, inv) of the layer it feeds.
+struct Shadow {
+  uint8_t *q;
+  const float *q_scale;
+};
+
 // out[r,:] = sum_k A[nbr[k][r],:] @ B[k]^T with B [K, c_cols, c_reduce] (reduction contiguous):
 // the forward passes w_t [K, c_out, c_in], the dgrad the layer's w_cast [K, c_in, c_out].
 // order (may be NULL; read when K <= 32): the tile order of nbr from meb200_kernel_map, so that
@@ -21,10 +28,12 @@ bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out);
 // epilogue (meb200_conv_epilogue); the dgrad passes NULL.
 // dtype kOperandE4M3: A and B are e4m3 bytes, out_dtype bf16 / fp16 / fp32, and the epilogue
 // (required) runs on the accumulator times *a_scale (a device pointer).
+// shadow (may be NULL; bf16 / fp16 / e4m3 operands with an epilogue): also write the shadow.
 int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, const void *B,
                     uint32_t K, uint32_t c_cols, const int32_t *nbr, const int32_t *order,
                     uint32_t n_rows, void *out, int out_dtype, const meb200_conv_epilogue *epi,
-                    cudaStream_t stream, const float *a_scale = nullptr);
+                    cudaStream_t stream, const float *a_scale = nullptr,
+                    const Shadow *shadow = nullptr);
 
 // fp32 W [K, c_in, c_out] -> w_t [K, c_out, c_in] in e4m3 with a scale per output channel:
 // w_scale[c] = amax_c / 448 (1 when amax_c = 0), w_t = satfinite_rn(W * (448 / amax_c)).
@@ -35,6 +44,11 @@ int conv_pack_weights_e4m3(const float *W, uint32_t K, uint32_t c_in, uint32_t c
 uint64_t quantize_e4m3_workspace_bytes();
 int quantize_e4m3(const void *in, int dtype, uint64_t count, void *out, float *scale, void *workspace,
                   cudaStream_t stream);
+// Static scales (meb200_amax_accumulate, meb200_e4m3_scales, meb200_quantize_e4m3_static).
+int amax_accumulate(const void *in, int dtype, uint64_t count, float *amax, cudaStream_t stream);
+int e4m3_scales_from_amax(const float *amax, float *scale, cudaStream_t stream);
+int quantize_e4m3_static(const void *in, int dtype, uint64_t count, void *out, const float *scale,
+                         cudaStream_t stream);
 
 // fp32 W[K,c_in,c_out] -> w_cast [K,c_in,c_out] and w_t [K,c_out,c_in] in bf16/fp16, or in fp32
 // words rounded to tf32 (MEB200_TF32).
@@ -74,7 +88,8 @@ int conv_wgrad_pairs(const void *in, const void *grad_out, int dtype, uint32_t c
 bool conv_stem_tc_supported(int dtype, uint32_t K, uint32_t c_cols);
 int conv_stem_forward_tc(const void *A4, int dtype, uint32_t K, const void *Wv, uint32_t c_cols,
                          const int32_t *nbr, uint32_t n_rows, void *out, int out_dtype,
-                         const meb200_conv_epilogue *epi, cudaStream_t stream);
+                         const meb200_conv_epilogue *epi, cudaStream_t stream,
+                         const Shadow *shadow = nullptr);
 bool conv_stem_wgrad_tc_supported(int dtype, uint32_t K, uint32_t c_out);
 int conv_stem_wgrad_tc(const void *in4, const void *grad_out, int dtype, uint32_t K,
                        uint32_t c_out, const int32_t *nbr, uint32_t n_rows, float *dWv,

@@ -46,9 +46,9 @@ __device__ __forceinline__ uint8_t e4m3_byte(float x, float inv) {
 // (non-negative floats order as their bit patterns).  The last CTA to finish writes scale[0] = scale,
 // scale[1] = inv and leaves the workspace zero again.  ws: [0] amax bits, [1] CTAs done (a ticket
 // that wraps to 0 at the last CTA).
+// The CTA's max, valid in thread 0 (the other threads return false).
 template <typename T, bool VEC>
-__global__ void __launch_bounds__(kQThreads) k_amax(const T *__restrict__ x, uint64_t count,
-                                                   float *__restrict__ scale, uint32_t *ws) {
+__device__ __forceinline__ bool cta_amax(const T *__restrict__ x, uint64_t count, float &m_out) {
   constexpr uint32_t V = VEC ? 16 / sizeof(T) : 1;
   float m = 0.f;
   const uint64_t n_vec = count / V, stride = (uint64_t)gridDim.x * blockDim.x;
@@ -66,8 +66,17 @@ __global__ void __launch_bounds__(kQThreads) k_amax(const T *__restrict__ x, uin
   __shared__ float wm[kQThreads / 32];
   if ((threadIdx.x & 31) == 0) wm[threadIdx.x >> 5] = m;
   __syncthreads();
-  if (threadIdx.x != 0) return;
+  if (threadIdx.x != 0) return false;
   for (uint32_t w = 1; w < kQThreads / 32; ++w) m = fmaxf(m, wm[w]);
+  m_out = m;
+  return true;
+}
+
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kQThreads) k_amax(const T *__restrict__ x, uint64_t count,
+                                                   float *__restrict__ scale, uint32_t *ws) {
+  float m;
+  if (!cta_amax<T, VEC>(x, count, m)) return;
   atomicMax(ws, __float_as_uint(m));
   __threadfence();
   if (atomicInc(ws + 1, gridDim.x - 1) != gridDim.x - 1) return;
@@ -114,11 +123,15 @@ __global__ void __launch_bounds__(kQThreads) k_quant(const T *__restrict__ x, ui
 
 uint64_t quantize_e4m3_workspace_bytes() { return 16; }
 
+static uint32_t quant_ctas(uint64_t count) {
+  return (uint32_t)std::min<uint64_t>(std::max<uint64_t>(cdiv(count, 16ull * kQThreads), 1),
+                                      std::min<uint32_t>(kQMaxCtas, 4 * num_sms()));
+}
+
 int quantize_e4m3(const void *in, int dtype, uint64_t count, void *out, float *scale,
                   void *workspace, cudaStream_t stream) {
   const bool vec = aligned(16, in, out);
-  const uint32_t ctas = (uint32_t)std::min<uint64_t>(
-      std::max<uint64_t>(cdiv(count, 16ull * kQThreads), 1), std::min<uint32_t>(kQMaxCtas, 4 * num_sms()));
+  const uint32_t ctas = quant_ctas(count);
   uint32_t *ws = reinterpret_cast<uint32_t *>(workspace);
   uint8_t *q = reinterpret_cast<uint8_t *>(out);
   MEB_DISPATCH_DTYPE(dtype, {
@@ -132,6 +145,56 @@ int quantize_e4m3(const void *in, int dtype, uint64_t count, void *out, float *s
       MEB_LAUNCH_OK();
       k_quant<T, false><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
     }
+    MEB_LAUNCH_OK();
+  });
+  return MEB200_OK;
+}
+
+// ---- static scales --------------------------------------------------------------------------------
+// Calibration: amax = max(amax, max |x| over the finite values), k_amax's CTA max and atomic max on
+// the fp32 bits, with nothing to count or reset: any number of calls accumulate into one float.
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kQThreads) k_amax_acc(const T *__restrict__ x, uint64_t count,
+                                                       uint32_t *amax) {
+  float m;
+  if (cta_amax<T, VEC>(x, count, m)) atomicMax(amax, __float_as_uint(m));
+}
+
+__global__ void k_scales(const float *__restrict__ amax, float *__restrict__ scale) {
+  float s, inv;
+  e4m3_scales(*amax, s, inv);
+  scale[0] = s;
+  scale[1] = inv;
+}
+
+int amax_accumulate(const void *in, int dtype, uint64_t count, float *amax, cudaStream_t stream) {
+  if (count == 0) return MEB200_OK;
+  const uint32_t ctas = quant_ctas(count);
+  uint32_t *a = reinterpret_cast<uint32_t *>(amax);
+  MEB_DISPATCH_DTYPE(dtype, {
+    const T *x = reinterpret_cast<const T *>(in);
+    if (aligned(16, in)) k_amax_acc<T, true><<<ctas, kQThreads, 0, stream>>>(x, count, a);
+    else k_amax_acc<T, false><<<ctas, kQThreads, 0, stream>>>(x, count, a);
+    MEB_LAUNCH_OK();
+  });
+  return MEB200_OK;
+}
+
+int e4m3_scales_from_amax(const float *amax, float *scale, cudaStream_t stream) {
+  k_scales<<<1, 1, 0, stream>>>(amax, scale);
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
+}
+
+int quantize_e4m3_static(const void *in, int dtype, uint64_t count, void *out, const float *scale,
+                         cudaStream_t stream) {
+  if (count == 0) return MEB200_OK;
+  const uint32_t ctas = quant_ctas(count);
+  uint8_t *q = reinterpret_cast<uint8_t *>(out);
+  MEB_DISPATCH_DTYPE(dtype, {
+    const T *x = reinterpret_cast<const T *>(in);
+    if (aligned(16, in, out)) k_quant<T, true><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
+    else k_quant<T, false><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
     MEB_LAUNCH_OK();
   });
   return MEB200_OK;
