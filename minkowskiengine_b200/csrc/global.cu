@@ -10,6 +10,8 @@
 // therefore bit-identical run to run, whatever order the CTAs run in.
 #include <float.h>
 
+#include <atomic>
+
 #include <cub/block/block_scan.cuh>
 
 #include "common.cuh"
@@ -396,20 +398,44 @@ static int group_rows(const int32_t *row_seg, uint32_t n, uint32_t B, int32_t *o
   return MEB200_OK;
 }
 
+// The combine of k_seg_reduce_tiles holds [rp][C] values (and, for MAX, rows): at most 8 * 8192
+// bytes, for MAX over C > 6144 channels on one row lane.  A launch above the default 48 KB needs
+// the kernel opted in on the current device, which is done once per instantiation and device.
+constexpr size_t kSegMaxSmem = 8 * 8192;
+
+template <typename T, int V, int MODE, bool PROD>
+static int seg_reduce_smem_opt_in(size_t smem) {
+  if (smem <= 48 * 1024) return MEB200_OK;
+  static std::atomic<uint32_t> done{0};   // bit d: device d opted in
+  int dev = 0;
+  MEB_CUDA(cudaGetDevice(&dev));
+  uint32_t bit = dev < 32 ? 1u << dev : 0u;
+  if (done.load() & bit) return MEB200_OK;
+  MEB_CUDA(cudaFuncSetAttribute(k_seg_reduce_tiles<T, V, MODE, PROD>,
+                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSegMaxSmem));
+  done.fetch_or(bit);
+  return MEB200_OK;
+}
+
 template <typename T, int V, int MODE>
-static void seg_reduce_launch(const void *a, const void *b, uint32_t C, const int32_t *order,
-                              const int32_t *seg_start, const int32_t *tile_start, uint32_t B,
-                              uint32_t max_tiles, float *part, int32_t *part_row, cudaStream_t st) {
+static int seg_reduce_launch(const void *a, const void *b, uint32_t C, const int32_t *order,
+                             const int32_t *seg_start, const int32_t *tile_start, uint32_t B,
+                             uint32_t max_tiles, float *part, int32_t *part_row, cudaStream_t st) {
   uint32_t CV = C / V, tpr = 1;
   while (tpr * 2 <= CV && tpr * 2 <= 256) tpr *= 2;     // threads per row: a power of two <= 256
   uint32_t rp = 256 / tpr;
   size_t smem = (size_t)rp * C * (MODE == MEB200_SEG_MAX ? 8 : 4);
-  if (b)
+  int rc;
+  if (b) {
+    if ((rc = seg_reduce_smem_opt_in<T, V, MODE, true>(smem)) != MEB200_OK) return rc;
     k_seg_reduce_tiles<T, V, MODE, true><<<max_tiles, 256, smem, st>>>(
         (const T *)a, (const T *)b, C, order, seg_start, tile_start, B, tpr, part, part_row);
-  else
+  } else {
+    if ((rc = seg_reduce_smem_opt_in<T, V, MODE, false>(smem)) != MEB200_OK) return rc;
     k_seg_reduce_tiles<T, V, MODE, false><<<max_tiles, 256, smem, st>>>(
         (const T *)a, nullptr, C, order, seg_start, tile_start, B, tpr, part, part_row);
+  }
+  return MEB200_OK;
 }
 
 template <typename T>
@@ -418,17 +444,19 @@ static int seg_reduce_t(const void *a, const void *b, uint32_t C, const int32_t 
                         uint32_t max_tiles, int mode, float *part, int32_t *part_row,
                         cudaStream_t st) {
   bool v4 = C % 4 == 0 && aligned(4 * sizeof(T), a, b);
+  int rc = MEB200_OK;
 #define MEB_SEG(MODE)                                                                           \
-  if (v4) seg_reduce_launch<T, 4, MODE>(a, b, C, order, seg_start, tile_start, B, max_tiles, part, \
-                                        part_row, st);                                          \
-  else seg_reduce_launch<T, 1, MODE>(a, b, C, order, seg_start, tile_start, B, max_tiles, part,   \
-                                     part_row, st);
+  if (v4) rc = seg_reduce_launch<T, 4, MODE>(a, b, C, order, seg_start, tile_start, B, max_tiles, \
+                                             part, part_row, st);                               \
+  else rc = seg_reduce_launch<T, 1, MODE>(a, b, C, order, seg_start, tile_start, B, max_tiles,  \
+                                          part, part_row, st);
   switch (mode) {
     case MEB200_SEG_SUM: MEB_SEG(MEB200_SEG_SUM); break;
     case MEB200_SEG_AVG: MEB_SEG(MEB200_SEG_AVG); break;
     case MEB200_SEG_MAX: MEB_SEG(MEB200_SEG_MAX); break;
   }
 #undef MEB_SEG
+  if (rc != MEB200_OK) return rc;
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
