@@ -328,6 +328,32 @@ int meb200_conv_stem_forward_q(const void *in4, int dtype, uint32_t K, const voi
                                int out_dtype, const meb200_conv_epilogue *epi, void *q,
                                const float *q_scale, void *stream);
 
+/* ---- fp8 training: the input gradient on e5m2 x e4m3 -------------------------------------------
+ * The dgrad of a convolution (meb200_conv_backward's grad_in) on the Hopper fp8 tensor cores: the
+ * output gradient quantised to e5m2 with one scale per tensor, the weights to e4m3 with one scale
+ * per INPUT channel (the dgrad's output column), the products summed by the tensor cores:
+ *   grad_in[i, ci] = acc[i, ci] * g_scale * w_scale[ci]
+ * with acc the sum of e5m2 x e4m3 products over in_nbr, rounded to grad_in_dtype (F32, BF16 or
+ * F16, the layer's feature dtype).  The weight gradient keeps meb200_conv_backward.
+ * e5m2 quantisation: the e4m3 formula above with 57344 (the largest finite e5m2) for 448:
+ *   scale = amax / 57344, inv = 57344 / amax, q = cvt.rn.satfinite.e5m2(x * inv)
+ *   (both 1 when amax = 0; inv = FLT_MAX and scale = 1 / FLT_MAX when 57344 / amax overflows;
+ *   +-inf -> +-57344, NaN -> NaN).
+ * meb200_quantize_e5m2: as meb200_quantize_e4m3 (two launches, the same workspace), in e5m2.
+ * meb200_conv_pack_weights_e4m3_dgrad: fp32 weight [K, c_in, c_out] -> w_e4m3 [K, c_in, c_out]
+ *   (not transposed) and w_scale fp32 [c_in], amax per input channel over (k, c_out).
+ * meb200_conv_dgrad_fp8: grad_e5m2 [n_out, c_out] and g_scale (DEVICE fp32, the dequantisation
+ *   factor) from meb200_quantize_e5m2; in_nbr / in_order as in meb200_conv_backward; the shape
+ *   must satisfy meb200_conv_fp8_supported(c_out, c_in).  No stem mode, no shadow. */
+int meb200_quantize_e5m2(const void *in, int dtype, uint32_t n, uint32_t c, void *out_e5m2,
+                         float *scale_dev, void *workspace, void *stream);
+int meb200_conv_pack_weights_e4m3_dgrad(const float *weight, uint32_t K, uint32_t c_in,
+                                        uint32_t c_out, void *w_e4m3, float *w_scale, void *stream);
+int meb200_conv_dgrad_fp8(const void *grad_e5m2, const float *g_scale, uint32_t n_out,
+                          uint32_t c_out, const void *w_e4m3, const float *w_scale, uint32_t K,
+                          uint32_t c_in, const int32_t *in_nbr, uint32_t n_in, void *grad_in,
+                          int grad_in_dtype, const int32_t *in_order, void *stream);
+
 /* Weight packing, once per optimizer step instead of once per call: fp32 master weight
  * [K, Cin, Cout] -> `dtype` (BF16/F16, or TF32: fp32 words rounded to tf32) operand copies
  * w_cast [K, Cin, Cout] and w_t [K, Cout, Cin].  The reference keeps weights in the feature dtype and needs no such step

@@ -49,7 +49,7 @@ from .broadcast import (MinkowskiBroadcast, MinkowskiBroadcastAddition,
 from .normalization import (MinkowskiBatchNorm, MinkowskiInstanceNorm,
                             MinkowskiInstanceNormFunction, MinkowskiSyncBatchNorm, fused_bn_relu)
 from .convolution import fused_conv_bn_relu
-from .backend import fp8_inference
+from .backend import fp8_inference, fp8_training
 from .fp8_calibration import Fp8Calibration
 from .nonlinearity import *  # noqa: F401,F403
 from .ops import (MinkowskiLinear, MinkowskiStackCat, MinkowskiStackMean, MinkowskiStackSum,

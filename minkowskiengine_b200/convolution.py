@@ -24,7 +24,7 @@ class MinkowskiConvolutionFunction(Function):
                 kernel_generator: KernelGenerator, convolution_mode: ConvolutionMode,
                 in_coordinate_map_key: CoordinateMapKey,
                 out_coordinate_map_key: CoordinateMapKey = None,
-                coordinate_manager: CoordinateManager = None):
+                coordinate_manager: CoordinateManager = None, fp8: bool = False):
         if out_coordinate_map_key is None:
             out_coordinate_map_key = CoordinateMapKey(
                 in_coordinate_map_key.get_coordinate_size())
@@ -33,12 +33,13 @@ class MinkowskiConvolutionFunction(Function):
         ctx.kernel_weights = kernel_weights
         ctx.misc = (kernel_generator, convolution_mode, in_coordinate_map_key,
                     out_coordinate_map_key, coordinate_manager)
+        ctx.fp8 = fp8
         return _C.ConvolutionForwardGPU(
             input_features, kernel_weights, kernel_generator.kernel_size,
             kernel_generator.kernel_stride, kernel_generator.kernel_dilation,
             kernel_generator.region_type, kernel_generator.region_offsets,
             kernel_generator.expand_coordinates, convolution_mode, in_coordinate_map_key,
-            out_coordinate_map_key, coordinate_manager._manager)
+            out_coordinate_map_key, coordinate_manager._manager, fp8=fp8)
 
     @staticmethod
     def backward(ctx, grad_out_feat: torch.Tensor):
@@ -48,8 +49,8 @@ class MinkowskiConvolutionFunction(Function):
             ctx.input_features, grad_out_feat, ctx.kernel_weights, kgen.kernel_size,
             kgen.kernel_stride, kgen.kernel_dilation, kgen.region_type, kgen.region_offsets,
             mode, in_key, out_key, manager._manager,
-            need_in=ctx.needs_input_grad[0], need_w=ctx.needs_input_grad[1])
-        return grad_in_feat, grad_kernel, None, None, None, None, None
+            need_in=ctx.needs_input_grad[0], need_w=ctx.needs_input_grad[1], fp8=ctx.fp8)
+        return grad_in_feat, grad_kernel, None, None, None, None, None, None
 
 
 class MinkowskiConvolutionTransposeFunction(Function):
@@ -58,7 +59,7 @@ class MinkowskiConvolutionTransposeFunction(Function):
                 kernel_generator: KernelGenerator, convolution_mode: ConvolutionMode,
                 in_coordinate_map_key: CoordinateMapKey,
                 out_coordinate_map_key: CoordinateMapKey = None,
-                coordinate_manager: CoordinateManager = None):
+                coordinate_manager: CoordinateManager = None, fp8: bool = False):
         if out_coordinate_map_key is None:
             out_coordinate_map_key = CoordinateMapKey(
                 in_coordinate_map_key.get_coordinate_size())
@@ -67,12 +68,13 @@ class MinkowskiConvolutionTransposeFunction(Function):
         ctx.kernel_weights = kernel_weights
         ctx.misc = (kernel_generator, convolution_mode, in_coordinate_map_key,
                     out_coordinate_map_key, coordinate_manager)
+        ctx.fp8 = fp8
         return _C.ConvolutionTransposeForwardGPU(
             input_features, kernel_weights, kernel_generator.kernel_size,
             kernel_generator.kernel_stride, kernel_generator.kernel_dilation,
             kernel_generator.region_type, kernel_generator.region_offsets,
             kernel_generator.expand_coordinates, convolution_mode, in_coordinate_map_key,
-            out_coordinate_map_key, coordinate_manager._manager)
+            out_coordinate_map_key, coordinate_manager._manager, fp8=fp8)
 
     @staticmethod
     def backward(ctx, grad_out_feat: torch.Tensor):
@@ -82,8 +84,8 @@ class MinkowskiConvolutionTransposeFunction(Function):
             ctx.input_features, grad_out_feat, ctx.kernel_weights, kgen.kernel_size,
             kgen.kernel_stride, kgen.kernel_dilation, kgen.region_type, kgen.region_offsets,
             mode, in_key, out_key, manager._manager,
-            need_in=ctx.needs_input_grad[0], need_w=ctx.needs_input_grad[1])
-        return grad_in_feat, grad_kernel, None, None, None, None, None
+            need_in=ctx.needs_input_grad[0], need_w=ctx.needs_input_grad[1], fp8=ctx.fp8)
+        return grad_in_feat, grad_kernel, None, None, None, None, None, None
 
 
 class MinkowskiConvolutionBase(MinkowskiModuleBase):
@@ -142,7 +144,8 @@ class MinkowskiConvolutionBase(MinkowskiModuleBase):
                 observer._observe(self, input, selected)
             outfeat = self.conv.apply(input.F, self.kernel, self.kernel_generator,
                                       self.convolution_mode, input.coordinate_map_key,
-                                      out_coordinate_map_key, input._manager)
+                                      out_coordinate_map_key, input._manager,
+                                      _fp8_train(self, input.F))
         if self.bias is not None:
             outfeat = outfeat + self.bias.to(outfeat.dtype)
         out = SparseTensor(outfeat, coordinate_map_key=out_coordinate_map_key,
@@ -258,6 +261,27 @@ def _fp8_rule(conv, feats):
             feats, conv.kernel, conv.bias)):
         return False
     return _C.fp8_supported(conv.in_channels, conv.out_channels)
+
+
+def _fp8_train(conv, feats):
+    """Whether `conv` runs its forward on e4m3 and its input gradient on e5m2 x e4m3 operands
+    (backend.fp8_training): inside the context, when _fp8_train_rule holds."""
+    return _C.fp8_training_enabled() and _fp8_train_rule(conv, feats)
+
+
+def _fp8_train_rule(conv, feats):
+    """The layers fp8 training selects: one that needs a gradient (grad mode on and feats, kernel
+    or bias requiring one: the negation of _fp8_rule's check), is not a plain matrix product (kernel
+    volume 1, stride 1), has fp32 / bf16 / fp16 features, and is on the e4m3 grid both ways,
+    c_in -> c_out for the forward and c_out -> c_in for the dgrad (whether or not the input needs a
+    gradient; this leaves out the stem, c_in <= 4)."""
+    if conv.use_mm or feats.dtype not in _C._FP8_DTYPES:
+        return False
+    if not (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (
+            feats, conv.kernel, conv.bias))):
+        return False
+    return (_C.fp8_supported(conv.in_channels, conv.out_channels)
+            and _C.fp8_supported(conv.out_channels, conv.in_channels))
 
 
 def _forward_with(conv, input, out_key, epilogue, fp8=False, act=None, shadow=None):

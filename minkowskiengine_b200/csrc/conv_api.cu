@@ -139,6 +139,45 @@ int meb200_conv_pack_weights_e4m3(const float *weight, uint32_t K, uint32_t c_in
 
 uint64_t meb200_quantize_e4m3_workspace_bytes(void) { return quantize_e4m3_workspace_bytes(); }
 
+int meb200_quantize_e5m2(const void *in, int dtype, uint32_t n, uint32_t c, void *out_e5m2,
+                         float *scale_dev, void *workspace, void *stream_) {
+  MEB_CHECK_ARG(dtype >= 0 && dtype <= 2, "dtype");
+  MEB_CHECK_ARG(out_e5m2 && scale_dev && workspace && (in || (uint64_t)n * c == 0), "null buffer");
+  return quantize_e5m2(in, dtype, (uint64_t)n * c, out_e5m2, scale_dev, workspace,
+                       (cudaStream_t)stream_);
+}
+
+int meb200_conv_pack_weights_e4m3_dgrad(const float *weight, uint32_t K, uint32_t c_in,
+                                        uint32_t c_out, void *w_e4m3, float *w_scale,
+                                        void *stream_) {
+  MEB_CHECK_ARG(weight && w_e4m3 && w_scale, "null buffer");
+  MEB_CHECK_ARG(c_in > 0 && c_out > 0 && K > 0, "empty channel/kernel dims");
+  return conv_pack_weights_e4m3_dgrad(weight, K, c_in, c_out, w_e4m3, w_scale,
+                                      (cudaStream_t)stream_);
+}
+
+// The forward kernel on the transposed table, as meb200_conv_backward's dgrad, with e5m2 gradients
+// against e4m3 weights [K, c_in, c_out]; the epilogue is the weight scale of each column alone.
+int meb200_conv_dgrad_fp8(const void *grad_e5m2, const float *g_scale, uint32_t n_out,
+                          uint32_t c_out, const void *w_e4m3, const float *w_scale, uint32_t K,
+                          uint32_t c_in, const int32_t *in_nbr, uint32_t n_in, void *grad_in,
+                          int grad_in_dtype, const int32_t *in_order, void *stream_) {
+  if (n_in == 0) return MEB200_OK;
+  MEB_CHECK_ARG(grad_in_dtype >= 0 && grad_in_dtype <= 2, "grad_in dtype");
+  MEB_CHECK_ARG(grad_in && w_e4m3 && w_scale && g_scale && in_nbr && (grad_e5m2 || n_out == 0),
+                "null buffer");
+  MEB_CHECK_ARG(K > 0, "empty kernel");
+  MEB_CHECK_ARG(aligned(8, w_scale), "w_scale must be 8-byte aligned");
+  if (!conv_fp8_supported(c_out, c_in)) {
+    set_error("fp8 dgrad: c_out=%u c_in=%u outside the e4m3 grid", c_out, c_in);
+    return MEB200_ERR_UNSUPPORTED;
+  }
+  const meb200_conv_epilogue epi{w_scale, nullptr, nullptr, 0};
+  return conv_forward_tc(grad_e5m2, kOperandE5M2E4M3, n_out, c_out, w_e4m3, K, c_in, in_nbr,
+                         in_order, n_in, grad_in, grad_in_dtype, &epi, (cudaStream_t)stream_,
+                         g_scale);
+}
+
 int meb200_quantize_e4m3(const void *in, int dtype, uint32_t n, uint32_t c, void *out_e4m3,
                          float *scale_dev, void *workspace, void *stream_) {
   MEB_CHECK_ARG(dtype >= 0 && dtype <= 2, "dtype");

@@ -6,8 +6,10 @@
 //
 // Operands are bf16 / fp16, or fp32 words multiplied in TF32 (MEB200_TF32: k_conv_wg<float, ..>
 // for forward / dgrad, k_wgrad_tf32 for the weight gradient, whose MN-major operands tf32 wgmma
-// cannot read).  The eval forward also runs on e4m3 bytes (meb200_conv_forward_fp8:
-// k_conv_wg<__nv_fp8_e4m3, ..>, 32 channels per k-step, always with its epilogue).  k_conv_wg_q is
+// cannot read).  The forward also runs on e4m3 bytes (meb200_conv_forward_fp8:
+// k_conv_wg<__nv_fp8_e4m3, ..>, 32 channels per k-step, always with its epilogue), and the fp8
+// dgrad on e5m2 gradients against e4m3 weights (meb200_conv_dgrad_fp8: k_conv_wg<__nv_fp8_e5m2,
+// ..>, the same staging with the e5m2 x e4m3 MMA).  k_conv_wg_q is
 // the forward with the epilogue that also stores an e4m3 shadow of its output (the _q entries).
 //
 // Replaces the reference's per-offset SIMT tile-matmul with per-element atomicAdd
@@ -52,8 +54,11 @@ template <typename T>
 constexpr bool kIsBf16 = std::is_same<T, __nv_bfloat16>::value;
 template <typename T>
 constexpr bool kIsTf32 = std::is_same<T, float>::value;   // fp32 storage, tf32 MMAs
+// fp8 operands: e4m3 both sides (the forward), or e5m2 A against e4m3 B (the dgrad: T names A)
 template <typename T>
-constexpr bool kIsFp8 = std::is_same<T, __nv_fp8_e4m3>::value;   // e4m3 operands (inference)
+constexpr bool kIsE5M2 = std::is_same<T, __nv_fp8_e5m2>::value;
+template <typename T>
+constexpr bool kIsFp8 = std::is_same<T, __nv_fp8_e4m3>::value || kIsE5M2<T>;
 
 template <typename T>
 __device__ __forceinline__ uint32_t pack2(float a, float b);
@@ -117,8 +122,9 @@ static_assert(sizeof(FwdParams) == 128 && offsetof(FwdParams, slot_row) == 80, "
 // NT wgmma instructions of N = NI columns each cover the c_cols = NI * NT columns of the slice.
 // grid = (128-row tiles, column slices).  EPI: apply the epilogue of p before the conversion (a
 // template parameter, so that the plain forward and the dgrad compile as if it did not exist).
-// TO: the 16-bit output type (out_f32: fp32), T itself except for e4m3 operands, whose kernels
-// always run the epilogue with the accumulator times *p.a_scale.
+// TO: the 16-bit output type (out_f32: fp32), T itself except for fp8 operands, whose kernels
+// multiply the accumulator by *p.a_scale first.  e4m3 kernels always run the epilogue; the e5m2
+// dgrad kernels (EPI = false) only multiply column col by p.scale[col], the weight scale.
 //
 // Q (the _q kernels): also store the shadow, the e4m3 copy of the output at the next layer's static
 // scale: q[orow, col] = e4m3(round_TO(v) * q_scale[1]), v the final epilogue value, so that the
@@ -203,6 +209,7 @@ __device__ __forceinline__ void conv_wg(const FwdParams &p, uint8_t *q, const fl
       for (int i = 0; i < NT; ++i) {
         const uint64_t db = wgmma_desc(b0 + i * NI * width + kk * 256, 128, sbo);
         if constexpr (kIsTf32<T>) wgmma_tf32<NI, 0, 0>(acc[i], da, db);
+        else if constexpr (kIsE5M2<T>) wgmma_e5m2e4m3<NI>(acc[i], da, db);
         else if constexpr (kIsFp8<T>) wgmma_e4m3<NI>(acc[i], da, db);
         else wgmma<NI, kIsBf16<T>, 0, 0>(acc[i], da, db);
       }
@@ -232,6 +239,11 @@ __device__ __forceinline__ void conv_wg(const FwdParams &p, uint8_t *q, const fl
         if constexpr (kIsFp8<T>) {
           v0 *= a_s;
           v1 *= a_s;
+        }
+        if constexpr (kIsE5M2<T>) {         // the fp8 dgrad: times the weight scale of column col
+          const float2 sc = *reinterpret_cast<const float2 *>(p.scale + col);
+          v0 *= sc.x;
+          v1 *= sc.y;
         }
         if constexpr (EPI) {
           // plain loads, ordered after the previous pair's store: the compiler then cannot hoist
@@ -839,6 +851,10 @@ static int run_fwd(int dtype, FwdParams p, cudaStream_t stream, int out_dtype = 
     return dtype == MEB200_BF16 ? dispatch_fwd_q<__nv_bfloat16>(qp, slices, stream)
                                 : dispatch_fwd_q<__half>(qp, slices, stream);
   }
+  if (dtype == kOperandE5M2E4M3) {    // the fp8 dgrad: column scales, no epilogue, no shadow
+    return out_dtype == MEB200_F16 ? dispatch_fwd<__nv_fp8_e5m2, false, __half>(p, slices, stream)
+                                   : dispatch_fwd<__nv_fp8_e5m2, false, __nv_bfloat16>(p, slices, stream);
+  }
   if (dtype == kOperandE4M3) {        // always with the epilogue; fp32 output through out_f32
     return out_dtype == MEB200_F16 ? dispatch_fwd<__nv_fp8_e4m3, true, __half>(p, slices, stream)
                                    : dispatch_fwd<__nv_fp8_e4m3, true, __nv_bfloat16>(p, slices, stream);
@@ -857,7 +873,7 @@ static int run_fwd(int dtype, FwdParams p, cudaStream_t stream, int out_dtype = 
 static void set_epilogue(FwdParams &p, const meb200_conv_epilogue *epi, uint32_t n0, size_t out_esz) {
   if (epi == nullptr) return;
   p.scale = epi->scale + n0;
-  p.shift = epi->shift + n0;
+  p.shift = epi->shift != nullptr ? epi->shift + n0 : nullptr;     // (the fp8 dgrad has none)
   p.res = epi->residual != nullptr ? reinterpret_cast<const uint8_t *>(epi->residual) + n0 * out_esz
                                    : nullptr;
   p.relu = epi->relu != 0;
@@ -938,7 +954,7 @@ static int run_wgrad(int dtype, WgParams p, uint32_t K_grid, uint32_t est_stages
 
 // ---- forward / dgrad ----------------------------------------------------------------------------
 static uint32_t operand_bytes(int dtype) {
-  return dtype == MEB200_TF32 ? 4 : (dtype == kOperandE4M3 ? 1 : 2);
+  return dtype == MEB200_TF32 ? 4 : (dtype == kOperandE4M3 || dtype == kOperandE5M2E4M3 ? 1 : 2);
 }
 
 bool conv_fp8_supported(uint32_t c_in, uint32_t c_out) {
@@ -958,11 +974,12 @@ int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, c
                     uint32_t n_rows, void *out, int out_dtype, const meb200_conv_epilogue *epi,
                     cudaStream_t stream, const float *a_scale, const Shadow *shadow) {
   if (n_rows == 0) return MEB200_OK;
-  const bool fp8 = dtype == kOperandE4M3;
+  const bool fp8 = dtype == kOperandE4M3 || dtype == kOperandE5M2E4M3;
   MEB_CHECK_ARG(fp8 ? conv_fp8_supported(c_reduce, c_cols) && epi != nullptr && a_scale != nullptr
                     : conv_tc_supported(dtype, c_reduce, c_cols),
                 "shape not supported by tc path");
-  MEB_CHECK_ARG(shadow == nullptr || (epi != nullptr && dtype != MEB200_TF32),
+  MEB_CHECK_ARG(shadow == nullptr || (epi != nullptr && dtype != MEB200_TF32 &&
+                                       dtype != kOperandE5M2E4M3),
                 "shadow: 16-bit or e4m3 operands with an epilogue");
   if (!aligned(16, A, B)) {
     set_error("conv tc: operands must be 16-byte aligned");

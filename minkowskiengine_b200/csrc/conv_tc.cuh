@@ -11,6 +11,9 @@ bool conv_tc_supported(int dtype, uint32_t c_reduce, uint32_t c_cols);
 // Operand code of the e4m3 forward (internal: not a feature dtype of the ABI).  Grid: whole 32-byte
 // k-steps of the reduction, output columns in multiples of 16.
 constexpr int kOperandE4M3 = 100;
+// Operand pair of the fp8 dgrad: A e5m2 (the gradient), B e4m3 (the weights); the same grid.  The
+// kernel multiplies column c by epi->scale[c] after *a_scale and runs no other epilogue.
+constexpr int kOperandE5M2E4M3 = 101;
 bool conv_fp8_supported(uint32_t c_in, uint32_t c_out);
 bool conv_wgrad_tc_supported(int dtype, uint32_t c_in, uint32_t c_out);
 
@@ -40,9 +43,17 @@ int conv_forward_tc(const void *A, int dtype, uint32_t n_a, uint32_t c_reduce, c
 int conv_pack_weights_e4m3(const float *W, uint32_t K, uint32_t c_in, uint32_t c_out, void *w_t,
                            float *w_scale, cudaStream_t stream);
 
-// Per-tensor e4m3 quantisation of [n, c] features (meb200_quantize_e4m3).
+// fp32 W [K, c_in, c_out] -> w_c [K, c_in, c_out] in e4m3 with a scale per input channel (the
+// dgrad's output column), amax over (k, co), by the formula of conv_pack_weights_e4m3.
+int conv_pack_weights_e4m3_dgrad(const float *W, uint32_t K, uint32_t c_in, uint32_t c_out,
+                                 void *w_c, float *w_scale, cudaStream_t stream);
+
+// Per-tensor e4m3 / e5m2 quantisation of [n, c] features (meb200_quantize_e4m3 / _e5m2); both
+// use the same zero-filled workspace.
 uint64_t quantize_e4m3_workspace_bytes();
 int quantize_e4m3(const void *in, int dtype, uint64_t count, void *out, float *scale, void *workspace,
+                  cudaStream_t stream);
+int quantize_e5m2(const void *in, int dtype, uint64_t count, void *out, float *scale, void *workspace,
                   cudaStream_t stream);
 // Static scales (meb200_amax_accumulate, meb200_e4m3_scales, meb200_quantize_e4m3_static).
 int amax_accumulate(const void *in, int dtype, uint64_t count, float *amax, cudaStream_t stream);

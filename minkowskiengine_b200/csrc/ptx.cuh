@@ -143,6 +143,25 @@ __device__ __forceinline__ void wgmma_64_e4m3(float (&d)[32], uint64_t da, uint6
                "%32, %33, p, 1, 1;\n\t}"
                : MEB_F8(d, 0), MEB_F8(d, 8), MEB_F8(d, 16), MEB_F8(d, 24) : "l"(da), "l"(db), "r"(1));
 }
+// e5m2 A times e4m3 B (the fp8 dgrad: gradients against weights), the same shapes and layouts.
+__device__ __forceinline__ void wgmma_16_e5m2e4m3(float (&d)[8], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k32.f32.e5m2.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7}, "
+               "%8, %9, p, 1, 1;\n\t}"
+               : MEB_F8(d, 0) : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_32_e5m2e4m3(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k32.f32.e5m2.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+               "%16, %17, p, 1, 1;\n\t}"
+               : MEB_F8(d, 0), MEB_F8(d, 8) : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_64_e5m2e4m3(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k32.f32.e5m2.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+               "%32, %33, p, 1, 1;\n\t}"
+               : MEB_F8(d, 0), MEB_F8(d, 8), MEB_F8(d, 16), MEB_F8(d, 24) : "l"(da), "l"(db), "r"(1));
+}
 #undef MEB_F8
 template <int N>
 __device__ __forceinline__ void wgmma_e4m3(float (&d)[N / 2], uint64_t da, uint64_t db) {
@@ -151,12 +170,25 @@ __device__ __forceinline__ void wgmma_e4m3(float (&d)[N / 2], uint64_t da, uint6
   else if constexpr (N == 32) wgmma_32_e4m3(d, da, db);
   else wgmma_64_e4m3(d, da, db);
 }
+template <int N>
+__device__ __forceinline__ void wgmma_e5m2e4m3(float (&d)[N / 2], uint64_t da, uint64_t db) {
+  static_assert(N == 16 || N == 32 || N == 64, "wgmma: N is 16, 32 or 64");
+  if constexpr (N == 16) wgmma_16_e5m2e4m3(d, da, db);
+  else if constexpr (N == 32) wgmma_32_e5m2e4m3(d, da, db);
+  else wgmma_64_e5m2e4m3(d, da, db);
+}
 
 // fp32 pair -> two e4m3 bytes (lo = a), rounded to nearest even; |x| past 448 (inf included)
 // saturates to +-448, NaN stays NaN
 __device__ __forceinline__ uint16_t e4m3x2_satfinite(float a, float b) {
   uint16_t r;
   asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(b), "f"(a));
+  return r;
+}
+// fp32 pair -> two e5m2 bytes (lo = a), the same rounding; saturates to +-57344
+__device__ __forceinline__ uint16_t e5m2x2_satfinite(float a, float b) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(r) : "f"(b), "f"(a));
   return r;
 }
 

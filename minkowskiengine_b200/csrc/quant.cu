@@ -1,7 +1,9 @@
-// fp8 (e4m3) operands of the inference forward (meb200_conv_forward_fp8): per-tensor quantisation of
-// the features and per-output-channel quantisation of the weights.
+// fp8 operands of the e4m3 forward (meb200_conv_forward_fp8): per-tensor quantisation of the features
+// and per-output-channel quantisation of the weights; and of the fp8 dgrad (meb200_conv_dgrad_fp8):
+// per-tensor e5m2 quantisation of the output gradient and per-input-channel e4m3 weights.
 //
-// Both use the same arithmetic, so that a torch expression reproduces the bytes exactly:
+// All use the same arithmetic, so that a torch expression reproduces the bytes exactly (e4m3 below;
+// e5m2 the same with 57344, its largest finite value, in place of 448):
 //   amax  = max |x| over the finite values (a max is exact and order-free: deterministic)
 //   scale = amax / 448, inv = 448 / amax                 (both IEEE divisions, rounded to nearest)
 //           scale = inv = 1 when amax = 0
@@ -20,26 +22,41 @@
 
 namespace meb200 {
 
-constexpr float kE4M3Max = 448.f;
 constexpr uint32_t kQThreads = 256;
 constexpr uint32_t kQMaxCtas = 1024;
 
+// The two fp8 formats: the largest finite value, and the saturating conversion of a pair (lo = a)
+struct E4M3 {
+  static constexpr float kMax = 448.f;
+  static __device__ __forceinline__ uint16_t cvt2(float a, float b) {
+    return ptx::e4m3x2_satfinite(a, b);
+  }
+};
+struct E5M2 {
+  static constexpr float kMax = 57344.f;
+  static __device__ __forceinline__ uint16_t cvt2(float a, float b) {
+    return ptx::e5m2x2_satfinite(a, b);
+  }
+};
+
 // scale and inv of a tensor (or column) whose finite values have the maximum magnitude amax
-__device__ __forceinline__ void e4m3_scales(float amax, float &scale, float &inv) {
+template <typename F>
+__device__ __forceinline__ void fp8_scales(float amax, float &scale, float &inv) {
   if (amax == 0.f) {
     scale = inv = 1.f;
-  } else if (isinf(inv = __fdiv_rn(kE4M3Max, amax))) {
+  } else if (isinf(inv = __fdiv_rn(F::kMax, amax))) {
     inv = FLT_MAX;
     scale = __fdiv_rn(1.f, FLT_MAX);
   } else {
-    scale = __fdiv_rn(amax, kE4M3Max);
+    scale = __fdiv_rn(amax, F::kMax);
   }
 }
 
 __device__ __forceinline__ float finite_abs(float v) { return isfinite(v) ? fabsf(v) : 0.f; }
 
-__device__ __forceinline__ uint8_t e4m3_byte(float x, float inv) {
-  return (uint8_t)(ptx::e4m3x2_satfinite(__fmul_rn(x, inv), 0.f) & 0xFFu);
+template <typename F>
+__device__ __forceinline__ uint8_t fp8_byte(float x, float inv) {
+  return (uint8_t)(F::cvt2(__fmul_rn(x, inv), 0.f) & 0xFFu);
 }
 
 // Launch 1: per-CTA max of |x| over the finite values, combined with an atomic max on the fp32 bits
@@ -72,7 +89,7 @@ __device__ __forceinline__ bool cta_amax(const T *__restrict__ x, uint64_t count
   return true;
 }
 
-template <typename T, bool VEC>
+template <typename T, bool VEC, typename F>
 __global__ void __launch_bounds__(kQThreads) k_amax(const T *__restrict__ x, uint64_t count,
                                                    float *__restrict__ scale, uint32_t *ws) {
   float m;
@@ -82,13 +99,13 @@ __global__ void __launch_bounds__(kQThreads) k_amax(const T *__restrict__ x, uin
   if (atomicInc(ws + 1, gridDim.x - 1) != gridDim.x - 1) return;
   const float amax = __uint_as_float(atomicExch(ws, 0u));  // every CTA's max has landed
   float s, inv;
-  e4m3_scales(amax, s, inv);
+  fp8_scales<F>(amax, s, inv);
   scale[0] = s;
   scale[1] = inv;
 }
 
-// Launch 2: q = e4m3(x * inv), 16 elements (16 output bytes) per thread and step.
-template <typename T, bool VEC>
+// Launch 2: q = fp8(x * inv), 16 elements (16 output bytes) per thread and step.
+template <typename T, bool VEC, typename F>
 __global__ void __launch_bounds__(kQThreads) k_quant(const T *__restrict__ x, uint64_t count,
                                                     const float *__restrict__ scale,
                                                     uint8_t *__restrict__ q) {
@@ -106,7 +123,7 @@ __global__ void __launch_bounds__(kQThreads) k_quant(const T *__restrict__ x, ui
 #pragma unroll
         for (uint32_t j = 0; j < V; j += 2) {
           const uint32_t e = h * V + j;           // element of the 16: byte e of the store
-          const uint32_t b = ptx::e4m3x2_satfinite(__fmul_rn(f[j], inv), __fmul_rn(f[j + 1], inv));
+          const uint32_t b = F::cvt2(__fmul_rn(f[j], inv), __fmul_rn(f[j + 1], inv));
           if (e % 4 == 0) w[e / 4] = b; else w[e / 4] |= b << 16;
         }
       }
@@ -114,10 +131,10 @@ __global__ void __launch_bounds__(kQThreads) k_quant(const T *__restrict__ x, ui
     }
     if (blockIdx.x == 0)
       for (uint64_t i = n16 * 16 + threadIdx.x; i < count; i += blockDim.x)
-        q[i] = e4m3_byte(to_f32<T>(x[i]), inv);
+        q[i] = fp8_byte<F>(to_f32<T>(x[i]), inv);
   } else {
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count; i += stride)
-      q[i] = e4m3_byte(to_f32<T>(x[i]), inv);
+      q[i] = fp8_byte<F>(to_f32<T>(x[i]), inv);
   }
 }
 
@@ -128,8 +145,9 @@ static uint32_t quant_ctas(uint64_t count) {
                                       std::min<uint32_t>(kQMaxCtas, 4 * num_sms()));
 }
 
-int quantize_e4m3(const void *in, int dtype, uint64_t count, void *out, float *scale,
-                  void *workspace, cudaStream_t stream) {
+template <typename F>
+static int quantize_dynamic(const void *in, int dtype, uint64_t count, void *out, float *scale,
+                            void *workspace, cudaStream_t stream) {
   const bool vec = aligned(16, in, out);
   const uint32_t ctas = quant_ctas(count);
   uint32_t *ws = reinterpret_cast<uint32_t *>(workspace);
@@ -137,17 +155,27 @@ int quantize_e4m3(const void *in, int dtype, uint64_t count, void *out, float *s
   MEB_DISPATCH_DTYPE(dtype, {
     const T *x = reinterpret_cast<const T *>(in);
     if (vec) {
-      k_amax<T, true><<<ctas, kQThreads, 0, stream>>>(x, count, scale, ws);
+      k_amax<T, true, F><<<ctas, kQThreads, 0, stream>>>(x, count, scale, ws);
       MEB_LAUNCH_OK();
-      k_quant<T, true><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
+      k_quant<T, true, F><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
     } else {
-      k_amax<T, false><<<ctas, kQThreads, 0, stream>>>(x, count, scale, ws);
+      k_amax<T, false, F><<<ctas, kQThreads, 0, stream>>>(x, count, scale, ws);
       MEB_LAUNCH_OK();
-      k_quant<T, false><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
+      k_quant<T, false, F><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
     }
     MEB_LAUNCH_OK();
   });
   return MEB200_OK;
+}
+
+int quantize_e4m3(const void *in, int dtype, uint64_t count, void *out, float *scale,
+                  void *workspace, cudaStream_t stream) {
+  return quantize_dynamic<E4M3>(in, dtype, count, out, scale, workspace, stream);
+}
+
+int quantize_e5m2(const void *in, int dtype, uint64_t count, void *out, float *scale,
+                  void *workspace, cudaStream_t stream) {
+  return quantize_dynamic<E5M2>(in, dtype, count, out, scale, workspace, stream);
 }
 
 // ---- static scales --------------------------------------------------------------------------------
@@ -162,7 +190,7 @@ __global__ void __launch_bounds__(kQThreads) k_amax_acc(const T *__restrict__ x,
 
 __global__ void k_scales(const float *__restrict__ amax, float *__restrict__ scale) {
   float s, inv;
-  e4m3_scales(*amax, s, inv);
+  fp8_scales<E4M3>(*amax, s, inv);
   scale[0] = s;
   scale[1] = inv;
 }
@@ -193,8 +221,8 @@ int quantize_e4m3_static(const void *in, int dtype, uint64_t count, void *out, c
   uint8_t *q = reinterpret_cast<uint8_t *>(out);
   MEB_DISPATCH_DTYPE(dtype, {
     const T *x = reinterpret_cast<const T *>(in);
-    if (aligned(16, in, out)) k_quant<T, true><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
-    else k_quant<T, false><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
+    if (aligned(16, in, out)) k_quant<T, true, E4M3><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
+    else k_quant<T, false, E4M3><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
     MEB_LAUNCH_OK();
   });
   return MEB200_OK;
@@ -220,7 +248,7 @@ __global__ void __launch_bounds__(256) k_pack_w_e4m3(const float *__restrict__ W
   if (ty == 0) {
     for (uint32_t i = 1; i < 8; ++i) m = fmaxf(m, tile[i][tx]);
     float s, inv;
-    e4m3_scales(m, s, inv);
+    fp8_scales<E4M3>(m, s, inv);
     inv_s[tx] = inv;
     if (co < c_out) w_scale[co] = s;
   }
@@ -233,7 +261,7 @@ __global__ void __launch_bounds__(256) k_pack_w_e4m3(const float *__restrict__ W
       __syncthreads();
       for (uint32_t i = ty; i < 32; i += 8)
         if (co0 + i < c_out && ci0 + tx < c_in)
-          Wt[base + (size_t)(co0 + i) * c_in + ci0 + tx] = e4m3_byte(tile[tx][i], inv_s[i]);
+          Wt[base + (size_t)(co0 + i) * c_in + ci0 + tx] = fp8_byte<E4M3>(tile[tx][i], inv_s[i]);
       __syncthreads();
     }
 }
@@ -242,6 +270,47 @@ int conv_pack_weights_e4m3(const float *W, uint32_t K, uint32_t c_in, uint32_t c
                            float *w_scale, cudaStream_t stream) {
   k_pack_w_e4m3<<<cdiv(c_out, 32), 256, 0, stream>>>(W, K, c_in, c_out,
                                                      reinterpret_cast<uint8_t *>(w_t), w_scale);
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
+}
+
+// The dgrad's weights: one CTA per input channel ci.  The amax of row ci over all (k, co) (thread
+// phases combined with fmaxf: order-free), then the row's bytes in place, [K, c_in, c_out].
+__global__ void __launch_bounds__(256) k_pack_w_e4m3_dgrad(const float *__restrict__ W, uint32_t K,
+                                                           uint32_t c_in, uint32_t c_out,
+                                                           uint8_t *__restrict__ Wc,
+                                                           float *__restrict__ w_scale) {
+  __shared__ float wm[8];
+  __shared__ float inv_s;
+  const uint32_t ci = blockIdx.x;
+  float m = 0.f;
+  for (uint32_t k = 0; k < K; ++k)
+    for (uint32_t co = threadIdx.x; co < c_out; co += 256)
+      m = fmaxf(m, finite_abs(W[((size_t)k * c_in + ci) * c_out + co]));
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, d));
+  if ((threadIdx.x & 31) == 0) wm[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (uint32_t w = 1; w < 8; ++w) m = fmaxf(m, wm[w]);
+    float s, inv;
+    fp8_scales<E4M3>(m, s, inv);
+    w_scale[ci] = s;
+    inv_s = inv;
+  }
+  __syncthreads();
+  const float inv = inv_s;
+  for (uint32_t k = 0; k < K; ++k)
+    for (uint32_t co = threadIdx.x; co < c_out; co += 256) {
+      const size_t e = ((size_t)k * c_in + ci) * c_out + co;
+      Wc[e] = fp8_byte<E4M3>(W[e], inv);
+    }
+}
+
+int conv_pack_weights_e4m3_dgrad(const float *W, uint32_t K, uint32_t c_in, uint32_t c_out,
+                                 void *w_c, float *w_scale, cudaStream_t stream) {
+  k_pack_w_e4m3_dgrad<<<c_in, 256, 0, stream>>>(W, K, c_in, c_out, reinterpret_cast<uint8_t *>(w_c),
+                                                w_scale);
   MEB_LAUNCH_OK();
   return MEB200_OK;
 }
