@@ -354,6 +354,32 @@ int meb200_conv_dgrad_fp8(const void *grad_e5m2, const float *g_scale, uint32_t 
                           uint32_t c_in, const int32_t *in_nbr, uint32_t n_in, void *grad_in,
                           int grad_in_dtype, const int32_t *in_order, void *stream);
 
+/* ---- fp8 training: the weight gradient on e4m3 x e5m2 ------------------------------------------
+ * The wgrad of a convolution (meb200_conv_backward's grad_weight) on the Hopper fp8 tensor cores,
+ * from the operands the forward and the dgrad already quantised: the input in e4m3 and the output
+ * gradient in e5m2, each with one scale per tensor:
+ *   grad_weight[k, ci, co] = (acc[k, ci, co] * a_scale) * g_scale   (fp32, fully written)
+ * with acc the sum over the pairs of offset k of in_e4m3[i, ci] * grad_e5m2[o, co].  Every interval
+ * of at most 128 pairs is summed by the tensor cores from zero and then added into fp32, so the
+ * error does not grow with the number of pairs (DESIGN.md §3, "fp8 training").
+ *   in_e4m3 [n_in, c_in], a_scale: meb200_quantize_e4m3 (a_scale the DEVICE dequantisation factor)
+ *   grad_e5m2 [n_out, c_out], g_scale: meb200_quantize_e5m2
+ *   pairs_in / pairs_out / seg_start / n_chunks: the pair lists of meb200_conv_backward (required)
+ *   workspace: meb200_conv_wgrad_fp8_workspace_bytes(n_out, c_in, c_out, K) bytes, 16-byte aligned;
+ *              as in meb200_conv_backward, less, NULL or unaligned means fewer row splits, and the
+ *              splits are added in a fixed order (bit-identical run to run)
+ * Grid (meb200_conv_wgrad_fp8_supported): c_in and c_out multiples of 32 up to 1024, 1 <= K <= 1023;
+ * off it the call returns MEB200_ERR_UNSUPPORTED and launches nothing.  n_out = 0: zero, no MMA. */
+int meb200_conv_wgrad_fp8_supported(uint32_t c_in, uint32_t c_out, uint32_t K);
+uint64_t meb200_conv_wgrad_fp8_workspace_bytes(uint32_t n_out, uint32_t c_in, uint32_t c_out,
+                                               uint32_t K);
+int meb200_conv_wgrad_fp8(const void *in_e4m3, const float *a_scale, const void *grad_e5m2,
+                          const float *g_scale, uint32_t c_in, uint32_t K, uint32_t c_out,
+                          const int32_t *pairs_in, const int32_t *pairs_out,
+                          const int32_t *seg_start, uint32_t n_chunks, uint32_t n_out,
+                          float *grad_weight, void *workspace, uint64_t workspace_bytes,
+                          void *stream);
+
 /* Weight packing, once per optimizer step instead of once per call: fp32 master weight
  * [K, Cin, Cout] -> `dtype` (BF16/F16, or TF32: fp32 words rounded to tf32) operand copies
  * w_cast [K, Cin, Cout] and w_t [K, Cout, Cin].  The reference keeps weights in the feature dtype and needs no such step

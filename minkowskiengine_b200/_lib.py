@@ -68,6 +68,10 @@ PROTOTYPES = {
     "meb200_conv_pack_weights_e4m3_dgrad": (_i32, [_vp, _u32, _u32, _u32, _vp, _vp, _vp]),
     "meb200_conv_dgrad_fp8": (_i32, [_vp, _vp, _u32, _u32, _vp, _vp, _u32, _u32, _vp, _u32, _vp,
                                      _i32, _vp, _vp]),
+    "meb200_conv_wgrad_fp8_supported": (_i32, [_u32, _u32, _u32]),
+    "meb200_conv_wgrad_fp8_workspace_bytes": (_u64, [_u32, _u32, _u32, _u32]),
+    "meb200_conv_wgrad_fp8": (_i32, [_vp, _vp, _vp, _vp, _u32, _u32, _u32, _vp, _vp, _vp, _u32,
+                                     _u32, _vp, _vp, _u64, _vp]),
     "meb200_conv_pack_weights": (_i32, [_vp, _u32, _u32, _u32, _i32, _vp, _vp, _vp]),
     "meb200_conv_pack_weights_batched": (_i32, [_vp, _u32, _u32, _i32, _vp]),
     "meb200_conv_stem_virtual_channels": (_u32, [_u32]),

@@ -1223,7 +1223,8 @@ def _workspace(n_out, c_in, c_out, K, code, device):
 
 
 # ---- live per-kernel timing for bench.py's roofline (CUDA events on the launch stream) ------
-_PROFILE = None   # None, or {"conv_fwd_dgrad": [...], "conv_wgrad": [...], "kernel_map": [...]}
+_PROFILE = None   # None, or {"conv_fwd_dgrad": [...], "conv_wgrad": [...], "conv_wgrad_fp8": [...],
+#                   "kernel_map": [...]}
 
 
 def _record(kind, fn, flops, nbytes, always=False):
@@ -1244,7 +1245,7 @@ def profile_conv_kernels(step_fn, steps=2):
     returns, per kernel family, the summed device time and ALGORITHMIC work:
     flops = 2*P*Cin*Cout per launch, bytes = the compulsory traffic of SURVEY.md §8d."""
     global _PROFILE
-    _PROFILE = {"conv_fwd_dgrad": [], "conv_wgrad": [], "kernel_map": []}
+    _PROFILE = {"conv_fwd_dgrad": [], "conv_wgrad": [], "conv_wgrad_fp8": [], "kernel_map": []}
     try:
         for _ in range(steps):
             step_fn()
@@ -1650,22 +1651,40 @@ FP8_DGRAD = "e4m3_dgrad"      # the packed-weight cache's operand of the dgrad's
 
 
 @contextlib.contextmanager
-def fp8_training():
+def fp8_training(*, weight_gradient=False):
     """Within the block, training sparse convolutions run their forward and input gradient on the
     Hopper fp8 tensor cores where they can (a gradient needed, c_in and c_out multiples of 32 up to
     1024, not a K = 1 stride-1 matrix product): the forward on e4m3 features and weights, the input
     gradient on the output gradient in e5m2 against e4m3 weights.  The weight gradient and every
     other layer run as they do outside the block.  Thread-local, and nestable with fp8_inference()
-    either way."""
-    _FP8_STATE.train_depth = getattr(_FP8_STATE, "train_depth", 0) + 1
+    either way.
+
+    weight_gradient=True: the selected layers also run their weight gradient on fp8, the e4m3 input
+    of the forward times the e5m2 output gradient of the input gradient (layers with over 1023
+    kernel offsets keep the weight gradient of the feature dtype).  Forward outputs and input
+    gradients are those of weight_gradient=False, bit for bit.  Nested blocks: the innermost
+    decides."""
+    modes = _FP8_STATE.__dict__.setdefault("train_modes", [])
+    modes.append(bool(weight_gradient))
     try:
         yield
     finally:
-        _FP8_STATE.train_depth -= 1
+        modes.pop()
 
 
 def fp8_training_enabled():
-    return getattr(_FP8_STATE, "train_depth", 0) > 0
+    return bool(getattr(_FP8_STATE, "train_modes", None))
+
+
+def fp8_training_weight_gradient():
+    """Whether the innermost fp8_training() block of this thread runs weight gradients on fp8."""
+    modes = getattr(_FP8_STATE, "train_modes", None)
+    return bool(modes) and modes[-1]
+
+
+def fp8_wgrad_supported(c_in, c_out, K):
+    """Whether the fp8 weight gradient (meb200_conv_wgrad_fp8) takes a layer of this shape."""
+    return bool(_lib.load().meb200_conv_wgrad_fp8_supported(c_in, c_out, K))
 
 
 def _fp8_dgrad_weights(kernel):
@@ -1688,21 +1707,74 @@ def _fp8_dgrad_weights(kernel):
     return packed
 
 
-def _conv_dgrad_fp8(grad_out, kernel, km, dtype):
+def _conv_dgrad_fp8(grad_out, kernel, km, dtype, grad_q=None):
     """The input gradient in `dtype` on the fp8 tensor cores (meb200_conv_dgrad_fp8): grad_out (in
-    `dtype`, contiguous) quantised to e5m2 at its amax, the weights from _fp8_dgrad_weights."""
+    `dtype`, contiguous) quantised to e5m2 at its amax, the weights from _fp8_dgrad_weights.
+    grad_q: grad_out already quantised, (e5m2 bytes, fp32 [2] scale), or None: quantised here."""
     K, c_in, c_out = kernel.shape
     _assert(K == km.K, "kernel volume", K, "does not match the kernel map", km.K)
     if km.n_out == 0 or km.n_in == 0:      # no output rows: no neighbour contributes
         return torch.zeros((km.n_in, c_in), dtype=dtype, device=grad_out.device)
     grad_in = torch.empty((km.n_in, c_in), dtype=dtype, device=grad_out.device)
     w_c, w_scale = _fp8_dgrad_weights(kernel)
-    q, g_scale = _quantize_dynamic(grad_out, "meb200_quantize_e5m2")
+    q, g_scale = grad_q if grad_q is not None else _quantize_dynamic(grad_out, "meb200_quantize_e5m2")
     _lib.check(_lib.load().meb200_conv_dgrad_fp8(
         _lib.ptr(q), _lib.ptr(g_scale), km.n_out, c_out, _lib.ptr(w_c), _lib.ptr(w_scale), K, c_in,
         _lib.ptr(km.in_nbr), km.n_in, _lib.ptr(grad_in), _lib.dtype_code(dtype),
         _lib.ptr(km.in_order), _lib.current_stream()))
     return grad_in
+
+
+def _conv_wgrad_fp8(act, grad_q, kernel, km):
+    """The weight gradient on the fp8 tensor cores (meb200_conv_wgrad_fp8), in the kernel's dtype:
+    act = (e4m3 bytes [n_in, c_in], fp32 [2] scale) the forward multiplied, grad_q = (e5m2 bytes
+    [n_out, c_out], fp32 [2] scale) the dgrad multiplied, over the map's pair lists.  An empty map
+    gives zero without a launch."""
+    K, c_in, c_out = kernel.shape
+    _assert(K == km.K, "kernel volume", K, "does not match the kernel map", km.K)
+    if km.n_out == 0 or km.n_in == 0:
+        return torch.zeros((K, c_in, c_out), dtype=kernel.dtype, device=kernel.device)
+    lib = _lib.load()
+    q, a_scale = act
+    g, g_scale = grad_q
+    grad_w = torch.empty((K, c_in, c_out), dtype=torch.float32, device=kernel.device)
+    pin, pout, seg, nch = km.pair_lists()
+    nbytes = int(lib.meb200_conv_wgrad_fp8_workspace_bytes(km.n_out, c_in, c_out, K))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=kernel.device) if nbytes else None
+    _lib.check(lib.meb200_conv_wgrad_fp8(
+        _lib.ptr(q), _lib.ptr(a_scale), _lib.ptr(g), _lib.ptr(g_scale), c_in, K, c_out,
+        _lib.ptr(pin), _lib.ptr(pout), _lib.ptr(seg), nch, km.n_out, _lib.ptr(grad_w), _lib.ptr(ws),
+        nbytes, _lib.current_stream()))
+    return grad_w if grad_w.dtype == kernel.dtype else grad_w.to(kernel.dtype)
+
+
+def _conv_backward_fp8w(act, dtype, grad_out, kernel, km, need_in=True, need_w=True):
+    """(grad_in or None, grad_w or None) of a layer run in fp8_training(weight_gradient=True), from
+    act = (e4m3 bytes, scale) of its forward and its feature dtype: grad_out quantised to e5m2 once,
+    for the input gradient (_conv_dgrad_fp8, as in fp8_training()) and the weight gradient
+    (_conv_wgrad_fp8)."""
+    if grad_out.dtype != dtype:
+        grad_out = grad_out.to(dtype)
+    grad_out = grad_out.contiguous()
+    grad_q = None
+    if km.n_out > 0 and km.n_in > 0:
+        grad_q = _quantize_dynamic(grad_out, "meb200_quantize_e5m2")
+    if _PROFILE is None:
+        return (_conv_dgrad_fp8(grad_out, kernel, km, dtype, grad_q) if need_in else None,
+                _conv_wgrad_fp8(act, grad_q, kernel, km) if need_w else None)
+    K, c_in, c_out = kernel.shape
+    P = km.n_pairs
+    flops = 2.0 * P * c_in * c_out
+    gi = gw = None
+    esz = torch.empty((), dtype=dtype).element_size()
+    if need_in:
+        nb = km.n_out * c_out * esz + km.n_in * c_in * esz + K * c_in * c_out * esz + P * 8
+        gi = _record("conv_fwd_dgrad", lambda: _conv_dgrad_fp8(grad_out, kernel, km, dtype, grad_q),
+                     flops, nb)
+    if need_w:    # e4m3 in and e5m2 dOut, dW (fp32) out, pairs
+        nb = km.n_in * c_in + km.n_out * c_out + K * c_in * c_out * 4 + P * 8
+        gw = _record("conv_wgrad_fp8", lambda: _conv_wgrad_fp8(act, grad_q, kernel, km), flops, nb)
+    return gi, gw
 
 
 def _pad4(feat):
@@ -1883,13 +1955,18 @@ def ConvolutionForwardGPU(in_feat, kernel, kernel_size, kernel_stride, kernel_di
 
 def ConvolutionBackwardGPU(in_feat, grad_out_feat, kernel, kernel_size, kernel_stride,
                            kernel_dilation, region_type, offset, convolution_mode, in_key,
-                           out_key, manager, need_in=True, need_w=True, fp8=False):
-    """reference: ConvolutionBackwardGPU src/convolution_gpu.cu:161-244.  fp8: as _conv_backward_impl."""
-    _check_feats(in_feat, manager, in_key)
+                           out_key, manager, need_in=True, need_w=True, fp8=False, act=None):
+    """reference: ConvolutionBackwardGPU src/convolution_gpu.cu:161-244.  fp8: as _conv_backward_impl.
+    act: (e4m3 bytes, fp32 [2] scale, feature dtype) of the input of a layer run in
+    fp8_training(weight_gradient=True), in place of in_feat (None): both gradients on fp8
+    (_conv_backward_fp8w)."""
+    _check_feats(in_feat if act is None else act[0], manager, in_key)
     _assert(manager.exists(out_key), ERROR_MAP_NOT_FOUND)
     _assert(grad_out_feat.size(0) == manager.size(out_key), "Invalid grad_out size")
     km = manager._kernel_map(in_key, out_key, kernel_size, kernel_stride, kernel_dilation,
                              region_type, offset, False, False)
+    if act is not None:
+        return _conv_backward_fp8w(act[:2], act[2], grad_out_feat, kernel, km, need_in, need_w)
     return _conv_backward(in_feat, grad_out_feat, kernel, km, need_in, need_w, fp8)
 
 
@@ -1912,11 +1989,15 @@ def ConvolutionTransposeForwardGPU(in_feat, kernel, kernel_size, kernel_stride,
 
 def ConvolutionTransposeBackwardGPU(in_feat, grad_out_feat, kernel, kernel_size, kernel_stride,
                                     kernel_dilation, region_type, offset, convolution_mode,
-                                    in_key, out_key, manager, need_in=True, need_w=True, fp8=False):
-    _check_feats(in_feat, manager, in_key)
+                                    in_key, out_key, manager, need_in=True, need_w=True, fp8=False,
+                                    act=None):
+    """`fp8`, `act`: as ConvolutionBackwardGPU."""
+    _check_feats(in_feat if act is None else act[0], manager, in_key)
     _assert(manager.exists(out_key), ERROR_MAP_NOT_FOUND)
     km = manager._kernel_map(in_key, out_key, kernel_size, kernel_stride, kernel_dilation,
                              region_type, offset, True, False)
+    if act is not None:
+        return _conv_backward_fp8w(act[:2], act[2], grad_out_feat, kernel, km, need_in, need_w)
     return _conv_backward(in_feat, grad_out_feat, kernel, km, need_in, need_w, fp8)
 
 

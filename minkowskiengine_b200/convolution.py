@@ -18,18 +18,31 @@ from .normalization import MinkowskiBatchNorm, _bn_tail, _eval_scale_shift, _nat
 from .sparse_tensor import SparseTensor, _get_coordinate_map_key
 
 
+def _fp8_input(ctx, input_features, fp8_wgrad):
+    """Saves what the backward reads of the input: with fp8_wgrad (fp8_training(weight_gradient=
+    True)) its e4m3 bytes and scale, which the forward multiplies (returned, for its `act`) and the
+    weight gradient reads, in place of the features; else the features (returns None)."""
+    if not fp8_wgrad:
+        ctx.input_features, ctx.act = input_features, None
+        return None
+    q, a_scale = _C._quantize_e4m3(input_features)
+    ctx.input_features, ctx.act = None, (q, a_scale, input_features.dtype)
+    return q, a_scale
+
+
 class MinkowskiConvolutionFunction(Function):
     @staticmethod
     def forward(ctx, input_features: torch.Tensor, kernel_weights: torch.Tensor,
                 kernel_generator: KernelGenerator, convolution_mode: ConvolutionMode,
                 in_coordinate_map_key: CoordinateMapKey,
                 out_coordinate_map_key: CoordinateMapKey = None,
-                coordinate_manager: CoordinateManager = None, fp8: bool = False):
+                coordinate_manager: CoordinateManager = None, fp8: bool = False,
+                fp8_wgrad: bool = False):
         if out_coordinate_map_key is None:
             out_coordinate_map_key = CoordinateMapKey(
                 in_coordinate_map_key.get_coordinate_size())
         input_features = input_features.contiguous()
-        ctx.input_features = input_features
+        act = _fp8_input(ctx, input_features, fp8_wgrad)
         ctx.kernel_weights = kernel_weights
         ctx.misc = (kernel_generator, convolution_mode, in_coordinate_map_key,
                     out_coordinate_map_key, coordinate_manager)
@@ -39,7 +52,7 @@ class MinkowskiConvolutionFunction(Function):
             kernel_generator.kernel_stride, kernel_generator.kernel_dilation,
             kernel_generator.region_type, kernel_generator.region_offsets,
             kernel_generator.expand_coordinates, convolution_mode, in_coordinate_map_key,
-            out_coordinate_map_key, coordinate_manager._manager, fp8=fp8)
+            out_coordinate_map_key, coordinate_manager._manager, fp8=fp8, act=act)
 
     @staticmethod
     def backward(ctx, grad_out_feat: torch.Tensor):
@@ -49,8 +62,9 @@ class MinkowskiConvolutionFunction(Function):
             ctx.input_features, grad_out_feat, ctx.kernel_weights, kgen.kernel_size,
             kgen.kernel_stride, kgen.kernel_dilation, kgen.region_type, kgen.region_offsets,
             mode, in_key, out_key, manager._manager,
-            need_in=ctx.needs_input_grad[0], need_w=ctx.needs_input_grad[1], fp8=ctx.fp8)
-        return grad_in_feat, grad_kernel, None, None, None, None, None, None
+            need_in=ctx.needs_input_grad[0], need_w=ctx.needs_input_grad[1], fp8=ctx.fp8,
+            act=ctx.act)
+        return grad_in_feat, grad_kernel, None, None, None, None, None, None, None
 
 
 class MinkowskiConvolutionTransposeFunction(Function):
@@ -59,12 +73,13 @@ class MinkowskiConvolutionTransposeFunction(Function):
                 kernel_generator: KernelGenerator, convolution_mode: ConvolutionMode,
                 in_coordinate_map_key: CoordinateMapKey,
                 out_coordinate_map_key: CoordinateMapKey = None,
-                coordinate_manager: CoordinateManager = None, fp8: bool = False):
+                coordinate_manager: CoordinateManager = None, fp8: bool = False,
+                fp8_wgrad: bool = False):
         if out_coordinate_map_key is None:
             out_coordinate_map_key = CoordinateMapKey(
                 in_coordinate_map_key.get_coordinate_size())
         input_features = input_features.contiguous()
-        ctx.input_features = input_features
+        act = _fp8_input(ctx, input_features, fp8_wgrad)
         ctx.kernel_weights = kernel_weights
         ctx.misc = (kernel_generator, convolution_mode, in_coordinate_map_key,
                     out_coordinate_map_key, coordinate_manager)
@@ -74,7 +89,7 @@ class MinkowskiConvolutionTransposeFunction(Function):
             kernel_generator.kernel_stride, kernel_generator.kernel_dilation,
             kernel_generator.region_type, kernel_generator.region_offsets,
             kernel_generator.expand_coordinates, convolution_mode, in_coordinate_map_key,
-            out_coordinate_map_key, coordinate_manager._manager, fp8=fp8)
+            out_coordinate_map_key, coordinate_manager._manager, fp8=fp8, act=act)
 
     @staticmethod
     def backward(ctx, grad_out_feat: torch.Tensor):
@@ -84,8 +99,9 @@ class MinkowskiConvolutionTransposeFunction(Function):
             ctx.input_features, grad_out_feat, ctx.kernel_weights, kgen.kernel_size,
             kgen.kernel_stride, kgen.kernel_dilation, kgen.region_type, kgen.region_offsets,
             mode, in_key, out_key, manager._manager,
-            need_in=ctx.needs_input_grad[0], need_w=ctx.needs_input_grad[1], fp8=ctx.fp8)
-        return grad_in_feat, grad_kernel, None, None, None, None, None, None
+            need_in=ctx.needs_input_grad[0], need_w=ctx.needs_input_grad[1], fp8=ctx.fp8,
+            act=ctx.act)
+        return grad_in_feat, grad_kernel, None, None, None, None, None, None, None
 
 
 class MinkowskiConvolutionBase(MinkowskiModuleBase):
@@ -142,10 +158,11 @@ class MinkowskiConvolutionBase(MinkowskiModuleBase):
             if observer is not None:
                 selected = _fp8_rule(self, input.F)
                 observer._observe(self, input, selected)
+            fp8 = _fp8_train(self, input.F)
             outfeat = self.conv.apply(input.F, self.kernel, self.kernel_generator,
                                       self.convolution_mode, input.coordinate_map_key,
-                                      out_coordinate_map_key, input._manager,
-                                      _fp8_train(self, input.F))
+                                      out_coordinate_map_key, input._manager, fp8,
+                                      fp8 and _fp8_train_wgrad(self))
         if self.bias is not None:
             outfeat = outfeat + self.bias.to(outfeat.dtype)
         out = SparseTensor(outfeat, coordinate_map_key=out_coordinate_map_key,
@@ -267,6 +284,14 @@ def _fp8_train(conv, feats):
     """Whether `conv` runs its forward on e4m3 and its input gradient on e5m2 x e4m3 operands
     (backend.fp8_training): inside the context, when _fp8_train_rule holds."""
     return _C.fp8_training_enabled() and _fp8_train_rule(conv, feats)
+
+
+def _fp8_train_wgrad(conv):
+    """Whether a layer fp8 training selected also runs its weight gradient on fp8: inside
+    fp8_training(weight_gradient=True) (the innermost block), when the fp8 wgrad takes its shape
+    (K <= 1023: the pair lists' limit; c_in and c_out are on the grid already)."""
+    return (_C.fp8_training_weight_gradient() and _C.fp8_wgrad_supported(
+        conv.in_channels, conv.out_channels, conv.kernel_generator.kernel_volume))
 
 
 def _fp8_train_rule(conv, feats):

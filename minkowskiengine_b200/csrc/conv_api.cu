@@ -178,6 +178,30 @@ int meb200_conv_dgrad_fp8(const void *grad_e5m2, const float *g_scale, uint32_t 
                          g_scale);
 }
 
+int meb200_conv_wgrad_fp8_supported(uint32_t c_in, uint32_t c_out, uint32_t K) {
+  return conv_wgrad_fp8_supported(c_in, c_out, K) ? 1 : 0;
+}
+
+uint64_t meb200_conv_wgrad_fp8_workspace_bytes(uint32_t n_out, uint32_t c_in, uint32_t c_out,
+                                               uint32_t K) {
+  return conv_wgrad_workspace_bytes(c_in, c_out, K, n_out);
+}
+
+int meb200_conv_wgrad_fp8(const void *in_e4m3, const float *a_scale, const void *grad_e5m2,
+                          const float *g_scale, uint32_t c_in, uint32_t K, uint32_t c_out,
+                          const int32_t *pairs_in, const int32_t *pairs_out,
+                          const int32_t *seg_start, uint32_t n_chunks, uint32_t n_out,
+                          float *grad_weight, void *workspace, uint64_t workspace_bytes,
+                          void *stream_) {
+  MEB_CHECK_ARG(grad_weight && a_scale && g_scale, "null buffer");
+  MEB_CHECK_ARG(n_out == 0 || (in_e4m3 && grad_e5m2 && pairs_in && pairs_out && seg_start &&
+                               n_chunks > 0),
+                "null buffer");
+  return conv_wgrad_fp8(in_e4m3, a_scale, grad_e5m2, g_scale, c_in, K, c_out, pairs_in, pairs_out,
+                        seg_start, n_chunks, n_out, grad_weight, workspace, workspace_bytes,
+                        (cudaStream_t)stream_);
+}
+
 int meb200_quantize_e4m3(const void *in, int dtype, uint32_t n, uint32_t c, void *out_e4m3,
                          float *scale_dev, void *workspace, void *stream_) {
   MEB_CHECK_ARG(dtype >= 0 && dtype <= 2, "dtype");

@@ -9,7 +9,9 @@
 // cannot read).  The forward also runs on e4m3 bytes (meb200_conv_forward_fp8:
 // k_conv_wg<__nv_fp8_e4m3, ..>, 32 channels per k-step, always with its epilogue), and the fp8
 // dgrad on e5m2 gradients against e4m3 weights (meb200_conv_dgrad_fp8: k_conv_wg<__nv_fp8_e5m2,
-// ..>, the same staging with the e5m2 x e4m3 MMA).  k_conv_wg_q is
+// ..>, the same staging with the e5m2 x e4m3 MMA), and the fp8 weight gradient on the e4m3 input
+// and the e5m2 gradient (meb200_conv_wgrad_fp8: k_wgrad_fp8, which transposes its gathered stages
+// in shared memory and promotes its sums to fp32 every 128 pairs).  k_conv_wg_q is
 // the forward with the epilogue that also stores an e4m3 shadow of its output (the _q entries).
 //
 // Replaces the reference's per-offset SIMT tile-matmul with per-element atomicAdd
@@ -681,6 +683,194 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_tf32(const WgParams p) {
     }
 }
 
+// fp8 wgrad: dW[k][ci][co] = (sum over the pairs of offset k of X[i][ci] * dY[o][co]) * a_scale *
+// g_scale, X the e4m3 input and dY the e5m2 output gradient of the layer, both quantised per
+// tensor.  Same units (offset, 128 input channels, share), shares (wg_range), split partials and
+// pair lists as k_wgrad_wg, over the column slice blockIdx.z % col_slices of NI * NT columns.
+//
+// fp8 wgmma reads K-major operands only, and a gathered pair row is MN-major (its channels are
+// contiguous), so each 64-pair stage is gathered row-major by cp.async as in k_wgrad_wg and then
+// transposed in shared memory: a thread takes 4 pairs x 4 channels (one 4-byte load from each of
+// four rows), regroups them with __byte_perm into one word per channel and stores the words into
+// the K-major core-matrix tile (tc::kWgFp8Sbo apart per 8 channels).  The MMAs of stage s read
+// tile s % 2 while the copies of stage s + 2 are in flight and stage s + 1 is transposed.
+//
+// Promotion: the fp8 tensor cores keep about 13 fraction bits of their sum (DESIGN.md §3), so an
+// interval of two stages (128 pairs, four k32 instructions) starts from zero (scale-d = 0) and its
+// sums are then added into fp32 registers; the error no longer grows with the share's length.
+struct Wg8Params {
+  WgParams w;              // pair mode; in: e4m3 [n_in, c_in], gout: e5m2 [n_out, c_out]
+  const float *a_scale, *g_scale;   // device fp32: the dequantisation factors of in and gout
+};
+
+// the 4-pair x 4-channel blocks of a row-major stage [64 pairs][C channels] (R bytes per row) ->
+// K-major core matrices: channel c, pairs p..p+3 at (c / 8) * kWgFp8Sbo + (p / 16) * 128 +
+// (c % 8) * 16 + p % 16.  Lanes run over (c / 4 % 2, p / 4 % 4, c / 8): the stores of a warp
+// hit 32 banks, the loads two ways each.
+template <uint32_t C, uint32_t R>
+__device__ __forceinline__ void wgrad_fp8_transpose(const uint8_t *src, uint8_t *dst, uint32_t tid) {
+  constexpr uint32_t kBlocks = 64 / 4 * C / 4;
+#pragma unroll
+  for (uint32_t m = 0; m < (kBlocks + kThreads - 1) / kThreads; ++m) {
+    const uint32_t u = tid + m * kThreads;
+    if (kBlocks % kThreads != 0 && u >= kBlocks) break;
+    const uint32_t b = u & 1u, pl = (u >> 1) & 3u, rest = u >> 3;
+    const uint32_t a = rest % (C / 8), pc = rest / (C / 8);
+    const uint8_t *s = src + (16 * pc + 4 * pl) * R + 8 * a + 4 * b;
+    const uint32_t w0 = *reinterpret_cast<const uint32_t *>(s);
+    const uint32_t w1 = *reinterpret_cast<const uint32_t *>(s + R);
+    const uint32_t w2 = *reinterpret_cast<const uint32_t *>(s + 2 * R);
+    const uint32_t w3 = *reinterpret_cast<const uint32_t *>(s + 3 * R);
+    const uint32_t t0 = __byte_perm(w0, w1, 0x5140), t1 = __byte_perm(w0, w1, 0x7362);
+    const uint32_t t2 = __byte_perm(w2, w3, 0x5140), t3 = __byte_perm(w2, w3, 0x7362);
+    uint8_t *d = dst + a * tc::kWgFp8Sbo + pc * 128 + 64 * b + 4 * pl;
+    *reinterpret_cast<uint32_t *>(d) = __byte_perm(t0, t2, 0x5410);        // channel c
+    *reinterpret_cast<uint32_t *>(d + 16) = __byte_perm(t0, t2, 0x7632);   // c + 1
+    *reinterpret_cast<uint32_t *>(d + 32) = __byte_perm(t1, t3, 0x5410);   // c + 2
+    *reinterpret_cast<uint32_t *>(d + 48) = __byte_perm(t1, t3, 0x7632);   // c + 3
+  }
+}
+
+template <int NI, int NT>
+__global__ void __launch_bounds__(kThreads, 1) k_wgrad_fp8(const Wg8Params q) {
+  const WgParams &p = q.w;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t *sm = align1k(smem_raw);
+  constexpr uint32_t kCols = NI * NT;
+  constexpr uint32_t kRowA = tc::kWgChannels + tc::kWgFp8Pad, kRowB = kCols + tc::kWgFp8Pad;
+  constexpr uint32_t kStage = tc::kWgRows * (kRowA + kRowB);
+  constexpr uint32_t kTileA = tc::kWgChannels / 8 * tc::kWgFp8Sbo;
+  constexpr uint32_t kTile = kTileA + kCols / 8 * tc::kWgFp8Sbo;
+  static_assert(tc::kWgRows == 64 && kCols <= tc::kWgFp8MaxCols, "fp8 wgrad tile");
+  const uint32_t tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
+  const uint32_t k = blockIdx.z / p.col_slices, col0 = blockIdx.z % p.col_slices * kCols;
+  const uint32_t ci0 = blockIdx.y * tc::kWgChannels;
+  const uint8_t *In = reinterpret_cast<const uint8_t *>(p.in);
+  const uint8_t *G = reinterpret_cast<const uint8_t *>(p.gout);
+
+  uint32_t n_st = 0;
+  for (uint32_t c = 0; c < p.n_chunks; ++c) {
+    uint32_t lo, hi;
+    wg_range(p, k, c, lo, hi);
+    n_st += (hi - lo + tc::kWgRows - 1) / tc::kWgRows;
+  }
+  // as in wgrad_unit: thread tid copies row ar = tid / 4 of both operands, 16-byte chunks
+  // (tid & 3) + 4m, from index words fetched a stage ahead
+  const uint32_t ar = tid >> 2, j0 = tid & 3u;
+  uint32_t wc = 0, pos = 0, end = 0;
+  auto open = [&]() {
+    for (; wc < p.n_chunks; ++wc) {
+      wg_range(p, k, wc, pos, end);
+      if (pos < end) return;
+    }
+  };
+  open();
+  struct Words { int32_t src, o; };
+  auto fetch = [&]() {
+    Words w{-1, -1};
+    const uint32_t r = pos + ar;
+    if (r < end) {
+      w.src = __ldg(p.pin + r);
+      w.o = __ldg(p.pout + r);
+    }
+    pos += tc::kWgRows;
+    if (pos >= end) { ++wc; open(); }
+    return w;
+  };
+  auto copy = [&](uint32_t s, Words w) {
+    const uint32_t base = smem_u32(sm + (s % kStages) * kStage);
+    const bool ok = w.src >= 0 && (uint32_t)w.src < p.n_in;
+    const uint8_t *rp = In + (size_t)(ok ? w.src : 0) * p.c_in + ci0;
+#pragma unroll
+    for (uint32_t m = 0; m < 2; ++m) {
+      const uint32_t j = j0 + 4 * m;
+      const bool okj = ok && ci0 + 16 * j < p.c_in;
+      cp_async16(base + ar * kRowA + 16 * j, okj ? rp + 16 * j : In, okj ? 16u : 0u);
+    }
+    const bool okr = w.o >= 0 && (uint32_t)w.o < p.n_out;
+    const uint8_t *gp = G + (size_t)(okr ? w.o : 0) * p.c_out + col0;
+#pragma unroll
+    for (uint32_t m = 0; m < (kCols / 16 + 3) / 4; ++m) {
+      const uint32_t j = j0 + 4 * m;
+      if (j < kCols / 16)
+        cp_async16(base + tc::kWgRows * kRowA + ar * kRowB + 16 * j, gp + 16 * j, okr ? 16u : 0u);
+    }
+  };
+
+  float acc[NT][NI / 2], sum[NT][NI / 2];
+#pragma unroll
+  for (int i = 0; i < NT; ++i)
+#pragma unroll
+    for (int e = 0; e < NI / 2; ++e) acc[i][e] = sum[i][e] = 0.f;
+
+  Words first[kStages - 2];
+#pragma unroll
+  for (uint32_t s = 0; s < kStages - 2; ++s)
+    if (s < n_st) first[s] = fetch();
+#pragma unroll
+  for (uint32_t s = 0; s < kStages - 2; ++s) {
+    if (s < n_st) copy(s, first[s]);
+    cp_async_commit();
+  }
+  Words next{-1, -1};
+  if (kStages - 2 < n_st) next = fetch();
+  for (uint32_t s = 0; s < n_st; ++s) {
+    cp_async_wait<kStages - 3>();
+    __syncthreads();     // stage s landed everywhere; the MMAs of stage s - 2 (tile s % 2) retired
+    if (s + kStages - 2 < n_st) {       // into the slot of stage s - 2, transposed at s - 2
+      copy(s + kStages - 2, next);
+      if (s + kStages - 1 < n_st) next = fetch();
+    }
+    cp_async_commit();
+    const uint8_t *st = sm + (s % kStages) * kStage;
+    uint8_t *tile = sm + kStages * kStage + (s & 1u) * kTile;
+    wgrad_fp8_transpose<tc::kWgChannels, kRowA>(st, tile, tid);
+    wgrad_fp8_transpose<kCols, kRowB>(st + tc::kWgRows * kRowA, tile + kTileA, tid);
+    fence_proxy_async();
+    __syncthreads();                    // the tile is written, and visible to the async proxy
+    const uint32_t a0 = smem_u32(tile) + wg * 8 * tc::kWgFp8Sbo, b0 = smem_u32(tile) + kTileA;
+    const uint32_t keep = s & 1u;       // 0: the first stage of an interval starts from zero
+    wgmma_fence();
+#pragma unroll
+    for (uint32_t kk = 0; kk < tc::kWgRows / 32; ++kk) {
+      const uint64_t da = wgmma_desc(a0 + kk * 256, 128, tc::kWgFp8Sbo);
+#pragma unroll
+      for (int i = 0; i < NT; ++i)
+        wgmma_e4m3e5m2<NI>(acc[i], da,
+                           wgmma_desc(b0 + i * (NI / 8) * tc::kWgFp8Sbo + kk * 256, 128, tc::kWgFp8Sbo),
+                           kk > 0 ? 1u : keep);
+    }
+    wgmma_commit();
+    if (keep || s + 1 == n_st) {        // the interval's end: its sums into the fp32 ones
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < NT; ++i)
+#pragma unroll
+        for (int e = 0; e < NI / 2; ++e) sum[i][e] += acc[i][e];
+    } else {
+      wgmma_wait<1>();
+    }
+  }
+
+  const float as = __ldg(q.a_scale), gs = __ldg(q.g_scale);
+  const uint32_t g = lane >> 2, t = lane & 3;
+  const uint32_t cbase = ci0 + wg * 64 + (warp & 3) * 16 + g;
+  const size_t dw_elems = (size_t)p.K * p.c_in * p.c_out;   // every element written by one CTA
+  float *dWk = (p.n_splits > 1 ? p.partial + blockIdx.x * dw_elems : p.dW) + (size_t)k * p.c_in * p.c_out;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const uint32_t ci = cbase + 8 * h;
+    if (ci >= p.c_in) continue;
+#pragma unroll
+    for (int i = 0; i < NT; ++i)
+#pragma unroll
+      for (int j = 0; j < NI / 8; ++j)
+        *reinterpret_cast<float2 *>(dWk + (size_t)ci * p.c_out + col0 + i * NI + 8 * j + 2 * t) =
+            make_float2(__fmul_rn(__fmul_rn(sum[i][4 * j + 2 * h], as), gs),
+                        __fmul_rn(__fmul_rn(sum[i][4 * j + 2 * h + 1], as), gs));
+  }
+}
+
 
 // ---- weight packing ----------------------------------------------------------------------------
 // Per-optimizer-step weight packing: fp32 master W[k][ci][co] -> the operand type in the two
@@ -952,6 +1142,16 @@ static int run_wgrad(int dtype, WgParams p, uint32_t K_grid, uint32_t est_stages
   return launch_split_sum(p.partial, p.dW, dw_elems, p.n_splits, stream);
 }
 
+template <int NI, int NT>
+static int launch_wgrad_fp8(const Wg8Params &q, dim3 grid, cudaStream_t stream) {
+  auto kern = k_wgrad_fp8<NI, NT>;
+  MEB_BIG_SMEM(kern);
+  kern<<<grid, kThreads, tc::wgrad_fp8_smem_bytes(NI * NT), stream>>>(q);
+  count_tc_launch();
+  MEB_LAUNCH_OK();
+  return MEB200_OK;
+}
+
 // ---- forward / dgrad ----------------------------------------------------------------------------
 static uint32_t operand_bytes(int dtype) {
   return dtype == MEB200_TF32 ? 4 : (dtype == kOperandE4M3 || dtype == kOperandE5M2E4M3 ? 1 : 2);
@@ -1113,6 +1313,51 @@ int conv_wgrad_pairs(const void *in, const void *grad_out, int dtype, uint32_t c
   p.n_out = n_out; p.n_chunks = n_chunks;
   // splits from the estimate "a third of the K * n_out table entries are pairs"
   return run_wgrad(dtype, p, K, n_out / (3 * tc::kWgRows) + 1, workspace, workspace_bytes, stream);
+}
+
+// ---- fp8 wgrad -----------------------------------------------------------------------------------
+bool conv_wgrad_fp8_supported(uint32_t c_in, uint32_t c_out, uint32_t K) {
+  return K >= 1 && K <= 1023 && c_in >= 32 && c_in % 32 == 0 && c_in <= 1024 && c_out >= 32 &&
+         c_out % 32 == 0 && c_out <= 1024;
+}
+
+int conv_wgrad_fp8(const void *in, const float *a_scale, const void *grad_out,
+                   const float *g_scale, uint32_t c_in, uint32_t K, uint32_t c_out,
+                   const int32_t *pairs_in, const int32_t *pairs_out, const int32_t *seg_start,
+                   uint32_t n_chunks, uint32_t n_out, float *grad_weight, void *workspace,
+                   uint64_t workspace_bytes, cudaStream_t stream) {
+  if (!conv_wgrad_fp8_supported(c_in, c_out, K) || !aligned(16, in, grad_out)) {
+    set_error("fp8 wgrad: shape or alignment off the grid (c_in=%u c_out=%u K=%u)", c_in, c_out, K);
+    return MEB200_ERR_UNSUPPORTED;
+  }
+  if (n_out == 0) {
+    MEB_CUDA(cudaMemsetAsync(grad_weight, 0, (size_t)K * c_in * c_out * sizeof(float), stream));
+    return MEB200_OK;
+  }
+  Wg8Params q{};
+  WgParams &p = q.w;
+  p.in = in; p.gout = grad_out; p.pin = pairs_in; p.pout = pairs_out; p.seg = seg_start;
+  p.dW = grad_weight; p.c_in = c_in; p.c_out = c_out; p.K = K; p.n_in = kNoLimit;
+  p.n_out = n_out; p.n_chunks = n_chunks;
+  q.a_scale = a_scale; q.g_scale = g_scale;
+  const uint32_t cols = tc::wgrad_fp8_cols(c_out);
+  p.col_slices = c_out / cols;
+  // the splits of conv_wgrad_pairs: conv_wgrad_workspace_bytes covers them
+  const size_t dw_elems = (size_t)K * c_in * c_out;
+  p.n_splits = workspace_splits(wgrad_planned_splits(c_in, K, n_out / (3 * tc::kWgRows) + 1),
+                                workspace, workspace_bytes, dw_elems * sizeof(float));
+  p.partial = p.n_splits > 1 ? reinterpret_cast<float *>(workspace) : nullptr;
+  const dim3 grid(p.n_splits, cdiv(c_in, tc::kWgChannels), K * p.col_slices);
+  int rc = MEB200_ERR_UNSUPPORTED;
+  switch (cols) {
+    case 32: rc = launch_wgrad_fp8<32, 1>(q, grid, stream); break;
+    case 64: rc = launch_wgrad_fp8<64, 1>(q, grid, stream); break;
+    case 96: rc = launch_wgrad_fp8<32, 3>(q, grid, stream); break;
+    case 128: rc = launch_wgrad_fp8<64, 2>(q, grid, stream); break;
+    default: set_error("fp8 wgrad: %u columns per CTA", cols);
+  }
+  if (rc != MEB200_OK || p.n_splits == 1) return rc;
+  return launch_split_sum(p.partial, p.dW, dw_elems, p.n_splits, stream);
 }
 
 }  // namespace meb200

@@ -93,6 +93,16 @@ int conv_wgrad_pairs(const void *in, const void *grad_out, int dtype, uint32_t c
                      float *grad_weight, void *workspace, uint64_t workspace_bytes,
                      cudaStream_t stream);
 
+// fp8 wgrad over the pair lists (meb200_conv_wgrad_fp8): e4m3 input and e5m2 output gradient, each
+// with its device dequantisation factor; c_in and c_out multiples of 32 up to 1024, K <= 1023.
+// Its row splits are those of conv_wgrad_pairs (conv_wgrad_workspace_bytes covers them).
+bool conv_wgrad_fp8_supported(uint32_t c_in, uint32_t c_out, uint32_t K);
+int conv_wgrad_fp8(const void *in, const float *a_scale, const void *grad_out,
+                   const float *g_scale, uint32_t c_in, uint32_t K, uint32_t c_out,
+                   const int32_t *pairs_in, const int32_t *pairs_out, const int32_t *seg_start,
+                   uint32_t n_chunks, uint32_t n_out, float *grad_weight, void *workspace,
+                   uint64_t workspace_bytes, cudaStream_t stream);
+
 // ---- network stem: rows of <= 4 channels, padded to 4 (8 bytes) ------------------------------
 // The layer is run as a K = 1 convolution over 4 * 16 ceil(K / 16) VIRTUAL channels (offset k,
 // channel c) -> 4 k + c, by the forward and wgrad kernels in their stem mode.

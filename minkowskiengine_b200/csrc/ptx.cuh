@@ -162,7 +162,30 @@ __device__ __forceinline__ void wgmma_64_e5m2e4m3(float (&d)[32], uint64_t da, u
                "%32, %33, p, 1, 1;\n\t}"
                : MEB_F8(d, 0), MEB_F8(d, 8), MEB_F8(d, 16), MEB_F8(d, 24) : "l"(da), "l"(db), "r"(1));
 }
+// e4m3 A times e5m2 B (the fp8 wgrad: features against gradients), the same shapes and layouts.
+// scale_d = 0: D = A * B, the accumulator's previous contents ignored (a promotion interval's start).
+__device__ __forceinline__ void wgmma_32_e4m3e5m2(float (&d)[16], uint64_t da, uint64_t db,
+                                                  uint32_t scale_d) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k32.f32.e4m3.e5m2 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+               "%16, %17, p, 1, 1;\n\t}"
+               : MEB_F8(d, 0), MEB_F8(d, 8) : "l"(da), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_64_e4m3e5m2(float (&d)[32], uint64_t da, uint64_t db,
+                                                  uint32_t scale_d) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e5m2 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+               "%32, %33, p, 1, 1;\n\t}"
+               : MEB_F8(d, 0), MEB_F8(d, 8), MEB_F8(d, 16), MEB_F8(d, 24) : "l"(da), "l"(db), "r"(scale_d));
+}
 #undef MEB_F8
+template <int N>
+__device__ __forceinline__ void wgmma_e4m3e5m2(float (&d)[N / 2], uint64_t da, uint64_t db,
+                                               uint32_t scale_d) {
+  static_assert(N == 32 || N == 64, "fp8 wgrad: N is 32 or 64");
+  if constexpr (N == 32) wgmma_32_e4m3e5m2(d, da, db, scale_d);
+  else wgmma_64_e4m3e5m2(d, da, db, scale_d);
+}
 template <int N>
 __device__ __forceinline__ void wgmma_e4m3(float (&d)[N / 2], uint64_t da, uint64_t db) {
   static_assert(N == 16 || N == 32 || N == 64, "wgmma: N is 16, 32 or 64");

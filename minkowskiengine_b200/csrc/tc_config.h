@@ -67,6 +67,28 @@ inline uint32_t wgrad_tf32_smem_bytes(uint32_t c_out) {
   return 1024 + kStages * kWgRowsTf32 * (kWgChannels + kWgPadTf32 + c_out + kWgPadTf32) * 4;
 }
 
+// fp8 wgrad (k_wgrad_fp8): a CTA keeps two fp32 accumulators per output element (the promotion
+// interval's and the share's), which caps its tile at kWgFp8MaxCols output columns; wider layers
+// run as column slices of wgrad_fp8_cols(c_out) columns, c_out a multiple of 32 up to 1024.
+constexpr uint32_t kWgFp8MaxCols = 128;
+constexpr uint32_t kWgFp8Pad = 16;          // bytes after every staged row and 8-row core group
+inline uint32_t wgrad_fp8_cols(uint32_t c_out) {
+  if (c_out <= kWgFp8MaxCols) return c_out;
+  return c_out % 128 == 0 ? 128 : (c_out % 96 == 0 ? 96 : (c_out % 64 == 0 ? 64 : 32));
+}
+// byte distance between 8-channel groups of a transposed tile: 8 channels x 64 pairs (4 core
+// matrices) and the pad, so that the transposing stores of a warp hit 32 different banks
+constexpr uint32_t kWgFp8Sbo = kWgRows / 16 * 128 + kWgFp8Pad;
+// ring of kStages row-major stages, X [64 pairs][128 + pad] and dY [64 pairs][cols + pad] bytes,
+// and two transposed (K-major) tiles of (128 + cols) / 8 groups; +1 KB for alignment
+inline uint32_t wgrad_fp8_stage_bytes(uint32_t cols) {
+  return kWgRows * (kWgChannels + kWgFp8Pad + cols + kWgFp8Pad);
+}
+inline uint32_t wgrad_fp8_tile_bytes(uint32_t cols) { return (kWgChannels + cols) / 8 * kWgFp8Sbo; }
+inline uint32_t wgrad_fp8_smem_bytes(uint32_t cols) {
+  return 1024 + kStages * wgrad_fp8_stage_bytes(cols) + 2 * wgrad_fp8_tile_bytes(cols);
+}
+
 // wgrad row splits: enough CTAs for two waves over (k, channel tile) pairs, but at least
 // 4 stages of work per CTA so the store of its 128 x c_out partial sums (and their later
 // ordered addition) stays amortised.

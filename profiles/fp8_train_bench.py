@@ -1,16 +1,17 @@
 """Times bench.py's cfg3 training step (MinkUNet34C, examples/minkunet.py, on 8 clouds x 100k voxels
 of examples.synthetic.surface_cloud, bf16 features, maps rebuilt every step, SGD) in bf16 against the
-same step inside ME.fp8_training().
+same step inside ME.fp8_training() and inside ME.fp8_training(weight_gradient=True).
 
     python profiles/fp8_train_bench.py [--steps 20] [--warmup 3]
 
-One network per mode, both from the same initial state; the two modes alternate within one loop,
+One network per mode, all from the same initial state; the modes alternate within one loop,
 each step timed with CUDA events from before its SparseTensor is built to after the optimizer step.
 Then, in a separate run of one step per mode, backend.profile_conv_kernels splits every backward
 into its dgrad and its wgrad call, and CUDA events around every library call of the convolutions,
-the fp8 quantisations and the weight packs give the per-family and per-layer breakdown.  Prints the
-card's name and power limit, one JSON line with the step times and the step-0 losses, one with the
-per-family totals and one JSON line per convolution layer."""
+the fp8 quantisations and the weight packs give the per-family and per-layer breakdown, and the peak
+memory of one step per mode.  Prints the card's name and power limit, one JSON line with the step
+times and the step-0 losses, one with the per-family totals, one with the peak memory and one JSON
+line per convolution layer."""
 import argparse
 import contextlib
 import json
@@ -46,7 +47,7 @@ class _Recorder:
              "meb200_conv_backward", "meb200_conv_stem_wgrad", "meb200_conv_dgrad_fp8",
              "meb200_quantize_e4m3", "meb200_quantize_e5m2", "meb200_conv_pack_weights",
              "meb200_conv_pack_weights_batched", "meb200_conv_pack_weights_e4m3",
-             "meb200_conv_pack_weights_e4m3_dgrad")
+             "meb200_conv_pack_weights_e4m3_dgrad", "meb200_conv_wgrad_fp8")
 
     def __init__(self):
         self.lib = _lib.load()
@@ -87,6 +88,8 @@ class _Recorder:
                 out.append(("forward", a[5], a[3], a[6], ms))
             elif name == "meb200_conv_dgrad_fp8":
                 out.append(("dgrad", a[6], a[7], a[3], ms))
+            elif name == "meb200_conv_wgrad_fp8":
+                out.append(("wgrad", a[5], a[4], a[6], ms))
             elif name == "meb200_conv_stem_forward":
                 out.append(("forward", a[2], 4, a[4], ms))
             elif name == "meb200_conv_stem_wgrad":
@@ -115,7 +118,7 @@ def main():
     feats = feats_h.to(dev).bfloat16()
     crit = torch.nn.CrossEntropyLoss()
     nets, opts = {}, {}
-    for mode in ("bf16", "fp8"):
+    for mode in ("bf16", "fp8", "fp8_wgrad"):
         torch.manual_seed(0)
         nets[mode] = minkunet("MinkUNet34C", ME, 3, 20, 3).to(dev)
         opts[mode] = torch.optim.SGD(nets[mode].parameters(), lr=1e-2)
@@ -123,7 +126,9 @@ def main():
     def step(mode):
         net, opt = nets[mode], opts[mode]
         opt.zero_grad(set_to_none=True)
-        with ME.fp8_training() if mode == "fp8" else contextlib.nullcontext():
+        ctx = contextlib.nullcontext() if mode == "bf16" else \
+            ME.fp8_training(weight_gradient=mode == "fp8_wgrad")
+        with ctx:
             out = net(ME.SparseTensor(feats, coords))
             loss = crit(out.F.float(), labels)
             loss.backward()
@@ -148,6 +153,7 @@ def main():
     for m, v in ms.items():
         res[m] = {"median_ms": statistics.median(v), "min_ms": min(v), "max_ms": max(v)}
     res["fp8_over_bf16"] = res["fp8"]["median_ms"] / res["bf16"]["median_ms"]
+    res["fp8_wgrad_over_bf16"] = res["fp8_wgrad"]["median_ms"] / res["bf16"]["median_ms"]
     print(json.dumps(res), flush=True)
 
     tables = {}
@@ -162,11 +168,20 @@ def main():
             d = fam.setdefault(key, {})
             d[m] = round(d.get(m, 0.0) + v, 4)
     print(json.dumps({"ms_per_family": fam}), flush=True)
+    peak = {}
+    for m in nets:
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        step(m)
+        torch.cuda.synchronize()
+        peak[m] = round(torch.cuda.max_memory_allocated() / 2 ** 30, 3)
+    print(json.dumps({"peak_memory_gib": peak}), flush=True)
     for f in ("forward", "dgrad", "wgrad"):
         rows = {m: [r for r in t if r[0] == f] for m, t in tables.items()}
-        for i, (b, q) in enumerate(zip(rows["bf16"], rows["fp8"])):
+        for i, (b, q, w) in enumerate(zip(rows["bf16"], rows["fp8"], rows["fp8_wgrad"])):
             print(json.dumps({"pass": f, "layer": i, "K": b[1], "c_in": b[2], "c_out": b[3],
-                              "bf16_ms": round(b[4], 4), "fp8_mode_ms": round(q[4], 4)}),
+                              "bf16_ms": round(b[4], 4), "fp8_mode_ms": round(q[4], 4),
+                              "fp8_wgrad_mode_ms": round(w[4], 4)}),
                   flush=True)
 
 
