@@ -380,6 +380,39 @@ int meb200_conv_wgrad_fp8(const void *in_e4m3, const float *a_scale, const void 
                           float *grad_weight, void *workspace, uint64_t workspace_bytes,
                           void *stream);
 
+/* ---- fp8 training with delayed scaling ---------------------------------------------------------
+ * Each fp8 operand role (a layer's e4m3 input, its e5m2 output gradient) is an ENTRY: a history of
+ * the amax of its last H steps and a current slot (DEVICE fp32, zero at the start of a step) that
+ * the running step records into.  Step t converts at the (scale, inv) of the history alone, so the
+ * conversion waits on no amax pass and can be fused into whoever writes the tensor:
+ *   amax  = max of the H past values
+ *   (scale, inv) = the e4m3 / e5m2 formula above of min(amax * 2^margin, FLT_MAX)
+ *   q     = cvt.rn.satfinite(x * inv): values beyond the scaled amax saturate to +-448 / +-57344
+ *   slot  = max(slot, max |x| over the finite values of x), an atomic max on the fp32 bits
+ * meb200_fp8_out describes one such write: q the bytes (8-byte aligned where a batch-norm pass
+ * writes them), scale the entry's DEVICE fp32 [2] (scale, inv) of the step, amax_slot its slot. */
+#define MEB200_FP8_E4M3 0
+#define MEB200_FP8_E5M2 1
+#define MEB200_FP8_MAX_HISTORY 1024 /* H of meb200_fp8_roll: one thread walks an entry's history */
+typedef struct meb200_fp8_out {
+  void *q;
+  const float *scale;
+  float *amax_slot;
+} meb200_fp8_out;
+/* Features [n, c] in `dtype` (F32 / BF16 / F16) -> out->q [n, c] in `format` (MEB200_FP8_E4M3 /
+ * _E5M2) at out->scale, recording the amax into out->amax_slot, in ONE launch (the conversion of
+ * meb200_quantize_e4m3_static, 16 output bytes per access when both buffers are 16-byte aligned).
+ * n * c = 0: nothing is launched, and in / out->q may be NULL. */
+int meb200_quantize_fp8_record(const void *in, int dtype, uint32_t n, uint32_t c, int format,
+                               const meb200_fp8_out *out, void *stream);
+/* The step boundary of L = n_e4m3 + n_e5m2 entries in one launch (no host read): entry i's slot
+ * cur[i] goes in front of its history row hist[i, 0:H] (newest first) and the oldest value drops
+ * out; scales[i, 0:2] = (scale, inv) of the new history by the formula above, in e4m3 for
+ * i < n_e4m3 and e5m2 from there; next_cur[i] = 0 (the slots of the new step; may be cur).
+ * 1 <= H <= MEB200_FP8_MAX_HISTORY, 0 <= margin <= 127. */
+int meb200_fp8_roll(const float *cur, float *hist, uint32_t n_e4m3, uint32_t n_e5m2, uint32_t H,
+                    int margin, float *next_cur, float *scales, void *stream);
+
 /* Weight packing, once per optimizer step instead of once per call: fp32 master weight
  * [K, Cin, Cout] -> `dtype` (BF16/F16, or TF32: fp32 words rounded to tf32) operand copies
  * w_cast [K, Cin, Cout] and w_t [K, Cout, Cin].  The reference keeps weights in the feature dtype and needs no such step
@@ -799,6 +832,41 @@ int meb200_bn_backward_reduce_peer(const void *dy, const void *x, const void *y_
                                    uint64_t slot_offset_bytes, uint32_t seq, uint32_t rank,
                                    uint32_t world, double *sums_out, float *grad_weight,
                                    float *grad_bias, void *stream);
+
+/* ---- batch norm writing an fp8 copy of its output (delayed scaling, above) -----------------------
+ * The _q twins take the arguments of their entry plus `fq` (required) and also write, in the apply
+ * pass, fq->q [n, C] = the fp8 bytes of the value the pass stores, rounded to `dtype` first:
+ *   forward (apply_fused, forward_train, forward_train_peer): q = e4m3(round_dtype(y) * fq->scale[1])
+ *   backward_apply_fused:                                      q = e5m2(round_dtype(dx) * fq->scale[1])
+ * so that q equals meb200_quantize_fp8_record of the stored y / dx byte for byte, and maxes
+ * max |round_dtype(v)| over the finite values into *fq->amax_slot.  Each thread's eight channels
+ * are one 8-byte store; fq->q must be 8-byte aligned (it may be NULL when n = 0: a rank without
+ * rows still takes part in the exchange of forward_train_peer_q).  Every other output (y, dx,
+ * d_residual, statistics, running statistics) is that of the entry without the copy, bit for
+ * bit. */
+int meb200_bn_apply_fused_q(const void *x, int dtype, uint32_t n, uint32_t C, const float *mean,
+                            const float *invstd, const float *weight, const float *bias,
+                            const void *residual, int relu, void *y, const meb200_fp8_out *fq,
+                            void *stream);
+int meb200_bn_forward_train_q(const void *x, int dtype, uint32_t n, uint32_t C,
+                              const float *weight, const float *bias, const void *residual,
+                              int relu, float eps, float momentum, float *running_mean,
+                              float *running_var, long long *num_batches_tracked, void *workspace,
+                              float *mean, float *invstd, void *y, const meb200_fp8_out *fq,
+                              void *stream);
+int meb200_bn_forward_train_peer_q(const void *x, int dtype, uint32_t n, uint32_t C,
+                                   const float *weight, const float *bias, const void *residual,
+                                   int relu, float eps, float momentum, float *running_mean,
+                                   float *running_var, long long *num_batches_tracked,
+                                   void *workspace, const void *peer_bases_dev,
+                                   uint64_t slot_offset_bytes, uint32_t seq, uint32_t rank,
+                                   uint32_t world, float *mean, float *invstd, double *total_rows,
+                                   void *y, const meb200_fp8_out *fq, void *stream);
+int meb200_bn_backward_apply_fused_q(const void *dy, const void *x, const void *y_mask, int dtype,
+                                     uint32_t n, uint32_t C, const float *mean,
+                                     const float *invstd, const float *weight, const double *sums,
+                                     double count, const double *d_count, void *dx,
+                                     void *d_residual, const meb200_fp8_out *fq, void *stream);
 
 #ifdef __cplusplus
 }

@@ -51,6 +51,7 @@ from .normalization import (MinkowskiBatchNorm, MinkowskiInstanceNorm,
 from .convolution import fused_conv_bn_relu
 from .backend import fp8_inference, fp8_training
 from .fp8_calibration import Fp8Calibration
+from .fp8_delayed import Fp8DelayedScaling
 from .nonlinearity import *  # noqa: F401,F403
 from .ops import (MinkowskiLinear, MinkowskiStackCat, MinkowskiStackMean, MinkowskiStackSum,
                   MinkowskiStackVar, MinkowskiToFeature, MinkowskiToSparseTensor, cat, mean, var)

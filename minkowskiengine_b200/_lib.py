@@ -20,6 +20,8 @@ BCAST_ADD, BCAST_MUL, BCAST_COPY, BCAST_MAXGRAD = 0, 1, 2, 3
 UNION_ADD, UNION_SUB, UNION_MUL, UNION_DIV = 0, 1, 2, 3
 FIELD_SUM, FIELD_AVG, FIELD_MAX, FIELD_SUBSAMPLE = 0, 1, 2, 3
 ERR_DOMAIN = -4
+FP8_E4M3, FP8_E5M2 = 0, 1
+FP8_MAX_HISTORY = 1024      # MEB200_FP8_MAX_HISTORY
 
 _u32, _u64, _i32, _vp = C.c_uint32, C.c_uint64, C.c_int, C.c_void_p
 
@@ -72,6 +74,8 @@ PROTOTYPES = {
     "meb200_conv_wgrad_fp8_workspace_bytes": (_u64, [_u32, _u32, _u32, _u32]),
     "meb200_conv_wgrad_fp8": (_i32, [_vp, _vp, _vp, _vp, _u32, _u32, _u32, _vp, _vp, _vp, _u32,
                                      _u32, _vp, _vp, _u64, _vp]),
+    "meb200_quantize_fp8_record": (_i32, [_vp, _i32, _u32, _u32, _i32, _vp, _vp]),
+    "meb200_fp8_roll": (_i32, [_vp, _vp, _u32, _u32, _u32, _i32, _vp, _vp, _vp]),
     "meb200_conv_pack_weights": (_i32, [_vp, _u32, _u32, _u32, _i32, _vp, _vp, _vp]),
     "meb200_conv_pack_weights_batched": (_i32, [_vp, _u32, _u32, _i32, _vp]),
     "meb200_conv_stem_virtual_channels": (_u32, [_u32]),
@@ -143,6 +147,16 @@ PROTOTYPES = {
                                             _u32, _vp, _vp, _vp, _vp, _vp]),
     "meb200_bn_backward_reduce_peer": (_i32, [_vp, _vp, _vp, _i32, _u32, _u32, _vp, _vp, _vp, _vp,
                                               C.c_uint64, _u32, _u32, _u32, _vp, _vp, _vp, _vp]),
+    "meb200_bn_apply_fused_q": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _i32, _vp,
+                                       _vp, _vp]),
+    "meb200_bn_forward_train_q": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _vp, _i32, C.c_float,
+                                         C.c_float, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "meb200_bn_forward_train_peer_q": (_i32, [_vp, _i32, _u32, _u32, _vp, _vp, _vp, _i32,
+                                              C.c_float, C.c_float, _vp, _vp, _vp, _vp, _vp,
+                                              C.c_uint64, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp,
+                                              _vp]),
+    "meb200_bn_backward_apply_fused_q": (_i32, [_vp, _vp, _vp, _i32, _u32, _u32, _vp, _vp, _vp,
+                                                _vp, C.c_double, _vp, _vp, _vp, _vp, _vp]),
 }
 
 # These calls gained an optional pointer just before the stream: meb200_conv_backward its

@@ -1651,7 +1651,7 @@ FP8_DGRAD = "e4m3_dgrad"      # the packed-weight cache's operand of the dgrad's
 
 
 @contextlib.contextmanager
-def fp8_training(*, weight_gradient=False):
+def fp8_training(*, weight_gradient=False, scaling=None):
     """Within the block, training sparse convolutions run their forward and input gradient on the
     Hopper fp8 tensor cores where they can (a gradient needed, c_in and c_out multiples of 32 up to
     1024, not a K = 1 stride-1 matrix product): the forward on e4m3 features and weights, the input
@@ -1663,9 +1663,16 @@ def fp8_training(*, weight_gradient=False):
     of the forward times the e5m2 output gradient of the input gradient (layers with over 1023
     kernel offsets keep the weight gradient of the feature dtype).  Forward outputs and input
     gradients are those of weight_gradient=False, bit for bit.  Nested blocks: the innermost
-    decides."""
+    decides.
+
+    scaling (an Fp8DelayedScaling, DESIGN.md §3 "delayed scaling"): the selected layers of the
+    model it is bound to quantise at the scales of its amax histories instead of their tensors'
+    own amax, and the training batch norms that feed them write their fp8 operands.  Each entry
+    into an outermost block with a given recipe is one step of it.  None: dynamic scales."""
     modes = _FP8_STATE.__dict__.setdefault("train_modes", [])
-    modes.append(bool(weight_gradient))
+    if scaling is not None and all(m[1] is not scaling for m in modes):
+        scaling._begin_step()
+    modes.append((bool(weight_gradient), scaling))
     try:
         yield
     finally:
@@ -1679,7 +1686,48 @@ def fp8_training_enabled():
 def fp8_training_weight_gradient():
     """Whether the innermost fp8_training() block of this thread runs weight gradients on fp8."""
     modes = getattr(_FP8_STATE, "train_modes", None)
-    return bool(modes) and modes[-1]
+    return bool(modes) and modes[-1][0]
+
+
+def fp8_training_scaling():
+    """The Fp8DelayedScaling of the innermost fp8_training() block of this thread, or None."""
+    modes = getattr(_FP8_STATE, "train_modes", None)
+    return modes[-1][1] if modes else None
+
+
+class _Fp8Out(ctypes.Structure):      # == meb200_fp8_out (include/meb200.h)
+    _fields_ = [("q", ctypes.c_void_p), ("scale", ctypes.c_void_p), ("amax_slot", ctypes.c_void_p)]
+
+
+def fp8_out(q, scale, slot):
+    """The meb200_fp8_out of bytes `q`, a DEVICE fp32 [2] (scale, inv) and an fp32 [1] amax slot."""
+    return _Fp8Out(_lib.ptr(q), _lib.ptr(scale), _lib.ptr(slot))
+
+
+def quantize_fp8_record(feat, fmt, scale, slot):
+    """fp8 bytes [n, c] as uint8 of contiguous features in `fmt` (_lib.FP8_E4M3 / FP8_E5M2) at a
+    given scale (fp32 [2] on the device), max |feat| over the finite values maxed into `slot` (fp32
+    [1] on the device): one launch, no host read (meb200_quantize_fp8_record)."""
+    n, c = feat.shape
+    q = torch.empty((n, c), dtype=torch.uint8, device=feat.device)
+    fq = fp8_out(q, scale, slot)
+    _lib.check(_lib.load().meb200_quantize_fp8_record(
+        _lib.ptr(feat), _lib.dtype_code(feat.dtype), n, c, fmt, ctypes.byref(fq),
+        _lib.current_stream()))
+    return q
+
+
+def fp8_roll(cur, hist, n_e4m3, n_e5m2, margin):
+    """The step boundary of delayed scaling (meb200_fp8_roll): the slots `cur` [L] pushed into the
+    histories `hist` [L, H] in place; returns (the next step's zeroed slots [L], scales [L, 2]), the
+    first n_e4m3 entries in e4m3 and the rest in e5m2.  One launch, no host read."""
+    L, H = hist.shape
+    nxt = torch.empty(L, dtype=torch.float32, device=hist.device)
+    scales = torch.empty((L, 2), dtype=torch.float32, device=hist.device)
+    _lib.check(_lib.load().meb200_fp8_roll(_lib.ptr(cur), _lib.ptr(hist), n_e4m3, n_e5m2, H,
+                                           int(margin), _lib.ptr(nxt), _lib.ptr(scales),
+                                           _lib.current_stream()))
+    return nxt, scales
 
 
 def fp8_wgrad_supported(c_in, c_out, K):
@@ -1748,16 +1796,15 @@ def _conv_wgrad_fp8(act, grad_q, kernel, km):
     return grad_w if grad_w.dtype == kernel.dtype else grad_w.to(kernel.dtype)
 
 
-def _conv_backward_fp8w(act, dtype, grad_out, kernel, km, need_in=True, need_w=True):
+def _conv_backward_fp8w(act, dtype, grad_out, kernel, km, need_in=True, need_w=True, grad_q=None):
     """(grad_in or None, grad_w or None) of a layer run in fp8_training(weight_gradient=True), from
     act = (e4m3 bytes, scale) of its forward and its feature dtype: grad_out quantised to e5m2 once,
     for the input gradient (_conv_dgrad_fp8, as in fp8_training()) and the weight gradient
-    (_conv_wgrad_fp8)."""
+    (_conv_wgrad_fp8).  grad_q: grad_out already quantised (delayed scaling), or None."""
     if grad_out.dtype != dtype:
         grad_out = grad_out.to(dtype)
     grad_out = grad_out.contiguous()
-    grad_q = None
-    if km.n_out > 0 and km.n_in > 0:
+    if grad_q is None and km.n_out > 0 and km.n_in > 0:
         grad_q = _quantize_dynamic(grad_out, "meb200_quantize_e5m2")
     if _PROFILE is None:
         return (_conv_dgrad_fp8(grad_out, kernel, km, dtype, grad_q) if need_in else None,
@@ -1833,7 +1880,14 @@ def _conv_forward_impl(in_feat, kernel, km, out_dtype=None, epilogue=None, fp8=F
     return done()
 
 
-def _conv_backward(in_feat, grad_out, kernel, km, need_in=True, need_w=True, fp8=False):
+def _grad_q(grad_q):
+    """The keyword of an output gradient quantised beforehand (delayed scaling), or none: without
+    one the backward calls keep the arguments they have under fp8_training()."""
+    return {} if grad_q is None else {"grad_q": grad_q}
+
+
+def _conv_backward(in_feat, grad_out, kernel, km, need_in=True, need_w=True, fp8=False,
+                   grad_q=None):
     if _PROFILE is not None:
         esz = in_feat.element_size()
         K, c_in, c_out = kernel.shape
@@ -1843,18 +1897,21 @@ def _conv_backward(in_feat, grad_out, kernel, km, need_in=True, need_w=True, fp8
         if need_in:   # dgrad alone: dOut in, dIn out, W, table
             nb = km.n_out * c_out * esz + km.n_in * c_in * esz + K * c_in * c_out * esz + P * 8
             gi, _ = _record("conv_fwd_dgrad", lambda: _conv_backward_impl(
-                in_feat, grad_out, kernel, km, True, False, fp8), flops, nb)
+                in_feat, grad_out, kernel, km, True, False, fp8, **_grad_q(grad_q)), flops, nb)
         if need_w:    # wgrad alone: In and dOut in, dW (fp32) out, table
             nb = km.n_in * c_in * esz + km.n_out * c_out * esz + K * c_in * c_out * 4 + P * 8
             _, gw = _record("conv_wgrad", lambda: _conv_backward_impl(
                 in_feat, grad_out, kernel, km, False, True), flops, nb)
         return gi, gw
-    return _conv_backward_impl(in_feat, grad_out, kernel, km, need_in, need_w, fp8)
+    return _conv_backward_impl(in_feat, grad_out, kernel, km, need_in, need_w, fp8,
+                               **_grad_q(grad_q))
 
 
-def _conv_backward_impl(in_feat, grad_out, kernel, km, need_in=True, need_w=True, fp8=False):
+def _conv_backward_impl(in_feat, grad_out, kernel, km, need_in=True, need_w=True, fp8=False,
+                        grad_q=None):
     """(grad_in or None, grad_w or None).  fp8 (the caller has checked the grid both ways): the
-    input gradient on e5m2 x e4m3 (_conv_dgrad_fp8); the weight gradient as without it."""
+    input gradient on e5m2 x e4m3 (_conv_dgrad_fp8, with grad_q when given); the weight gradient as
+    without it."""
     lib = _lib.load()
     op = _operand(in_feat.dtype)
     code = _lib.dtype_code(op)
@@ -1862,7 +1919,7 @@ def _conv_backward_impl(in_feat, grad_out, kernel, km, need_in=True, need_w=True
         grad_out = grad_out.to(in_feat.dtype)
     grad_out = grad_out.contiguous()
     if fp8 and need_in:
-        grad_in = _conv_dgrad_fp8(grad_out, kernel, km, in_feat.dtype)
+        grad_in = _conv_dgrad_fp8(grad_out, kernel, km, in_feat.dtype, **_grad_q(grad_q))
         if not need_w:
             return grad_in, None
         return grad_in, _conv_backward_impl(in_feat, grad_out, kernel, km, False, True)[1]
@@ -1955,19 +2012,23 @@ def ConvolutionForwardGPU(in_feat, kernel, kernel_size, kernel_stride, kernel_di
 
 def ConvolutionBackwardGPU(in_feat, grad_out_feat, kernel, kernel_size, kernel_stride,
                            kernel_dilation, region_type, offset, convolution_mode, in_key,
-                           out_key, manager, need_in=True, need_w=True, fp8=False, act=None):
+                           out_key, manager, need_in=True, need_w=True, fp8=False, act=None,
+                           grad_q=None):
     """reference: ConvolutionBackwardGPU src/convolution_gpu.cu:161-244.  fp8: as _conv_backward_impl.
     act: (e4m3 bytes, fp32 [2] scale, feature dtype) of the input of a layer run in
     fp8_training(weight_gradient=True), in place of in_feat (None): both gradients on fp8
-    (_conv_backward_fp8w)."""
+    (_conv_backward_fp8w).  grad_q: (e5m2 bytes, fp32 [2] scale) of grad_out_feat (delayed
+    scaling), or None: quantised at its amax."""
     _check_feats(in_feat if act is None else act[0], manager, in_key)
     _assert(manager.exists(out_key), ERROR_MAP_NOT_FOUND)
     _assert(grad_out_feat.size(0) == manager.size(out_key), "Invalid grad_out size")
     km = manager._kernel_map(in_key, out_key, kernel_size, kernel_stride, kernel_dilation,
                              region_type, offset, False, False)
     if act is not None:
-        return _conv_backward_fp8w(act[:2], act[2], grad_out_feat, kernel, km, need_in, need_w)
-    return _conv_backward(in_feat, grad_out_feat, kernel, km, need_in, need_w, fp8)
+        return _conv_backward_fp8w(act[:2], act[2], grad_out_feat, kernel, km, need_in, need_w,
+                                   **_grad_q(grad_q))
+    return _conv_backward(in_feat, grad_out_feat, kernel, km, need_in, need_w, fp8,
+                          **_grad_q(grad_q))
 
 
 def ConvolutionTransposeForwardGPU(in_feat, kernel, kernel_size, kernel_stride,
@@ -1990,15 +2051,17 @@ def ConvolutionTransposeForwardGPU(in_feat, kernel, kernel_size, kernel_stride,
 def ConvolutionTransposeBackwardGPU(in_feat, grad_out_feat, kernel, kernel_size, kernel_stride,
                                     kernel_dilation, region_type, offset, convolution_mode,
                                     in_key, out_key, manager, need_in=True, need_w=True, fp8=False,
-                                    act=None):
-    """`fp8`, `act`: as ConvolutionBackwardGPU."""
+                                    act=None, grad_q=None):
+    """`fp8`, `act`, `grad_q`: as ConvolutionBackwardGPU."""
     _check_feats(in_feat if act is None else act[0], manager, in_key)
     _assert(manager.exists(out_key), ERROR_MAP_NOT_FOUND)
     km = manager._kernel_map(in_key, out_key, kernel_size, kernel_stride, kernel_dilation,
                              region_type, offset, True, False)
     if act is not None:
-        return _conv_backward_fp8w(act[:2], act[2], grad_out_feat, kernel, km, need_in, need_w)
-    return _conv_backward(in_feat, grad_out_feat, kernel, km, need_in, need_w, fp8)
+        return _conv_backward_fp8w(act[:2], act[2], grad_out_feat, kernel, km, need_in, need_w,
+                                   **_grad_q(grad_q))
+    return _conv_backward(in_feat, grad_out_feat, kernel, km, need_in, need_w, fp8,
+                          **_grad_q(grad_q))
 
 
 _POOL_CODE = {PoolingMode.LOCAL_SUM_POOLING: _lib.POOL_SUM,

@@ -18,16 +18,35 @@ from .normalization import MinkowskiBatchNorm, _bn_tail, _eval_scale_shift, _nat
 from .sparse_tensor import SparseTensor, _get_coordinate_map_key
 
 
-def _fp8_input(ctx, input_features, fp8_wgrad):
+def _fp8_input(ctx, input_features, fp8_wgrad, delayed):
     """Saves what the backward reads of the input: with fp8_wgrad (fp8_training(weight_gradient=
     True)) its e4m3 bytes and scale, which the forward multiplies (returned, for its `act`) and the
-    weight gradient reads, in place of the features; else the features (returns None)."""
+    weight gradient reads, in place of the features; else the features (returns None, or with
+    delayed scaling the e4m3 input `delayed` carries)."""
+    ctx.grad_entry = None if delayed is None else delayed.grad
     if not fp8_wgrad:
         ctx.input_features, ctx.act = input_features, None
-        return None
-    q, a_scale = _C._quantize_e4m3(input_features)
+        return None if delayed is None else delayed.act
+    q, a_scale = _C._quantize_e4m3(input_features) if delayed is None else delayed.act
     ctx.input_features, ctx.act = None, (q, a_scale, input_features.dtype)
     return q, a_scale
+
+
+def _fp8_grad(ctx, grad_out_feat):
+    """(grad_out_feat, its e5m2 operand or None) for the backward: with delayed scaling, the
+    gradient in the feature dtype and its operand from the layer's grad_output entry (None without
+    it, or when no fp8 gradient product runs: the backward quantises at the amax)."""
+    entry = ctx.grad_entry
+    need_in, need_w = ctx.needs_input_grad[:2]
+    if entry is None or not ((ctx.fp8 and need_in) or (ctx.act is not None and need_w)):
+        return grad_out_feat, None
+    dtype = ctx.act[2] if ctx.act is not None else ctx.input_features.dtype
+    if grad_out_feat.dtype != dtype:
+        grad_out_feat = grad_out_feat.to(dtype)
+    grad_out_feat = grad_out_feat.contiguous()
+    if grad_out_feat.numel() == 0:
+        return grad_out_feat, None
+    return grad_out_feat, entry.operand(grad_out_feat)
 
 
 class MinkowskiConvolutionFunction(Function):
@@ -37,12 +56,12 @@ class MinkowskiConvolutionFunction(Function):
                 in_coordinate_map_key: CoordinateMapKey,
                 out_coordinate_map_key: CoordinateMapKey = None,
                 coordinate_manager: CoordinateManager = None, fp8: bool = False,
-                fp8_wgrad: bool = False):
+                fp8_wgrad: bool = False, fp8_delayed=None):
         if out_coordinate_map_key is None:
             out_coordinate_map_key = CoordinateMapKey(
                 in_coordinate_map_key.get_coordinate_size())
         input_features = input_features.contiguous()
-        act = _fp8_input(ctx, input_features, fp8_wgrad)
+        act = _fp8_input(ctx, input_features, fp8_wgrad, fp8_delayed)
         ctx.kernel_weights = kernel_weights
         ctx.misc = (kernel_generator, convolution_mode, in_coordinate_map_key,
                     out_coordinate_map_key, coordinate_manager)
@@ -56,15 +75,15 @@ class MinkowskiConvolutionFunction(Function):
 
     @staticmethod
     def backward(ctx, grad_out_feat: torch.Tensor):
-        grad_out_feat = grad_out_feat.contiguous()
+        grad_out_feat, grad_q = _fp8_grad(ctx, grad_out_feat.contiguous())
         kgen, mode, in_key, out_key, manager = ctx.misc
         grad_in_feat, grad_kernel = _C.ConvolutionBackwardGPU(
             ctx.input_features, grad_out_feat, ctx.kernel_weights, kgen.kernel_size,
             kgen.kernel_stride, kgen.kernel_dilation, kgen.region_type, kgen.region_offsets,
             mode, in_key, out_key, manager._manager,
             need_in=ctx.needs_input_grad[0], need_w=ctx.needs_input_grad[1], fp8=ctx.fp8,
-            act=ctx.act)
-        return grad_in_feat, grad_kernel, None, None, None, None, None, None, None
+            act=ctx.act, grad_q=grad_q)
+        return grad_in_feat, grad_kernel, None, None, None, None, None, None, None, None
 
 
 class MinkowskiConvolutionTransposeFunction(Function):
@@ -74,12 +93,12 @@ class MinkowskiConvolutionTransposeFunction(Function):
                 in_coordinate_map_key: CoordinateMapKey,
                 out_coordinate_map_key: CoordinateMapKey = None,
                 coordinate_manager: CoordinateManager = None, fp8: bool = False,
-                fp8_wgrad: bool = False):
+                fp8_wgrad: bool = False, fp8_delayed=None):
         if out_coordinate_map_key is None:
             out_coordinate_map_key = CoordinateMapKey(
                 in_coordinate_map_key.get_coordinate_size())
         input_features = input_features.contiguous()
-        act = _fp8_input(ctx, input_features, fp8_wgrad)
+        act = _fp8_input(ctx, input_features, fp8_wgrad, fp8_delayed)
         ctx.kernel_weights = kernel_weights
         ctx.misc = (kernel_generator, convolution_mode, in_coordinate_map_key,
                     out_coordinate_map_key, coordinate_manager)
@@ -93,15 +112,15 @@ class MinkowskiConvolutionTransposeFunction(Function):
 
     @staticmethod
     def backward(ctx, grad_out_feat: torch.Tensor):
-        grad_out_feat = grad_out_feat.contiguous()
+        grad_out_feat, grad_q = _fp8_grad(ctx, grad_out_feat.contiguous())
         kgen, mode, in_key, out_key, manager = ctx.misc
         grad_in_feat, grad_kernel = _C.ConvolutionTransposeBackwardGPU(
             ctx.input_features, grad_out_feat, ctx.kernel_weights, kgen.kernel_size,
             kgen.kernel_stride, kgen.kernel_dilation, kgen.region_type, kgen.region_offsets,
             mode, in_key, out_key, manager._manager,
             need_in=ctx.needs_input_grad[0], need_w=ctx.needs_input_grad[1], fp8=ctx.fp8,
-            act=ctx.act)
-        return grad_in_feat, grad_kernel, None, None, None, None, None, None, None
+            act=ctx.act, grad_q=grad_q)
+        return grad_in_feat, grad_kernel, None, None, None, None, None, None, None, None
 
 
 class MinkowskiConvolutionBase(MinkowskiModuleBase):
@@ -141,7 +160,7 @@ class MinkowskiConvolutionBase(MinkowskiModuleBase):
                 coordinates: Union[torch.Tensor, CoordinateMapKey, SparseTensor] = None):
         assert isinstance(input, SparseTensor)
         assert input.D == self.dimension
-        observer = selected = None
+        observer = selected = delayed = None
         if self.use_mm:
             out_coordinate_map_key = input.coordinate_map_key
             kernel = self.kernel if self.kernel.dtype == input.F.dtype else self.kernel.to(input.F.dtype)
@@ -159,16 +178,20 @@ class MinkowskiConvolutionBase(MinkowskiModuleBase):
                 selected = _fp8_rule(self, input.F)
                 observer._observe(self, input, selected)
             fp8 = _fp8_train(self, input.F)
+            scaling = _C.fp8_training_scaling() if fp8 else None
+            delayed = None if scaling is None else scaling._conv_begin(self, input)
             outfeat = self.conv.apply(input.F, self.kernel, self.kernel_generator,
                                       self.convolution_mode, input.coordinate_map_key,
                                       out_coordinate_map_key, input._manager, fp8,
-                                      fp8 and _fp8_train_wgrad(self))
+                                      fp8 and _fp8_train_wgrad(self), delayed)
         if self.bias is not None:
             outfeat = outfeat + self.bias.to(outfeat.dtype)
         out = SparseTensor(outfeat, coordinate_map_key=out_coordinate_map_key,
                            coordinate_manager=input._manager)
         if selected:        # in fp8 it runs the e4m3 route, which writes shadows
             observer._tag(self, out)
+        if delayed is not None:     # a training batch norm on `out` writes its e5m2 gradient
+            scaling._tag(out, delayed)
         return out
 
     def reset_parameters(self, is_transpose=False):

@@ -12,7 +12,10 @@
 //   apply      : y = (x - mean) * invstd * w + b                        (optional ReLU)
 //   bwd_reduce : G1[c] = sum_r dy,  G2[c] = sum_r dy * (x - mean) * invstd   (fp64 [2C])
 //   bwd_apply  : dx = (dy - G1/n - xhat * G2/n) * invstd * w
+#include <type_traits>
+
 #include "common.cuh"
+#include "fp8.cuh"
 #include "peer.cuh"
 
 namespace meb200 {
@@ -320,18 +323,22 @@ __global__ void k_bn_finalize(const double *__restrict__ sums, double count,
   }
 }
 
-// MODE 0: y = (x - mean) * invstd * w + b (+ ReLU);  MODE 1: dx from dy (see file header)
-template <typename T, int MODE>
-__global__ void __launch_bounds__(kBnThreads)
-k_bn_apply(const T *__restrict__ a, const T *__restrict__ x, const T *__restrict__ aux,
-           const float *__restrict__ mean, const float *__restrict__ invstd,
-           const float *__restrict__ weight, const float *__restrict__ bias,
-           const double *__restrict__ gsums, double count, const double *__restrict__ d_count,
-           uint32_t n, uint32_t C, uint32_t rows_per_cta, int relu, T *__restrict__ out,
-           T *__restrict__ out2) {
+// MODE 0: y = (x - mean) * invstd * w + b (+ ReLU);  MODE 1: dx from dy (see file header).
+// F (E4M3 / E5M2, with fq): also the fp8 copy of what `out` receives, q = fp8(round_T(v) * inv) as
+// one 8-byte store per thread and row, and max |round_T(v)| over the finite values maxed into
+// fq.amax_slot; void: no copy (fq unused).
+template <typename T, int MODE, typename F>
+__device__ __forceinline__ void
+bn_apply(const T *__restrict__ a, const T *__restrict__ x, const T *__restrict__ aux,
+         const float *__restrict__ mean, const float *__restrict__ invstd,
+         const float *__restrict__ weight, const float *__restrict__ bias,
+         const double *__restrict__ gsums, double count, const double *__restrict__ d_count,
+         uint32_t n, uint32_t C, uint32_t rows_per_cta, int relu, T *__restrict__ out,
+         T *__restrict__ out2, const meb200_fp8_out &fq) {
   // aux: MODE 0 = residual added before the ReLU (may be NULL); MODE 1 = the layer's fused output
   // y whose sign is the ReLU mask (may be NULL).  out2 (MODE 1, may be NULL) = masked dy, the
   // gradient of the residual branch.
+  constexpr bool Q = !std::is_void<F>::value;
   const BnGeom g = bn_geom(C);
   if (threadIdx.x >= g.active) return;
   if (d_count != nullptr) count = *d_count;
@@ -354,6 +361,8 @@ k_bn_apply(const T *__restrict__ a, const T *__restrict__ x, const T *__restrict
       k2[i] = (float)(gsums[C + c] / count);
     }
   }
+  float q_inv = 0.f, q_max = 0.f;
+  if constexpr (Q) q_inv = __ldg(fq.scale + 1);
   constexpr int U = 4;      // rows per iteration, all loads first (see k_bn_reduce)
   const uint32_t step = g.rows_per_pass;
   for (uint32_t r = row_begin + r0; r < row_end; r += U * step) {
@@ -393,8 +402,47 @@ k_bn_apply(const T *__restrict__ a, const T *__restrict__ x, const T *__restrict
         }
       }
       Vec8<T>::store(out + (size_t)ru * C + cg * 8, vo);
+      if constexpr (Q) {
+        uint32_t w[2];
+#pragma unroll
+        for (int i = 0; i < 8; i += 2) {
+          const float r0v = to_f32<T>(from_f32<T>(vo[i])), r1v = to_f32<T>(from_f32<T>(vo[i + 1]));
+          q_max = fmaxf(q_max, fmaxf(finite_abs(r0v), finite_abs(r1v)));
+          const uint32_t b = F::cvt2(__fmul_rn(r0v, q_inv), __fmul_rn(r1v, q_inv));
+          if (i % 4 == 0) w[i / 4] = b; else w[i / 4] |= b << 16;
+        }
+        *reinterpret_cast<uint2 *>(static_cast<uint8_t *>(fq.q) + (size_t)ru * C + cg * 8) =
+            make_uint2(w[0], w[1]);
+      }
     }
   }
+  if constexpr (Q) warp_amax_to(q_max, reinterpret_cast<uint32_t *>(fq.amax_slot));
+}
+
+template <typename T, int MODE>
+__global__ void __launch_bounds__(kBnThreads)
+k_bn_apply(const T *__restrict__ a, const T *__restrict__ x, const T *__restrict__ aux,
+           const float *__restrict__ mean, const float *__restrict__ invstd,
+           const float *__restrict__ weight, const float *__restrict__ bias,
+           const double *__restrict__ gsums, double count, const double *__restrict__ d_count,
+           uint32_t n, uint32_t C, uint32_t rows_per_cta, int relu, T *__restrict__ out,
+           T *__restrict__ out2) {
+  bn_apply<T, MODE, void>(a, x, aux, mean, invstd, weight, bias, gsums, count, d_count, n, C,
+                          rows_per_cta, relu, out, out2, meb200_fp8_out{});
+}
+
+// k_bn_apply writing the fp8 copy of its output: e4m3 of y (MODE 0), e5m2 of dx (MODE 1)
+template <typename T, int MODE>
+__global__ void __launch_bounds__(kBnThreads)
+k_bn_apply_q(const T *__restrict__ a, const T *__restrict__ x, const T *__restrict__ aux,
+             const float *__restrict__ mean, const float *__restrict__ invstd,
+             const float *__restrict__ weight, const float *__restrict__ bias,
+             const double *__restrict__ gsums, double count, const double *__restrict__ d_count,
+             uint32_t n, uint32_t C, uint32_t rows_per_cta, int relu, T *__restrict__ out,
+             T *__restrict__ out2, const meb200_fp8_out fq) {
+  using F = typename std::conditional<MODE == 0, E4M3, E5M2>::type;
+  bn_apply<T, MODE, F>(a, x, aux, mean, invstd, weight, bias, gsums, count, d_count, n, C,
+                       rows_per_cta, relu, out, out2, fq);
 }
 
 static inline uint32_t bn_rows_per_cta(uint32_t n, uint32_t C, unsigned *grid) {
@@ -428,19 +476,47 @@ int meb200_bn_finalize(const double *sums, double count, const double *d_count, 
   return MEB200_OK;
 }
 
-int meb200_bn_apply_fused(const void *x, int dtype, uint32_t n, uint32_t C, const float *mean,
-                          const float *invstd, const float *weight, const float *bias,
-                          const void *residual, int relu, void *y, void *stream_) {
-  cudaStream_t s = (cudaStream_t)stream_;
+// fq: NULL, or the fp8 copy of y (k_bn_apply_q)
+static int bn_apply_forward(const void *x, int dtype, uint32_t n, uint32_t C, const float *mean,
+                            const float *invstd, const float *weight, const float *bias,
+                            const void *residual, int relu, void *y, const meb200_fp8_out *fq,
+                            cudaStream_t s) {
   MEB_BN_CHECK(C);
   if (n == 0) return MEB200_OK;
   unsigned grid;
   uint32_t rows = bn_rows_per_cta(n, C, &grid);
-  MEB_DISPATCH_DTYPE(dtype, k_bn_apply<T, 0><<<grid, kBnThreads, 0, s>>>(
-                                (const T *)x, nullptr, (const T *)residual, mean, invstd, weight,
-                                bias, nullptr, 1.0, nullptr, n, C, rows, relu, (T *)y, nullptr));
+  if (fq == nullptr) {
+    MEB_DISPATCH_DTYPE(dtype, k_bn_apply<T, 0><<<grid, kBnThreads, 0, s>>>(
+                                  (const T *)x, nullptr, (const T *)residual, mean, invstd, weight,
+                                  bias, nullptr, 1.0, nullptr, n, C, rows, relu, (T *)y, nullptr));
+  } else {
+    MEB_DISPATCH_DTYPE(dtype, k_bn_apply_q<T, 0><<<grid, kBnThreads, 0, s>>>(
+                                  (const T *)x, nullptr, (const T *)residual, mean, invstd, weight,
+                                  bias, nullptr, 1.0, nullptr, n, C, rows, relu, (T *)y, nullptr,
+                                  *fq));
+  }
   MEB_LAUNCH_OK();
   return MEB200_OK;
+}
+
+int meb200_bn_apply_fused(const void *x, int dtype, uint32_t n, uint32_t C, const float *mean,
+                          const float *invstd, const float *weight, const float *bias,
+                          const void *residual, int relu, void *y, void *stream_) {
+  return bn_apply_forward(x, dtype, n, C, mean, invstd, weight, bias, residual, relu, y, nullptr,
+                          (cudaStream_t)stream_);
+}
+
+#define MEB_FQ_CHECK()                                                                            \
+  MEB_CHECK_ARG(fq && fq->scale && fq->amax_slot && (n == 0 || (fq->q && aligned(8, fq->q))),     \
+                "fp8 output: null buffer or q not 8-byte aligned")
+
+int meb200_bn_apply_fused_q(const void *x, int dtype, uint32_t n, uint32_t C, const float *mean,
+                            const float *invstd, const float *weight, const float *bias,
+                            const void *residual, int relu, void *y, const meb200_fp8_out *fq,
+                            void *stream_) {
+  MEB_FQ_CHECK();
+  return bn_apply_forward(x, dtype, n, C, mean, invstd, weight, bias, residual, relu, y, fq,
+                          (cudaStream_t)stream_);
 }
 
 static int bn_launch_reduce(int mode, const void *a, const void *x, const void *ymask, int dtype,
@@ -473,12 +549,11 @@ static inline uint32_t *bn_ticket(void *workspace) {
   return reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(workspace) + kBnPartialBytes);
 }
 
-int meb200_bn_forward_train(const void *x, int dtype, uint32_t n, uint32_t C, const float *weight,
+static int bn_forward_train(const void *x, int dtype, uint32_t n, uint32_t C, const float *weight,
                             const float *bias, const void *residual, int relu, float eps,
                             float momentum, float *running_mean, float *running_var,
                             long long *num_batches_tracked, void *workspace, float *mean,
-                            float *invstd, void *y, void *stream_) {
-  cudaStream_t s = (cudaStream_t)stream_;
+                            float *invstd, void *y, const meb200_fp8_out *fq, cudaStream_t s) {
   MEB_BN_CHECK(C);
   MEB_CHECK_ARG(n > 0 && workspace && mean && invstd && y, "bn forward: empty input / null buffer");
   BnTail tail{};
@@ -489,7 +564,29 @@ int meb200_bn_forward_train(const void *x, int dtype, uint32_t n, uint32_t C, co
   int rc = bn_launch_reduce(0, x, nullptr, nullptr, dtype, n, C, nullptr, nullptr,
                             (double *)workspace, tail, s);
   if (rc != MEB200_OK) return rc;
-  return meb200_bn_apply_fused(x, dtype, n, C, mean, invstd, weight, bias, residual, relu, y, stream_);
+  return bn_apply_forward(x, dtype, n, C, mean, invstd, weight, bias, residual, relu, y, fq, s);
+}
+
+int meb200_bn_forward_train(const void *x, int dtype, uint32_t n, uint32_t C, const float *weight,
+                            const float *bias, const void *residual, int relu, float eps,
+                            float momentum, float *running_mean, float *running_var,
+                            long long *num_batches_tracked, void *workspace, float *mean,
+                            float *invstd, void *y, void *stream_) {
+  return bn_forward_train(x, dtype, n, C, weight, bias, residual, relu, eps, momentum, running_mean,
+                          running_var, num_batches_tracked, workspace, mean, invstd, y, nullptr,
+                          (cudaStream_t)stream_);
+}
+
+int meb200_bn_forward_train_q(const void *x, int dtype, uint32_t n, uint32_t C,
+                              const float *weight, const float *bias, const void *residual,
+                              int relu, float eps, float momentum, float *running_mean,
+                              float *running_var, long long *num_batches_tracked, void *workspace,
+                              float *mean, float *invstd, void *y, const meb200_fp8_out *fq,
+                              void *stream_) {
+  MEB_FQ_CHECK();
+  return bn_forward_train(x, dtype, n, C, weight, bias, residual, relu, eps, momentum, running_mean,
+                          running_var, num_batches_tracked, workspace, mean, invstd, y, fq,
+                          (cudaStream_t)stream_);
 }
 
 int meb200_bn_stats_to(const void *x, int dtype, uint32_t n, uint32_t C, void *workspace,
@@ -541,15 +638,14 @@ static void bn_tail_peer(BnTail &tail, const void *peer_bases_dev, uint64_t slot
                 "peer exchange: bases / rank %u of %u / slot offset / sequence number",          \
                 (unsigned)rank, (unsigned)world)
 
-int meb200_bn_forward_train_peer(const void *x, int dtype, uint32_t n, uint32_t C,
+static int bn_forward_train_peer(const void *x, int dtype, uint32_t n, uint32_t C,
                                  const float *weight, const float *bias, const void *residual,
                                  int relu, float eps, float momentum, float *running_mean,
                                  float *running_var, long long *num_batches_tracked,
                                  void *workspace, const void *peer_bases_dev,
                                  uint64_t slot_offset_bytes, uint32_t seq, uint32_t rank,
                                  uint32_t world, float *mean, float *invstd, double *total_rows,
-                                 void *y, void *stream_) {
-  cudaStream_t s = (cudaStream_t)stream_;
+                                 void *y, const meb200_fp8_out *fq, cudaStream_t s) {
   MEB_BN_CHECK(C);
   MEB_CHECK_ARG(workspace && mean && invstd && total_rows && (y || n == 0), "bn forward: null buffer");
   MEB_PEER_CHECK();
@@ -563,7 +659,36 @@ int meb200_bn_forward_train_peer(const void *x, int dtype, uint32_t n, uint32_t 
   int rc = bn_launch_reduce(0, x, nullptr, nullptr, dtype, n, C, nullptr, nullptr,
                             (double *)workspace, tail, s);
   if (rc != MEB200_OK || n == 0) return rc;
-  return meb200_bn_apply_fused(x, dtype, n, C, mean, invstd, weight, bias, residual, relu, y, stream_);
+  return bn_apply_forward(x, dtype, n, C, mean, invstd, weight, bias, residual, relu, y, fq, s);
+}
+
+int meb200_bn_forward_train_peer(const void *x, int dtype, uint32_t n, uint32_t C,
+                                 const float *weight, const float *bias, const void *residual,
+                                 int relu, float eps, float momentum, float *running_mean,
+                                 float *running_var, long long *num_batches_tracked,
+                                 void *workspace, const void *peer_bases_dev,
+                                 uint64_t slot_offset_bytes, uint32_t seq, uint32_t rank,
+                                 uint32_t world, float *mean, float *invstd, double *total_rows,
+                                 void *y, void *stream_) {
+  return bn_forward_train_peer(x, dtype, n, C, weight, bias, residual, relu, eps, momentum,
+                               running_mean, running_var, num_batches_tracked, workspace,
+                               peer_bases_dev, slot_offset_bytes, seq, rank, world, mean, invstd,
+                               total_rows, y, nullptr, (cudaStream_t)stream_);
+}
+
+int meb200_bn_forward_train_peer_q(const void *x, int dtype, uint32_t n, uint32_t C,
+                                   const float *weight, const float *bias, const void *residual,
+                                   int relu, float eps, float momentum, float *running_mean,
+                                   float *running_var, long long *num_batches_tracked,
+                                   void *workspace, const void *peer_bases_dev,
+                                   uint64_t slot_offset_bytes, uint32_t seq, uint32_t rank,
+                                   uint32_t world, float *mean, float *invstd, double *total_rows,
+                                   void *y, const meb200_fp8_out *fq, void *stream_) {
+  MEB_FQ_CHECK();
+  return bn_forward_train_peer(x, dtype, n, C, weight, bias, residual, relu, eps, momentum,
+                               running_mean, running_var, num_batches_tracked, workspace,
+                               peer_bases_dev, slot_offset_bytes, seq, rank, world, mean, invstd,
+                               total_rows, y, fq, (cudaStream_t)stream_);
 }
 
 int meb200_bn_backward_reduce_peer(const void *dy, const void *x, const void *y_mask, int dtype,
@@ -585,23 +710,48 @@ int meb200_bn_backward_reduce_peer(const void *dy, const void *x, const void *y_
   return bn_launch_reduce(1, dy, x, y_mask, dtype, n, C, mean, invstd, (double *)workspace, tail, s);
 }
 
-int meb200_bn_backward_apply_fused(const void *dy, const void *x, const void *y_mask, int dtype,
-                                   uint32_t n, uint32_t C, const float *mean, const float *invstd,
-                                   const float *weight, const double *sums, double count,
-                                   const double *d_count, void *dx, void *d_residual,
-                                   void *stream_) {
-  cudaStream_t s = (cudaStream_t)stream_;
+static int bn_backward_apply(const void *dy, const void *x, const void *y_mask, int dtype,
+                             uint32_t n, uint32_t C, const float *mean, const float *invstd,
+                             const float *weight, const double *sums, double count,
+                             const double *d_count, void *dx, void *d_residual,
+                             const meb200_fp8_out *fq, cudaStream_t s) {
   MEB_BN_CHECK(C);
   if (n == 0) return MEB200_OK;
   MEB_CHECK_ARG(count > 0 || d_count != nullptr, "count");
   unsigned grid;
   uint32_t rows = bn_rows_per_cta(n, C, &grid);
-  MEB_DISPATCH_DTYPE(dtype, k_bn_apply<T, 1><<<grid, kBnThreads, 0, s>>>(
-                                (const T *)dy, (const T *)x, (const T *)y_mask, mean, invstd,
-                                weight, nullptr, sums, count, d_count, n, C, rows, 0, (T *)dx,
-                                (T *)d_residual));
+  if (fq == nullptr) {
+    MEB_DISPATCH_DTYPE(dtype, k_bn_apply<T, 1><<<grid, kBnThreads, 0, s>>>(
+                                  (const T *)dy, (const T *)x, (const T *)y_mask, mean, invstd,
+                                  weight, nullptr, sums, count, d_count, n, C, rows, 0, (T *)dx,
+                                  (T *)d_residual));
+  } else {
+    MEB_DISPATCH_DTYPE(dtype, k_bn_apply_q<T, 1><<<grid, kBnThreads, 0, s>>>(
+                                  (const T *)dy, (const T *)x, (const T *)y_mask, mean, invstd,
+                                  weight, nullptr, sums, count, d_count, n, C, rows, 0, (T *)dx,
+                                  (T *)d_residual, *fq));
+  }
   MEB_LAUNCH_OK();
   return MEB200_OK;
+}
+
+int meb200_bn_backward_apply_fused(const void *dy, const void *x, const void *y_mask, int dtype,
+                                   uint32_t n, uint32_t C, const float *mean, const float *invstd,
+                                   const float *weight, const double *sums, double count,
+                                   const double *d_count, void *dx, void *d_residual,
+                                   void *stream_) {
+  return bn_backward_apply(dy, x, y_mask, dtype, n, C, mean, invstd, weight, sums, count, d_count,
+                           dx, d_residual, nullptr, (cudaStream_t)stream_);
+}
+
+int meb200_bn_backward_apply_fused_q(const void *dy, const void *x, const void *y_mask, int dtype,
+                                     uint32_t n, uint32_t C, const float *mean,
+                                     const float *invstd, const float *weight, const double *sums,
+                                     double count, const double *d_count, void *dx,
+                                     void *d_residual, const meb200_fp8_out *fq, void *stream_) {
+  MEB_FQ_CHECK();
+  return bn_backward_apply(dy, x, y_mask, dtype, n, C, mean, invstd, weight, sums, count, d_count,
+                           dx, d_residual, fq, (cudaStream_t)stream_);
 }
 
 }

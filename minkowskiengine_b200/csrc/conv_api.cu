@@ -230,6 +230,25 @@ int meb200_quantize_e4m3_static(const void *in, int dtype, uint32_t n, uint32_t 
                               (cudaStream_t)stream_);
 }
 
+int meb200_quantize_fp8_record(const void *in, int dtype, uint32_t n, uint32_t c, int format,
+                               const meb200_fp8_out *out, void *stream_) {
+  MEB_CHECK_ARG(dtype >= 0 && dtype <= 2, "dtype");
+  MEB_CHECK_ARG(format == MEB200_FP8_E4M3 || format == MEB200_FP8_E5M2, "fp8 format %d", format);
+  MEB_CHECK_ARG(out && out->scale && out->amax_slot && ((in && out->q) || (uint64_t)n * c == 0),
+                "null buffer");
+  return quantize_record(in, dtype, (uint64_t)n * c, format, out->q, out->scale, out->amax_slot,
+                         (cudaStream_t)stream_);
+}
+
+int meb200_fp8_roll(const float *cur, float *hist, uint32_t n_e4m3, uint32_t n_e5m2, uint32_t H,
+                    int margin, float *next_cur, float *scales, void *stream_) {
+  MEB_CHECK_ARG(H >= 1 && H <= MEB200_FP8_MAX_HISTORY, "history length %u outside [1, %d]",
+                (unsigned)H, MEB200_FP8_MAX_HISTORY);
+  MEB_CHECK_ARG(margin >= 0 && margin <= 127, "margin %d outside [0, 127]", margin);
+  MEB_CHECK_ARG(n_e4m3 + n_e5m2 == 0 || (cur && hist && next_cur && scales), "null buffer");
+  return fp8_roll(cur, hist, n_e4m3, n_e5m2, H, margin, next_cur, scales, (cudaStream_t)stream_);
+}
+
 static bool packed_dtype(int dtype) {
   return dtype == MEB200_BF16 || dtype == MEB200_F16 || dtype == MEB200_TF32;
 }

@@ -60,6 +60,11 @@ int amax_accumulate(const void *in, int dtype, uint64_t count, float *amax, cuda
 int e4m3_scales_from_amax(const float *amax, float *scale, cudaStream_t stream);
 int quantize_e4m3_static(const void *in, int dtype, uint64_t count, void *out, const float *scale,
                          cudaStream_t stream);
+// Delayed scaling (meb200_quantize_fp8_record, meb200_fp8_roll).
+int quantize_record(const void *in, int dtype, uint64_t count, int format, void *out,
+                    const float *scale, float *slot, cudaStream_t stream);
+int fp8_roll(const float *cur, float *hist, uint32_t n_e4m3, uint32_t n_e5m2, uint32_t H,
+             int margin, float *next_cur, float *scales, cudaStream_t stream);
 
 // fp32 W[K,c_in,c_out] -> w_cast [K,c_in,c_out] and w_t [K,c_out,c_in] in bf16/fp16, or in fp32
 // words rounded to tf32 (MEB200_TF32).

@@ -18,51 +18,26 @@
 
 #include "common.cuh"
 #include "conv_tc.cuh"
-#include "ptx.cuh"
+#include "fp8.cuh"
 
 namespace meb200 {
 
 constexpr uint32_t kQThreads = 256;
 constexpr uint32_t kQMaxCtas = 1024;
 
-// The two fp8 formats: the largest finite value, and the saturating conversion of a pair (lo = a)
-struct E4M3 {
-  static constexpr float kMax = 448.f;
-  static __device__ __forceinline__ uint16_t cvt2(float a, float b) {
-    return ptx::e4m3x2_satfinite(a, b);
-  }
-};
-struct E5M2 {
-  static constexpr float kMax = 57344.f;
-  static __device__ __forceinline__ uint16_t cvt2(float a, float b) {
-    return ptx::e5m2x2_satfinite(a, b);
-  }
-};
-
-// scale and inv of a tensor (or column) whose finite values have the maximum magnitude amax
-template <typename F>
-__device__ __forceinline__ void fp8_scales(float amax, float &scale, float &inv) {
-  if (amax == 0.f) {
-    scale = inv = 1.f;
-  } else if (isinf(inv = __fdiv_rn(F::kMax, amax))) {
-    inv = FLT_MAX;
-    scale = __fdiv_rn(1.f, FLT_MAX);
-  } else {
-    scale = __fdiv_rn(amax, F::kMax);
-  }
+// The max of every thread's m over the CTA, valid in thread 0 (the other threads return false).
+__device__ __forceinline__ bool cta_max(float m, float &m_out) {
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, d));
+  __shared__ float wm[kQThreads / 32];
+  if ((threadIdx.x & 31) == 0) wm[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x != 0) return false;
+  for (uint32_t w = 1; w < kQThreads / 32; ++w) m = fmaxf(m, wm[w]);
+  m_out = m;
+  return true;
 }
 
-__device__ __forceinline__ float finite_abs(float v) { return isfinite(v) ? fabsf(v) : 0.f; }
-
-template <typename F>
-__device__ __forceinline__ uint8_t fp8_byte(float x, float inv) {
-  return (uint8_t)(F::cvt2(__fmul_rn(x, inv), 0.f) & 0xFFu);
-}
-
-// Launch 1: per-CTA max of |x| over the finite values, combined with an atomic max on the fp32 bits
-// (non-negative floats order as their bit patterns).  The last CTA to finish writes scale[0] = scale,
-// scale[1] = inv and leaves the workspace zero again.  ws: [0] amax bits, [1] CTAs done (a ticket
-// that wraps to 0 at the last CTA).
 // The CTA's max, valid in thread 0 (the other threads return false).
 template <typename T, bool VEC>
 __device__ __forceinline__ bool cta_amax(const T *__restrict__ x, uint64_t count, float &m_out) {
@@ -78,17 +53,13 @@ __device__ __forceinline__ bool cta_amax(const T *__restrict__ x, uint64_t count
   if (blockIdx.x == 0)                                    // elements past the last vector
     for (uint64_t i = n_vec * V + threadIdx.x; i < count; i += blockDim.x)
       m = fmaxf(m, finite_abs(to_f32<T>(x[i])));
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, d));
-  __shared__ float wm[kQThreads / 32];
-  if ((threadIdx.x & 31) == 0) wm[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x != 0) return false;
-  for (uint32_t w = 1; w < kQThreads / 32; ++w) m = fmaxf(m, wm[w]);
-  m_out = m;
-  return true;
+  return cta_max(m, m_out);
 }
 
+// Launch 1: per-CTA max of |x| over the finite values, combined with an atomic max on the fp32 bits
+// (non-negative floats order as their bit patterns).  The last CTA to finish writes scale[0] = scale,
+// scale[1] = inv and leaves the workspace zero again.  ws: [0] amax bits, [1] CTAs done (a ticket
+// that wraps to 0 at the last CTA).
 template <typename T, bool VEC, typename F>
 __global__ void __launch_bounds__(kQThreads) k_amax(const T *__restrict__ x, uint64_t count,
                                                    float *__restrict__ scale, uint32_t *ws) {
@@ -104,12 +75,12 @@ __global__ void __launch_bounds__(kQThreads) k_amax(const T *__restrict__ x, uin
   scale[1] = inv;
 }
 
-// Launch 2: q = fp8(x * inv), 16 elements (16 output bytes) per thread and step.
-template <typename T, bool VEC, typename F>
-__global__ void __launch_bounds__(kQThreads) k_quant(const T *__restrict__ x, uint64_t count,
-                                                    const float *__restrict__ scale,
-                                                    uint8_t *__restrict__ q) {
-  const float inv = __ldg(scale + 1);
+// Launch 2: q = fp8(x * inv), 16 elements (16 output bytes) per thread and step.  RECORD: also
+// returns the thread's max |x| over the finite values it converted (else 0, computed by nothing).
+template <typename T, bool VEC, typename F, bool RECORD>
+__device__ __forceinline__ float quant_body(const T *__restrict__ x, uint64_t count, float inv,
+                                            uint8_t *__restrict__ q) {
+  float m = 0.f;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   if constexpr (VEC) {
     constexpr uint32_t V = 16 / sizeof(T);
@@ -125,17 +96,45 @@ __global__ void __launch_bounds__(kQThreads) k_quant(const T *__restrict__ x, ui
           const uint32_t e = h * V + j;           // element of the 16: byte e of the store
           const uint32_t b = F::cvt2(__fmul_rn(f[j], inv), __fmul_rn(f[j + 1], inv));
           if (e % 4 == 0) w[e / 4] = b; else w[e / 4] |= b << 16;
+          if (RECORD) m = fmaxf(m, fmaxf(finite_abs(f[j]), finite_abs(f[j + 1])));
         }
       }
       *reinterpret_cast<uint4 *>(q + i * 16) = make_uint4(w[0], w[1], w[2], w[3]);
     }
     if (blockIdx.x == 0)
-      for (uint64_t i = n16 * 16 + threadIdx.x; i < count; i += blockDim.x)
-        q[i] = fp8_byte<F>(to_f32<T>(x[i]), inv);
+      for (uint64_t i = n16 * 16 + threadIdx.x; i < count; i += blockDim.x) {
+        const float v = to_f32<T>(x[i]);
+        q[i] = fp8_byte<F>(v, inv);
+        if (RECORD) m = fmaxf(m, finite_abs(v));
+      }
   } else {
-    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count; i += stride)
-      q[i] = fp8_byte<F>(to_f32<T>(x[i]), inv);
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count; i += stride) {
+      const float v = to_f32<T>(x[i]);
+      q[i] = fp8_byte<F>(v, inv);
+      if (RECORD) m = fmaxf(m, finite_abs(v));
+    }
   }
+  return m;
+}
+
+template <typename T, bool VEC, typename F>
+__global__ void __launch_bounds__(kQThreads) k_quant(const T *__restrict__ x, uint64_t count,
+                                                    const float *__restrict__ scale,
+                                                    uint8_t *__restrict__ q) {
+  quant_body<T, VEC, F, false>(x, count, __ldg(scale + 1), q);
+}
+
+// Convert and record (delayed scaling): k_quant at the given scale, and the CTA's max |x| over the
+// finite values atomically maxed into *slot (fp32 bits), in the same pass.
+template <typename T, bool VEC, typename F>
+__global__ void __launch_bounds__(kQThreads) k_quant_record(const T *__restrict__ x,
+                                                           uint64_t count,
+                                                           const float *__restrict__ scale,
+                                                           uint8_t *__restrict__ q,
+                                                           uint32_t *slot) {
+  float m;
+  if (cta_max(quant_body<T, VEC, F, true>(x, count, __ldg(scale + 1), q), m))
+    atomicMax(slot, __float_as_uint(m));
 }
 
 uint64_t quantize_e4m3_workspace_bytes() { return 16; }
@@ -225,6 +224,68 @@ int quantize_e4m3_static(const void *in, int dtype, uint64_t count, void *out, c
     else k_quant<T, false, E4M3><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q);
     MEB_LAUNCH_OK();
   });
+  return MEB200_OK;
+}
+
+// ---- delayed scaling --------------------------------------------------------------------------
+template <typename F>
+static int quantize_record_as(const void *in, int dtype, uint64_t count, void *out,
+                              const float *scale, float *slot, cudaStream_t stream) {
+  const uint32_t ctas = quant_ctas(count);
+  uint8_t *q = reinterpret_cast<uint8_t *>(out);
+  uint32_t *a = reinterpret_cast<uint32_t *>(slot);
+  MEB_DISPATCH_DTYPE(dtype, {
+    const T *x = reinterpret_cast<const T *>(in);
+    if (aligned(16, in, out))
+      k_quant_record<T, true, F><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q, a);
+    else
+      k_quant_record<T, false, F><<<ctas, kQThreads, 0, stream>>>(x, count, scale, q, a);
+    MEB_LAUNCH_OK();
+  });
+  return MEB200_OK;
+}
+
+int quantize_record(const void *in, int dtype, uint64_t count, int format, void *out,
+                    const float *scale, float *slot, cudaStream_t stream) {
+  if (count == 0) return MEB200_OK;
+  return format == MEB200_FP8_E5M2
+             ? quantize_record_as<E5M2>(in, dtype, count, out, scale, slot, stream)
+             : quantize_record_as<E4M3>(in, dtype, count, out, scale, slot, stream);
+}
+
+// One thread per entry: history [L, H] (newest first) takes the step's slot in front and drops its
+// oldest value, amax = the max of the new history, (scale, inv) = fp8_scales(min(amax * 2^margin,
+// FLT_MAX)) in the entry's format (e4m3 below n_e4m3, e5m2 from there), next_cur = 0.
+__global__ void __launch_bounds__(128) k_fp8_roll(const float *__restrict__ cur,
+                                                  float *__restrict__ hist, uint32_t n_e4m3,
+                                                  uint32_t L, uint32_t H, int margin,
+                                                  float *__restrict__ next_cur,
+                                                  float *__restrict__ scales) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= L) return;
+  float *h = hist + (size_t)i * H;
+  float v = cur[i], amax = 0.f;
+  for (uint32_t k = 0; k < H; ++k) {
+    const float older = h[k];
+    h[k] = v;
+    amax = fmaxf(amax, v);
+    v = older;
+  }
+  const float a = fminf(ldexpf(amax, margin), FLT_MAX);
+  float s, inv;
+  if (i < n_e4m3) fp8_scales<E4M3>(a, s, inv);
+  else fp8_scales<E5M2>(a, s, inv);
+  scales[2 * (size_t)i] = s;
+  scales[2 * (size_t)i + 1] = inv;
+  next_cur[i] = 0.f;
+}
+
+int fp8_roll(const float *cur, float *hist, uint32_t n_e4m3, uint32_t n_e5m2, uint32_t H,
+             int margin, float *next_cur, float *scales, cudaStream_t stream) {
+  const uint32_t L = n_e4m3 + n_e5m2;
+  if (L == 0) return MEB200_OK;
+  k_fp8_roll<<<cdiv(L, 128u), 128, 0, stream>>>(cur, hist, n_e4m3, L, H, margin, next_cur, scales);
+  MEB_LAUNCH_OK();
   return MEB200_OK;
 }
 

@@ -19,6 +19,15 @@ _SHADOW = "_fp8_shadow"        # SparseTensor attribute: (q, scale, features, fe
 _PRODUCER = "_fp8_producer"    # SparseTensor attribute while observing: (calibration, name)
 
 
+def module_names(model):
+    """{id(module): qualified name} of every module of `model` (a module reached twice keeps its
+    first name): how the fp8 recipes bind to a model's layers."""
+    names = {}
+    for name, m in model.named_modules():
+        names.setdefault(id(m), name)
+    return names
+
+
 class Fp8Calibration:
     """Static e4m3 scales for the convolutions of `model`, keyed by their qualified module names.
 
@@ -38,9 +47,7 @@ class Fp8Calibration:
     consumers it fed."""
 
     def __init__(self, model):
-        self._names = {}
-        for name, m in model.named_modules():
-            self._names.setdefault(id(m), name)
+        self._names = module_names(model)
         self._amax = {}          # consumer name -> fp32 [1] amax (on the device it was observed on)
         self._feeds = {}         # producer name -> set of consumer names
         self._scales = {}        # (kind, name, device) -> fp32 [2] (scale, inv) on the device

@@ -16,12 +16,14 @@ what a local one does.
 `MEB200_SYNCBN_PEER=0` (or symmetric memory being unavailable) selects NCCL all-reduces.
 """
 import contextlib
+import ctypes
 import os
 
 import torch
 import torch.nn as nn
 
 from . import _lib
+from .backend import fp8_out as _fp8_out
 from .sparse_tensor import SparseTensor
 from .tensor_field import same_kind as _same_kind
 
@@ -113,7 +115,10 @@ class _BatchNormFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, bias, running_mean, running_var, momentum, eps, group, relu,
-                residual, use_running, num_batches_tracked=None):
+                residual, use_running, num_batches_tracked=None, fp8=None):
+        """fp8 (training only): a fp8_delayed._BnStep, whose y_out = (q, scale, slot) the apply
+        pass writes the e4m3 copy of y into and whose grad entry the backward writes the e5m2 copy
+        of dx for (each may be None)."""
         lib = _lib.load()
         x = x.contiguous()
         n, C = x.shape
@@ -138,9 +143,17 @@ class _BatchNormFunction(torch.autograd.Function):
             peer = None
             if not use_running and group is not None and _USE_PEER:
                 peer = _PeerExchange.get(group, dev)
+            fq = None if fp8 is None or fp8.y_out is None or n == 0 else _fp8_out(*fp8.y_out)
+
+            def call(name, *args):
+                """Entry `name`, or with fq its _q twin (the same arguments, fq before the
+                stream)."""
+                if fq is None:
+                    return getattr(lib, name)(*args)
+                return getattr(lib, name + "_q")(*args[:-1], ctypes.byref(fq), args[-1])
             if not use_running and group is None and n > 0:
                 # statistics + finalize in one launch, then the apply pass
-                _lib.check(lib.meb200_bn_forward_train(
+                _lib.check(call("meb200_bn_forward_train",
                     _lib.ptr(x), code, n, C, _lib.ptr(w32), _lib.ptr(b32), _lib.ptr(residual),
                     1 if relu else 0, float(eps), float(momentum), _lib.ptr(running_mean),
                     _lib.ptr(running_var), _lib.ptr(num_batches_tracked), _lib.ptr(ws),
@@ -151,7 +164,7 @@ class _BatchNormFunction(torch.autograd.Function):
                 # with the other ranks over NVLink peer memory before it finalizes
                 off = peer.next_slot_offset(2 * C + 1)
                 d_count = torch.empty(1, dtype=torch.float64, device=dev)
-                _lib.check(lib.meb200_bn_forward_train_peer(
+                _lib.check(call("meb200_bn_forward_train_peer",
                     _lib.ptr(x), code, n, C, _lib.ptr(w32), _lib.ptr(b32), _lib.ptr(residual),
                     1 if relu else 0, float(eps), float(momentum), _lib.ptr(running_mean),
                     _lib.ptr(running_var), _lib.ptr(num_batches_tracked), _lib.ptr(ws),
@@ -171,9 +184,11 @@ class _BatchNormFunction(torch.autograd.Function):
                         _lib.ptr(sums), float(max(n, 1)), _lib.ptr(d_count), C, float(eps),
                         float(momentum), _lib.ptr(running_mean), _lib.ptr(running_var),
                         _lib.ptr(mean), _lib.ptr(invstd), stream))
-                _lib.check(lib.meb200_bn_apply_fused(
+                _lib.check(call("meb200_bn_apply_fused",
                     _lib.ptr(x), code, n, C, _lib.ptr(mean), _lib.ptr(invstd), _lib.ptr(w32),
                     _lib.ptr(b32), _lib.ptr(residual), 1 if relu else 0, _lib.ptr(y), stream))
+            if fp8 is not None:
+                fp8.written = not use_running
         if num_batches_tracked is not None and not use_running:
             num_batches_tracked.add_(1)        # paths whose kernels do not count the batch themselves
         ctx.save_for_backward(x, mean, invstd, w32 if w32 is not None else mean.new_empty(0),
@@ -183,6 +198,7 @@ class _BatchNormFunction(torch.autograd.Function):
         ctx.has_affine = weight is not None
         ctx.param_dtype = None if weight is None else weight.dtype
         ctx.relu, ctx.has_residual, ctx.use_running = bool(relu), residual is not None, use_running
+        ctx.grad_entry = None if fp8 is None or use_running else fp8.grad
         return y
 
     @staticmethod
@@ -228,12 +244,20 @@ class _BatchNormFunction(torch.autograd.Function):
                 torch.distributed.all_reduce(gs, group=group)
             dx = torch.empty_like(x)
             dres = torch.empty_like(x) if ctx.has_residual else None
-            _lib.check(lib.meb200_bn_backward_apply_fused(
-                _lib.ptr(dy), _lib.ptr(x), _lib.ptr(ymask), code, n, C, _lib.ptr(mean),
-                _lib.ptr(invstd), _lib.ptr(w32) if w32.numel() else None, _lib.ptr(gs),
-                float(max(n, 1)), _lib.ptr(d_count) if d_count.numel() else None, _lib.ptr(dx),
-                _lib.ptr(dres), stream))
-        return dx, grad_w, grad_b, None, None, None, None, None, None, dres, None, None
+            args = (_lib.ptr(dy), _lib.ptr(x), _lib.ptr(ymask), code, n, C, _lib.ptr(mean),
+                    _lib.ptr(invstd), _lib.ptr(w32) if w32.numel() else None, _lib.ptr(gs),
+                    float(max(n, 1)), _lib.ptr(d_count) if d_count.numel() else None, _lib.ptr(dx),
+                    _lib.ptr(dres))
+            g = ctx.grad_entry
+            if g is None or n == 0:
+                _lib.check(lib.meb200_bn_backward_apply_fused(*args, stream))
+            else:
+                # the e5m2 copy of dx for the backward of the convolution that produced x
+                q = torch.empty(x.shape, dtype=torch.uint8, device=x.device)
+                fq = _fp8_out(q, g.scale, g.slot)
+                _lib.check(lib.meb200_bn_backward_apply_fused_q(*args, ctypes.byref(fq), stream))
+                g.shadow = (q, dx.data_ptr(), dx.shape, dx._version)
+        return dx, grad_w, grad_b, None, None, None, None, None, None, dres, None, None, None
 
 
 def _native_ok(bn, x):
@@ -249,8 +273,9 @@ def _native_ok(bn, x):
             and buf_ok(bn.running_mean) and buf_ok(bn.running_var))
 
 
-def _batch_norm(bn, x, group=None, relu=False, residual=None):
-    """Functional core shared by the modules and fused_bn_relu."""
+def _batch_norm(bn, x, group=None, relu=False, residual=None, fp8=None):
+    """Functional core shared by the modules and fused_bn_relu.  fp8: the delayed-scaling outputs
+    of a training batch norm (_BatchNormFunction), written only by the native training pass."""
     if not _native_ok(bn, x) or (residual is not None and (residual.shape != x.shape
                                                            or residual.dtype != x.dtype)):
         y = bn(x)
@@ -265,7 +290,8 @@ def _batch_norm(bn, x, group=None, relu=False, residual=None):
             nbt.add_(1)
             nbt = None
         return _BatchNormFunction.apply(x, bn.weight, bn.bias, bn.running_mean, bn.running_var,
-                                        bn.momentum, bn.eps, group, relu, residual, False, nbt)
+                                        bn.momentum, bn.eps, group, relu, residual, False, nbt,
+                                        fp8)
     return _BatchNormFunction.apply(x, bn.weight, bn.bias, bn.running_mean, bn.running_var,
                                     bn.momentum, bn.eps, None, relu, residual, True)
 
@@ -286,9 +312,27 @@ def _bn_tail(norm, input, residual, relu):
         assert residual.coordinate_map_key == input.coordinate_map_key, \
             "residual and input must live on the same coordinate map"
         res = residual.F
-    out = _batch_norm(bn, input.F, group, relu=relu, residual=res)
-    return SparseTensor(out, coordinate_map_key=input.coordinate_map_key,
-                        coordinate_manager=input.coordinate_manager)
+    fp8 = _fp8_begin(norm, input)
+    out = _batch_norm(bn, input.F, group, relu=relu, residual=res, fp8=fp8)
+    return _fp8_end(fp8, SparseTensor(out, coordinate_map_key=input.coordinate_map_key,
+                                      coordinate_manager=input.coordinate_manager))
+
+
+def _fp8_begin(norm, input):
+    """The delayed-scaling fp8 outputs of a training batch norm on `input` inside
+    fp8_training(scaling=...) (fp8_delayed.Fp8DelayedScaling._bn_begin), or None."""
+    if not norm.bn.training:
+        return None
+    from . import backend as _C
+    scaling = _C.fp8_training_scaling()
+    return None if scaling is None else scaling._bn_begin(norm, input)
+
+
+def _fp8_end(fp8, out):
+    """`out`, with the producer tag and the shadow of the fp8 outputs (if any)."""
+    if fp8 is not None:
+        fp8.recipe._bn_end(fp8, out)
+    return out
 
 
 def _eval_scale_shift(bn, conv_bias=None):
@@ -313,8 +357,9 @@ class MinkowskiBatchNorm(nn.Module):
                                        track_running_stats=track_running_stats)
 
     def forward(self, input):
-        output = _batch_norm(self.bn, input.F)
-        return _same_kind(input, output)
+        fp8 = _fp8_begin(self, input)
+        output = _batch_norm(self.bn, input.F, fp8=fp8)
+        return _fp8_end(fp8, _same_kind(input, output))
 
     def __repr__(self):
         s = "({}, eps={}, momentum={}, affine={}, track_running_stats={})".format(
@@ -341,8 +386,9 @@ class MinkowskiSyncBatchNorm(MinkowskiBatchNorm):
         return None
 
     def forward(self, input):
-        output = _batch_norm(self.bn, input.F, self._group())
-        return _same_kind(input, output)
+        fp8 = _fp8_begin(self, input)
+        output = _batch_norm(self.bn, input.F, self._group(), fp8=fp8)
+        return _fp8_end(fp8, _same_kind(input, output))
 
     @classmethod
     def convert_sync_batchnorm(cls, module, process_group=None):
